@@ -7,7 +7,12 @@
 One "step" = one pass of the hot path over one batch of synthetic 48 kHz PCM already resident in HBM:
 65 536 mono frames of N=2048 per GPU, laid out as 4096 independent streams x 16 consecutive frames (hop = N)
 so that the EMA recurrence state stays on-chip between frames (DESIGN.md §Measurement).  Inputs (512 MiB)
-and outputs (256 MiB) are each larger than the 126 MB L2, so every step streams from/to HBM.
+and outputs (256 MiB) are each larger than the H100's 50 MB L2, so every step streams from/to HBM.
+
+  --dump-outputs DIR   after the timed steps, writes what the last timed step computed (the dB spectra a caller of
+                       the timed path receives) for a fixed, seeded sample of streams as DIR/db.npy (float32,
+                       [streams, frames, 1, bins]) with the sampled stream indices as DIR/streams.npy (float64); the
+                       inputs depend only on the arguments, so two builds can be compared output for output.
 
 Besides the contract's keys the line carries (DESIGN.md §5):
   parity            the measured launch (same engine geometry, fresh state) against the reference's generic CPU path on a
@@ -64,7 +69,7 @@ def load_peaks():
             return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback: H100 SXM data-sheet HBM3 bandwidth"
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -260,8 +265,9 @@ def parity_subset(torch, device, pcm, S, T):
     torch.cuda.synchronize()
     kernel = eng.last_kernel_name()
     n_first = max(1, min(S, -(-256 // T)))
-    pick = sorted(set(range(n_first)) | {S - 1, S - 2, S // 2, S // 3, 147 % S, 148 % S, (148 * 16) % S, (148 * 16 + 147) % S,
-                                         (148 * 27) % S} | set(range(0, S, max(1, S // 40))))
+    sms = torch.cuda.get_device_properties(device).multi_processor_count  # stream s -> CTA s % sms of the N=2048 kernel
+    pick = sorted(set(range(n_first)) | {S - 1, S - 2, S // 2, S // 3, (sms - 1) % S, sms % S, (sms * 16) % S,
+                                         (sms * 16 + sms - 1) % S, (sms * 27) % S} | set(range(0, S, max(1, S // 40))))
     idx = torch.tensor(pick, device=device)
     got = out["db"][idx].cpu().numpy()
     got_sil = out["silent"][idx].cpu().numpy()
@@ -364,6 +370,22 @@ def run_c5(torch, dist, device, world, steps):
             "exchange_exact": ok, "kernel": eng.last_kernel_name()}
 
 
+DUMP_STREAMS = 512  # 512 streams x 16 frames x 1024 bins x 4 B = 32 MiB at the default shape
+
+
+def dump_outputs(path, out, S):
+    """The last timed step's dB spectra for a seeded sample of streams (all streams when there are few)."""
+    import numpy as np
+    import torch
+
+    d = Path(path)
+    d.mkdir(parents=True, exist_ok=True)
+    pick = np.arange(S) if S <= DUMP_STREAMS else np.sort(np.random.default_rng(0).choice(S, DUMP_STREAMS, replace=False))
+    db =out[torch.from_numpy(pick).to(out.device)].cpu().numpy()
+    np.save(d / "db.npy", db.astype(np.float32, copy=False))
+    np.save(d / "streams.npy", pick.astype(np.float64))
+
+
 def run_gpu_arm(args):
     import torch
     import torch.distributed as dist
@@ -425,6 +447,8 @@ def run_gpu_arm(args):
         evs[k + 1].record(stream)
     torch.cuda.synchronize()
     t_end = time.perf_counter()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out, S)
     launches = eng.launch_count - launches0
     kernel_name = eng.last_kernel_name()
     total_ms = evs[0].elapsed_time(evs[-1])
@@ -546,7 +570,7 @@ def run_gpu_arm(args):
             "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": workload_name(), "fft_size": N_FFT, "streams_per_gpu": S, "frames_per_stream": T,
                        "hop": N_FFT, "frames_per_step_per_gpu": frames_per_gpu,
-                       "l2_policy": "inputs 512 MiB + outputs 256 MiB per step exceed the 126 MB L2 (no flush needed)",
+                       "l2_policy": "inputs 512 MiB + outputs 256 MiB per step exceed the 50 MB L2 (no flush needed)",
                        "parallelism": f"streams sharded over {world} GPU(s), no data-path collective",
                        "extra": {"layouts_same_batch": layouts, "strong_scaling": strong, "c5": c5, "other_shapes": other}},
             "clocks": clocks,
@@ -585,6 +609,8 @@ def main():
     ap.add_argument("--no-layouts", action="store_true")
     ap.add_argument("--no-c5", action="store_true")
     ap.add_argument("--no-numa-bind", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (seeded sample of streams) as DIR/*.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference_arm(args)

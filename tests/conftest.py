@@ -10,7 +10,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with `-m gpu` under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with `-m gpu`)")
     config.addinivalue_line("markers", "ref: needs oracle/_ref/libwaveform_ref.so (the compiled reference)")
 
 

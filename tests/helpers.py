@@ -29,14 +29,15 @@ def db_to_lin(db):
     return np.power(10.0, np.asarray(db, dtype=np.float64) / 20.0)
 
 
-def parity_report(got_db, ref_db, db_min=-758.0):
+def parity_report(got_db, ref_db, db_min=-758.0, peak=None):
     """Compare dB spectra in the LINEAR domain (what the 1e-5 relative bar of the north star is about).
 
     A pure per-bin relative test is meaningless for an fp32 FFT (bins far below the frame's energy carry the
     rounding noise of the big bins; the real FFTW has the same property against an fp64 DFT), so the criterion is
         |gpu - ref| <= 1e-5 * |ref| + 1e-6 * frame_peak        (linear magnitudes)
     and we also report: normwise error (max|d| / frame peak), fraction of bins inside the pure 1e-5 relative test,
-    and max |d dB| over the bins within 60 dB of the frame peak.
+    and max |d dB| over the bins within 60 dB of the frame peak.  `peak` (linear, one per frame) is given when the
+    spectra are a sample of each frame's bins (refdata.frame_peak of the whole reference frame).
     """
     got_db = np.asarray(got_db, dtype=np.float64)
     ref_db = np.asarray(ref_db, dtype=np.float64)
@@ -45,7 +46,7 @@ def parity_report(got_db, ref_db, db_min=-758.0):
     g, r = db_to_lin(got_db), db_to_lin(ref_db)
     g[floor_mask] = 0.0
     r[floor_mask] = 0.0
-    peak = np.maximum(r.max(axis=-1, keepdims=True), 1e-300)
+    peak = np.maximum(r.max(axis=-1, keepdims=True), 1e-300) if peak is None else np.asarray(peak, dtype=np.float64)
     d = np.abs(g - r)
     tol = 1e-5 * r + 1e-6 * peak
     strong = (r >= peak * 1e-3) & ~floor_mask

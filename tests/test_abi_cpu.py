@@ -182,7 +182,7 @@ def test_plugin_binding_compiles_against_the_unmodified_reference():
     from oracle import refbind
 
     if not refbind.cuda_seam_available():
-        pytest.skip("oracle/_ref/libwaveform_ref_cuda.so not built (needs /root/reference)")
+        pytest.skip("oracle/_ref/libwaveform_ref_cuda.so not built (needs the reference sources)")
     src = refbind.RefSource({"fft_size": 2048, "window": "hann"}, impl=refbind.IMPL_CUDA, channels=1)
     assert src.fft_size == 2048
     if not torch.cuda.is_available():

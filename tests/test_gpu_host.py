@@ -1,5 +1,6 @@
 """The C++ host-side mirror (waveform_b200/host/SpectrumSourceCUDA: ring buffers, A/V sync, timeout, live ticks through
-the C-ABI) against the compiled reference driven with the SAME packet / tick schedule."""
+the C-ABI) against the compiled reference driven with the SAME packet / tick schedule (what the reference computed is
+stored under tests/golden/, tests/refdata.py: silent flags in full, the spectra of a fixed sample of ticks and bins)."""
 import subprocess
 import sys
 from pathlib import Path
@@ -8,6 +9,7 @@ import numpy as np
 import pytest
 
 from helpers import parity_report, synth_pcm
+from refdata import frame_peak, reference, sample_index
 
 pytestmark = pytest.mark.gpu
 ROOT = Path(__file__).resolve().parents[1]
@@ -24,8 +26,7 @@ def _build_driver(tmp_path):
 
 def _reference_live(settings, cc, pcm, N, packet, fps, ticks):
     from oracle import refbind
-    if not refbind.available():
-        pytest.skip("oracle/_ref not built")
+
     ref = refbind.RefSource(settings, impl=refbind.IMPL_GENERIC, channels=cc)
     L, h = ref.L, ref.h
     now = 10 * 10**9
@@ -55,13 +56,35 @@ def _reference_live(settings, cc, pcm, N, packet, fps, ticks):
     return np.stack(out), np.array(sil, dtype=np.uint8)
 
 
-@pytest.mark.parametrize("N,cc,stereo,normalize", [(4096, 2, 1, 0), (2048, 1, 0, 0), (1024, 2, 0, 0), (2048, 2, 1, 1), (800, 1, 0, 1)])
-def test_live_adapter_matches_reference_plugin(tmp_path, N, cc, stereo, normalize):
-    exe = _build_driver(tmp_path)
-    packet, fps, ticks = 480, 60, 45
-    ns = 48000
+def _reference(N, cc, stereo, normalize, pcm, packet, fps, ticks):
+    settings = {"fft_size": N, "channel_mode": "stereo" if stereo else "mono"}
+    if normalize:  # the RMS feed runs live in both: capture_audio pre-accumulate + update_input_rms (not forced)
+        settings["normalize_volume"] = True
+    t_at, b_at = sample_index((ticks,), 8, N), sample_index((N // 2,), 64, N + 1)
+
+    def live():
+        ref, ref_sil = _reference_live(settings, cc, pcm, N, packet, fps, ticks)
+        return {"silent": ref_sil, "db": ref[t_at][..., b_at], "peak": frame_peak(ref[t_at], -758.0)}
+
+    return reference(f"live_adapter/{N}_{cc}_{stereo}_{normalize}", live), t_at, b_at
+
+
+def _input(cc, ns):
     pcm = synth_pcm(1, cc, ns, seed=21)[0]
     pcm[:, 20000:] = 0.0  # goes silent: EMA decay, then the gate
+    return pcm
+
+
+CASES = [(4096, 2, 1, 0), (2048, 1, 0, 0), (1024, 2, 0, 0), (2048, 2, 1, 1), (800, 1, 0, 1)]
+PACKET, FPS, TICKS, SAMPLES = 480, 60, 45, 48000
+
+
+@pytest.mark.parametrize("N,cc,stereo,normalize", CASES)
+def test_live_adapter_matches_reference_plugin(tmp_path, N, cc, stereo, normalize):
+    exe = _build_driver(tmp_path)
+    packet, fps, ticks = PACKET, FPS, TICKS
+    ns = SAMPLES
+    pcm = _input(cc, ns)
     inp, outp = tmp_path / "pcm.f32", tmp_path / "out.f32"
     pcm.astype(np.float32).tofile(inp)
     r = subprocess.run([str(exe), str(inp), str(cc), str(ns), str(N), str(packet), str(fps), str(ticks), str(outp),
@@ -72,10 +95,7 @@ def test_live_adapter_matches_reference_plugin(tmp_path, N, cc, stereo, normaliz
     raw = np.fromfile(outp, dtype=np.uint8).reshape(ticks, dch * B * 4 + 1)
     got = raw[:, :-1].copy().view(np.float32).reshape(ticks, dch, B)
     got_sil = raw[:, -1]
-    settings = {"fft_size": N, "channel_mode": "stereo" if stereo else "mono"}
-    if normalize:  # the RMS feed runs live in both: capture_audio pre-accumulate + update_input_rms (not forced)
-        settings["normalize_volume"] = True
-    ref, ref_sil = _reference_live(settings, cc, pcm, N, packet, fps, ticks)
-    assert np.array_equal(got_sil, ref_sil)
-    rep = parity_report(got, ref)
+    ref, t_at, b_at = _reference(N, cc, stereo, normalize, pcm, packet, fps, ticks)
+    assert np.array_equal(got_sil, ref["silent"])
+    rep = parity_report(got[t_at][..., b_at], ref["db"], peak=ref["peak"])
     assert rep["ok"], rep

@@ -1,6 +1,6 @@
 """GPU parity tests proper: the CUDA path (through the C-ABI) against the oracle on identical PCM.
 
-Run on a B200:  python -m pytest tests -m gpu -x -q
+Run on an H100:  python -m pytest tests -m gpu -x -q
 """
 from __future__ import annotations
 

@@ -1,12 +1,12 @@
 """GPU parity at the launch geometries that are actually MEASURED (bench.py, tools/bench_shapes.py), not toy shapes.
 
 The small-shape tests (test_gpu_parity.py) run 1-37 streams, which the N=2048 warp-per-stream kernel maps to one warp
-per CTA and one round.  The headline launch is 148 CTAs x 16 warps x 2 rounds with SM-interleaved stream indices and
+per CTA and one round.  The headline launch is 132 CTAs x 16 warps x 2 rounds with SM-interleaved stream indices and
 next-stream TMA prefetch; the CTA-per-tick kernel picks its cluster size from the stream count.  These tests run the
 real geometries on the device and compare a strided sample of streams (first / last warp of several CTAs, every round,
 plus random ones: >= 64 streams) against the oracle, and every stream against a cheap whole-batch invariant.
 
-Run on a B200:  python -m pytest tests -m gpu -x -q
+Run on an H100:  python -m pytest tests -m gpu -x -q
 """
 from __future__ import annotations
 
@@ -20,15 +20,15 @@ from helpers import check_points, device_pcm, fp64_truth_db, parity_report, synt
 
 pytestmark = pytest.mark.gpu
 
-SMS = 148
+SMS = 132  # H100 SXM: the N=2048 kernel launches one CTA per SM
 
 
 def _sample_streams(S: int, n_random: int = 40, seed: int = 1) -> list[int]:
-    """Streams at the corners of the N=2048 kernel's decomposition (stream s -> CTA s % 148, local index s // 148,
+    """Streams at the corners of the N=2048 kernel's decomposition (stream s -> CTA s % SMS, local index s // SMS,
     warp = local % 16, round = local // 16) + the first/last few + random ones."""
     per_cta = (S + SMS - 1) // SMS
     locals_ = sorted({0, 1, 15, 16, 17, per_cta - 2, per_cta - 1} & set(range(per_cta)))
-    ctas = [0, 1, 2, 73, 74, 146, 147]
+    ctas = [0, 1, 2, SMS // 2 - 1, SMS // 2, SMS - 2, SMS - 1]
     pick = {c + li * SMS for li in locals_ for c in ctas}
     pick |= {0, 1, 2, S - 1, S - 2, S // 2}
     rng = np.random.default_rng(seed)
@@ -92,8 +92,8 @@ def _run_and_check(settings, channels, S, T, hop_div=1, zero_every=7, want_point
 
 FAST_SHAPES = [
     # (S, T, calls): 300 -> 3 warps/CTA; 2500 -> 16 warps + a ragged second round; 4096x16 = the bench launch;
-    # 65536x1 and 1024x64 = two more layouts of profiles/r0x_layouts.txt; 2369 -> one stream more than 148 x 16
-    (300, 9, 1), (2500, 5, 2), (4096, 16, 1), (2369, 3, 1), (65536, 1, 1), (1024, 40, 2), (768, 33, 3),
+    # 65536x1 and 1024x64 = two more layouts of profiles/r0x_layouts.txt; 2113 -> one stream more than 132 x 16; 2369 -> a ragged second round
+    (300, 9, 1), (2500, 5, 2), (4096, 16, 1), (2369, 3, 1), (2113, 3, 1), (65536, 1, 1), (1024, 40, 2), (768, 33, 3),
 ]
 
 
@@ -108,7 +108,7 @@ def test_fast2048_parity_at_measured_geometry(S, T, calls, monkeypatch):
 
 @pytest.mark.parametrize("S,T,calls,opts", [
     (4096, 16, 1, {}), (2500, 5, 2, {}), (2369, 3, 1, {}), (8192, 8, 1, {}), (4000, 9, 2, {"slope": 0.5, "fast_peaks": True, "rolloff_q": 1.0, "rolloff_rate": 6.0}),
-    (3000, 12, 1, {"gravity": 0.2, "floor": -40}),
+    (3000, 12, 1, {"gravity": 0.2, "floor": -40}), (2113, 3, 1, {}),
 ])
 def test_fast2048_split_runs_are_bit_identical_to_whole_streams(S, T, calls, opts, monkeypatch):
     """Split mode of the warp-per-stream kernel (an SM's frames cut into 16 equal runs: a stream changes warps mid-call through
@@ -167,7 +167,8 @@ def test_warp2_split_runs_are_bit_identical_to_whole_streams(N, S, T, points, mo
 
 TEAM_SHAPES = [
     # (S, T, calls, W expected): few streams x many ticks (SURVEY §8(d) C3 '256 x 256' family) -> a team of W warps per stream
-    (256, 64, 2, 8), (512, 48, 2, 4), (148, 48, 3, 16), (1024, 21, 2, 4), (300, 9, 1, 4), (37, 5, 1, 4), (600, 8, 2, 4), (1184, 6, 1, 4),
+    # W follows the streams per SM (132 SMs): 1 -> 16, 2 -> 8, 3..8 -> 4
+    (256, 64, 2, 8), (512, 48, 2, 4), (132, 48, 3, 16), (1024, 21, 2, 4), (300, 9, 1, 4), (37, 5, 1, 4), (600, 8, 2, 4), (1056, 6, 1, 4),
 ]
 
 

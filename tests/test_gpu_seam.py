@@ -16,7 +16,7 @@ def _pair(settings, channels):
     from oracle import refbind
 
     if not (refbind.available() and refbind.cuda_seam_available()):
-        pytest.skip("oracle/_ref libraries not built (make -C oracle/ref_build)")
+        pytest.skip("oracle/_ref libraries not built (needs the reference sources)")
     return (refbind.RefSource(settings, impl=refbind.IMPL_GENERIC, channels=channels),
             refbind.RefSource(settings, impl=refbind.IMPL_CUDA, channels=channels))
 

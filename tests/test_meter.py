@@ -1,7 +1,7 @@
 """Level meter (tick_meter) and RMS feed (update_input_rms): SURVEY.md §8(f) rank 4 / §8(a) a9.
 
-CPU: the oracle restatement (oracle/wf_oracle_meter.c) bit-exact against the compiled reference and against the
-committed golden fixtures.  GPU: the CUDA path (wf_meter_* through the C-ABI) against the oracle — bit-exact for peak
+CPU: the oracle restatement (oracle/wf_oracle_meter.c) bit-exact against the compiled reference (its outputs stored as
+digests, tests/refdata.py) and against the committed golden fixtures.  GPU: the CUDA path (wf_meter_* through the C-ABI) against the oracle — bit-exact for peak
 values and silent flags, 1e-5 relative for RMS values: an fp32 sum of W squares depends on the order of the additions —
 the reference's own AVX path (src/source_avx.cpp:257-268, 16 partial sums) differs from its generic path (ring order,
 one accumulator) by 1.8e-6 on this data; the CUDA path sums 256-sample blocks.
@@ -15,6 +15,7 @@ import numpy as np
 import pytest
 
 from helpers import synth_pcm
+from refdata import digest, reference
 
 GOLD = sorted((Path(__file__).parent / "golden").glob("meter_*.npz"))
 
@@ -37,30 +38,31 @@ def _case_pcm(ch, T, hop, S=1):
 
 @pytest.mark.parametrize("settings,ch,hop", METER_CASES)
 def test_meter_oracle_is_bit_exact_vs_compiled_reference(settings, ch, hop):
-    refbind = pytest.importorskip("oracle.refbind")
-    if not refbind.available():
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
     from oracle.oraclebind import OracleMeter
 
     T = 60
     pcm = _case_pcm(ch, T, hop)[0]
-    r = refbind.RefSource({"display_mode": "level_meter", **settings}, channels=ch)
-    ref = r.run_meter(pcm, T, hop)
+    ref = reference(f"meter/case{METER_CASES.index((settings, ch, hop))}", lambda: _live_meter(settings, ch, pcm, T, hop))
     o = OracleMeter(settings, channels=ch)
-    assert o.window == r.fft_size
+    assert o.window == int(ref["window"])
     out = o.run(pcm, T, hop)
     for key in ("db", "lin", "silent"):
-        assert np.array_equal(ref[key], out[key]), key
-    assert ref["silent"].sum() > 0 or settings.get("floor", -65) < -60
+        assert np.array_equal(digest(out[key]), ref[key]), key
+    assert out["silent"].sum() > 0 or settings.get("floor", -65) < -60
+
+
+def _live_meter(settings, ch, pcm, T, hop):
+    from oracle import refbind
+
+    r = refbind.RefSource({"display_mode": "level_meter", **settings}, channels=ch)
+    ref = r.run_meter(pcm, T, hop)
+    return {"window": r.fft_size, **{key: digest(ref[key]) for key in ("db", "lin", "silent")}}
 
 
 @pytest.mark.parametrize("seed", range(30))
 def test_meter_oracle_randomised_settings_bit_exact_vs_compiled_reference(seed):
     """Differential fuzz of the level-meter oracle against the unmodified reference (generic path): random window, mode,
     smoothing, gravity, floor, packet size and channel count, with a silent stretch."""
-    refbind = pytest.importorskip("oracle.refbind")
-    if not refbind.available():
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
     from oracle.oraclebind import OracleMeter
 
     rng = np.random.default_rng(9000 + seed)
@@ -72,28 +74,30 @@ def test_meter_oracle_randomised_settings_bit_exact_vs_compiled_reference(seed):
     hop = int(rng.choice([97, 441, 480, 800, 801, 1024, 1601]))
     T = 50
     pcm = _case_pcm(ch, T, hop)[0] * np.float32(rng.choice([1.0, 0.1, 0.01]))
-    r = refbind.RefSource({"display_mode": "level_meter", **settings}, channels=ch)
-    ref = r.run_meter(pcm, T, hop)
+    ref = reference(f"meter/seed{seed}", lambda: _live_meter(settings, ch, pcm, T, hop))
     o = OracleMeter(settings, channels=ch)
-    assert o.window == r.fft_size
+    assert o.window == int(ref["window"])
     out = o.run(pcm, T, hop)
     for key in ("db", "lin", "silent"):
-        assert np.array_equal(ref[key], out[key]), (key, settings, hop)
+        assert np.array_equal(digest(out[key]), ref[key]), (key, settings, hop)
 
 
 @pytest.mark.parametrize("ch", [1, 2])
 def test_rms_feed_oracle_is_bit_exact_vs_compiled_reference(ch):
-    refbind = pytest.importorskip("oracle.refbind")
-    if not refbind.available():
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
     from oracle.oraclebind import OracleMeter
 
     T, hop = 90, 800
     pcm = _case_pcm(ch, T, hop)[0]
-    r = refbind.RefSource({"normalize_volume": True, "fft_size": 1024}, channels=ch)
-    ref = r.run_meter(pcm, T, hop)["rms"]
+
+    def live():
+        from oracle import refbind
+
+        r = refbind.RefSource({"normalize_volume": True, "fft_size": 1024}, channels=ch)
+        return {"rms": digest(r.run_meter(pcm, T, hop)["rms"])}
+
+    ref = reference(f"rms_feed/ch{ch}", live)
     out = OracleMeter({}, channels=ch).run(pcm, T, hop, meter=False, rms=True)["rms"]
-    assert np.array_equal(ref, out)
+    assert np.array_equal(digest(out), ref["rms"])
 
 
 @pytest.mark.parametrize("path", GOLD, ids=[p.stem for p in GOLD])

@@ -1,7 +1,7 @@
 """Waveform (oscilloscope) mode, tick_waveform: SURVEY.md §8(f) rank 4.
 
-CPU: the oracle restatement (oracle/wf_oracle_meter.c, wfo_wave_*) bit-exact against the compiled reference and against the
-committed golden fixtures.  GPU: the CUDA path (wf_wave_* through the C-ABI) against the oracle — which points are emitted and
+CPU: the oracle restatement (oracle/wf_oracle_meter.c, wfo_wave_*) bit-exact against the compiled reference (its outputs
+stored as digests, tests/refdata.py) and against the committed golden fixtures.  GPU: the CUDA path (wf_wave_* through the C-ABI) against the oracle — which points are emitted and
 which sample each takes is integer arithmetic and must match exactly (checked through the DB_MIN pattern and the silent
 flags); the dBFS values agree to 1e-4 dB (log10f last-bit differences between glibc and CUDA).
 """
@@ -14,6 +14,7 @@ import numpy as np
 import pytest
 
 from helpers import synth_pcm
+from refdata import digest, reference
 
 GOLD = sorted((Path(__file__).parent / "golden").glob("wave_*.npz"))
 
@@ -39,27 +40,29 @@ def _case(settings, ch, hop, T=50, S=1):
 
 @pytest.mark.parametrize("settings,ch,hop", WAVE_CASES)
 def test_wave_oracle_is_bit_exact_vs_compiled_reference(settings, ch, hop):
-    refbind = pytest.importorskip("oracle.refbind")
-    if not refbind.available():
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
     from oracle.oraclebind import OracleWave
 
     T = 50
     pcm, rms = _case(settings, ch, hop, T)
+    rms = None if rms is None else rms[0]
+    ref = reference(f"wave/case{WAVE_CASES.index((settings, ch, hop))}", lambda: _live_wave(settings, ch, pcm[0], T, hop, rms))
+    out = OracleWave(settings, channels=ch).run(pcm[0], T, hop, rms=rms)
+    assert np.array_equal(digest(out["out"]), ref["out"])
+    assert np.array_equal(digest(out["silent"]), ref["silent"])
+
+
+def _live_wave(settings, ch, pcm, T, hop, rms):
+    from oracle import refbind
+
     r = refbind.RefSource({"display_mode": "waveform", **settings}, channels=ch)
-    ref = r.run_wave(pcm[0], T, hop, rms=None if rms is None else rms[0])
-    out = OracleWave(settings, channels=ch).run(pcm[0], T, hop, rms=None if rms is None else rms[0])
-    assert np.array_equal(ref["out"], out["out"])
-    assert np.array_equal(ref["silent"], out["silent"])
+    ref = r.run_wave(pcm, T, hop, rms=rms)
+    return {"out": digest(ref["out"]), "silent": digest(ref["silent"])}
 
 
 @pytest.mark.parametrize("seed", range(30))
 def test_wave_oracle_randomised_settings_bit_exact_vs_compiled_reference(seed):
     """Differential fuzz of the waveform-mode oracle against the unmodified reference: random width, window length, packet size,
     channel layout, volume normalisation, stretches of zeros and of full-scale samples (the all-zero silent rule's raw material)."""
-    refbind = pytest.importorskip("oracle.refbind")
-    if not refbind.available():
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
     from oracle.oraclebind import OracleWave
 
     rng = np.random.default_rng(7000 + seed)
@@ -78,11 +81,11 @@ def test_wave_oracle_randomised_settings_bit_exact_vs_compiled_reference(seed):
     if ch == 2 and rng.uniform() < 0.4:
         pcm[:, 1] = 0.0
     rms = (0.05 + 0.2 * rng.uniform(size=(1, T))).astype(np.float32) if settings.get("normalize_volume") else None
-    r = refbind.RefSource({"display_mode": "waveform", **settings}, channels=ch)
-    ref = r.run_wave(pcm[0], T, hop, rms=None if rms is None else rms[0])
-    out = OracleWave(settings, channels=ch).run(pcm[0], T, hop, rms=None if rms is None else rms[0])
-    assert np.array_equal(ref["out"], out["out"]), settings
-    assert np.array_equal(ref["silent"], out["silent"]), settings
+    rms = None if rms is None else rms[0]
+    ref = reference(f"wave/seed{seed}", lambda: _live_wave(settings, ch, pcm[0], T, hop, rms))
+    out = OracleWave(settings, channels=ch).run(pcm[0], T, hop, rms=rms)
+    assert np.array_equal(digest(out["out"]), ref["out"]), settings
+    assert np.array_equal(digest(out["silent"]), ref["silent"]), settings
 
 
 @pytest.mark.parametrize("path", GOLD, ids=[p.stem for p in GOLD])
@@ -236,7 +239,7 @@ def test_gpu_wave_chunked_kernel_is_bit_identical_to_the_per_tick_kernel(setting
 @pytest.mark.gpu
 @pytest.mark.parametrize("settings,ch,hop", [CHUNK_CASES[0], CHUNK_CASES[1], CHUNK_CASES[5]])
 def test_gpu_wave_chunked_kernel_many_streams(settings, ch, hop, monkeypatch):
-    """More streams than resident CTAs (148 SMs x 5): every CTA walks several streams, its shared-memory state is rebuilt per stream."""
+    """More streams than resident CTAs (132 SMs x 5): every CTA walks several streams, its shared-memory state is rebuilt per stream."""
     _chunk_vs_per_tick(settings, ch, hop, 1700, 24, monkeypatch)
 
 

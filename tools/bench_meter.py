@@ -10,7 +10,7 @@ import torch
 from waveform_b200 import MeterEngine, WaveEngine
 from waveform_b200.engine import METER_INPUT_RMS
 
-PEAK = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())["hbm_gbs"] if (ROOT / "MEASURED_PEAKS.json").exists() else 6650.0
+PEAK = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())["hbm_gbs"] if (ROOT / "MEASURED_PEAKS.json").exists() else 3350.0
 for name, settings, ch, S, T, hop, mode in [
         ("meter RMS 150 ms stereo", {"meter_buf": 150, "rms_mode": True}, 2, 4096, 64, 800, None),
         ("meter peak 100 ms mono", {"meter_buf": 100, "rms_mode": False}, 1, 8192, 64, 800, None),

@@ -12,7 +12,7 @@ import torch
 from waveform_b200 import Engine
 from helpers import synth_pcm
 
-PEAK = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())["hbm_gbs"] if (ROOT / "MEASURED_PEAKS.json").exists() else 6650.0
+PEAK = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())["hbm_gbs"] if (ROOT / "MEASURED_PEAKS.json").exists() else 3350.0
 print("== rank 1: non-power-of-two sizes, device-resident, S=4096 streams x T=16 ticks, hop=N")
 for N in (800, 720, 960, 1600, 1920, 2000, 4160):
     S, T = 4096, 16

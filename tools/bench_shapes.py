@@ -33,7 +33,7 @@ def run_shapes(torch, only=None, iters=10, peak_gbs=None):
 
     if peak_gbs is None:
         pk = ROOT / "MEASURED_PEAKS.json"
-        peak_gbs = json.loads(pk.read_text())["hbm_gbs"] if pk.exists() else 6650.0
+        peak_gbs = json.loads(pk.read_text())["hbm_gbs"] if pk.exists() else 3350.0
     res = []
     for name, settings, ch, S, T, hop, mode in SHAPES:
         if only and not any(o in name for o in only):

@@ -1,4 +1,4 @@
-"""waveform_b200 — B200 (sm_100a) batched STFT engine behind phandasm/waveform's tick_spectrum seam.
+"""waveform_b200 — H100 (sm_90a) batched STFT engine behind phandasm/waveform's tick_spectrum seam.
 
 Only what the hot path needs lives here: csrc/ (CUDA kernels + the C-ABI of include/wfstft.h),
 host/ (C++ host-side mirror of the plugin's capture/tick plumbing) and this thin ctypes binding.

@@ -1,4 +1,4 @@
-// wf_engine.cu — libwfstft.so: the C ABI of include/wfstft.h on top of the fused sm_100a kernel.
+// wf_engine.cu — libwfstft.so: the C ABI of include/wfstft.h on top of the fused sm_90a kernel.
 //
 // Host responsibilities (mirrors what WAVSource owns in the reference, src/source.hpp:95-347):
 //   * settings -> tables (wf_tables.cpp ≙ WAVSource::update), uploaded once per engine
@@ -620,8 +620,8 @@ int wf_create(const wf_config *cfg, wf_engine **out)
     cudaDeviceProp prop{};
     WF_CUDA_C(cudaGetDeviceProperties(&prop, dev));
     e->sm_count = prop.multiProcessorCount;
-    if(prop.major < 10)
-        return bail(set_err(e, WF_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_100a only", dev,
+    if(prop.major != 9 || prop.minor != 0) // sm_90a code runs on compute capability 9.0 only
+        return bail(set_err(e, WF_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", dev,
                             prop.major, prop.minor));
     WF_CUDA_C(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
     WF_CUDA_C(cudaEventCreate(&e->ev0));
@@ -878,7 +878,7 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
         kp.split = e->split_runs ? 1 : 0;
         if(kp.lazy_hold)
             e->hold_implicit = true;
-        // Fewer streams than 148 SMs x 16 warps: a team of W warps per stream works on W ticks at once (wf_team2048.cuh).
+        // Fewer streams than SMs x 16 warps: a team of W warps per stream works on W ticks at once (wf_team2048.cuh).
         // Up to 8 streams per SM: 16 / W = 1, 2 or 4 teams per SM (a team takes its streams one after the other); measured
         // (profiles/r02_layouts.txt) 256 x 256: 142 -> 272 M spectra/s, 512 x 128: 200 -> 310 M, 1024 x 64: 289 -> 332 M.
         int W = 1;

@@ -1,4 +1,4 @@
-// wf_fast2048.cuh — hand-specialised sm_100a kernel for the headline shape: N = 2048, one capture
+// wf_fast2048.cuh — hand-specialised sm_90a kernel for the headline shape: N = 2048, one capture
 // channel, 16-byte aligned frames (hop % 4 == 0), spectrum output only.
 //
 // One WARP owns one stream and walks its frames; per frame:

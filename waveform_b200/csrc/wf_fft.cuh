@@ -1,4 +1,4 @@
-// wf_fft.cuh — register-resident DFT building blocks for the sm_100a STFT kernels.
+// wf_fft.cuh — register-resident DFT building blocks for the sm_90a STFT kernels.
 //
 // A thread holds R complex points in registers (R = 2..32) and performs a radix-2 decimation-in-
 // frequency network on them with compile-time twiddles; the result of bin k ends up in register
@@ -137,11 +137,10 @@ __device__ __forceinline__ void dft_bitrev(float2 (&v)[R])
 } // namespace wf
 
 // ---------------------------------------------------------------------------------------------------
-// Packed complex arithmetic on Blackwell's f32x2 datapath (add/mul/fma.rn.f32x2 -> FADD2/FMUL2/FFMA2).
-// A complex number lives in one 64-bit register pair (re = low half, im = high half).  The SASS operand
-// modifiers (.F32x2.LO_HI, .NP/.PN) make swap / conj / multiply-by-±i free, so a complex add is ONE
-// instruction and a complex multiply is TWO (vs 2 and 4 scalar) — the kernels here are issue-bound, not
-// FP-pipe-bound (tools/ubench/f32x2.cu: FFMA2 has the same FMA/clk as FFMA but half the issue slots).
+// Complex arithmetic on a 64-bit register pair (re = low half, im = high half).  Hopper has no packed FP32
+// datapath, so every elementwise operation is two scalar IEEE round-to-nearest operations; the explicit
+// __fadd_rn / __fmul_rn / __fmaf_rn forms keep ptxas from contracting a separate mul + add into one FMA, so
+// each lane rounds exactly as written.  The pair packing (mov.b64) is a register renaming and costs nothing.
 // ---------------------------------------------------------------------------------------------------
 namespace wf {
 namespace pk {
@@ -179,27 +178,32 @@ __device__ __forceinline__ float2 to_float2(c64 a)
 }
 __device__ __forceinline__ c64 add(c64 a, c64 b)
 {
-    c64 r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float ax, ay, bx, by;
+    split(a, ax, ay);
+    split(b, bx, by);
+    return make(__fadd_rn(ax, bx), __fadd_rn(ay, by));
 }
 __device__ __forceinline__ c64 sub(c64 a, c64 b)
 {
-    c64 r;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float ax, ay, bx, by;
+    split(a, ax, ay);
+    split(b, bx, by);
+    return make(__fsub_rn(ax, bx), __fsub_rn(ay, by));
 }
 __device__ __forceinline__ c64 mul(c64 a, c64 b) // elementwise
 {
-    c64 r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float ax, ay, bx, by;
+    split(a, ax, ay);
+    split(b, bx, by);
+    return make(__fmul_rn(ax, bx), __fmul_rn(ay, by));
 }
 __device__ __forceinline__ c64 fma(c64 a, c64 b, c64 c) // elementwise a*b+c
 {
-    c64 r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
+    float ax, ay, bx, by, cr, ci;
+    split(a, ax, ay);
+    split(b, bx, by);
+    split(c, cr, ci);
+    return make(__fmaf_rn(ax, bx, cr), __fmaf_rn(ay, by, ci));
 }
 __device__ __forceinline__ c64 swap(c64 a)
 {
@@ -220,7 +224,6 @@ __device__ __forceinline__ c64 mul_neg_i(c64 a) // a * (-i) = (im, -re)
     return make(y, -x);
 }
 // complex multiply by a run-time twiddle w = (c, s):  a*(c,c) + (-a.im, a.re)*(s,s).
-// In this form ptxas emits exactly FMUL2 + FFMA2 (broadcast .F32 operands, .LO_HI.NP on the A operand).
 __device__ __forceinline__ c64 cmul(c64 a, c64 w)
 {
     float x, y, c, s;

@@ -1,4 +1,4 @@
-// wf_kernels.cuh — the fused per-frame spectrum pipeline as ONE sm_100a kernel:
+// wf_kernels.cuh — the fused per-frame spectrum pipeline as ONE sm_90a kernel:
 //
 //   PCM frame (HBM, read once) -> window multiply in the load prologue -> real-to-complex FFT as a
 //   Stockham autosort FFT of the N/2 packed complex points (register radix-8/16/32 butterflies,
@@ -254,7 +254,7 @@ struct Pass {
         for(int b = 0; b < BPT; ++b)
         {
             const int j = tid + b * TN;
-            pk::c64 x[R]; // packed f32x2 complex arithmetic: FADD2 / FMUL2 / FFMA2 (see wf_fft.cuh)
+            pk::c64 x[R]; // complex values as register pairs (see wf_fft.cuh)
 #pragma unroll
             for(int t = 0; t < R; ++t)
                 x[t] = pk::from(v[b * R + t]);

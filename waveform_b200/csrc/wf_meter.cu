@@ -1,4 +1,4 @@
-// wf_meter.cu — level meter (tick_meter) and RMS feed (update_input_rms) of the plugin as batched sm_100a reductions
+// wf_meter.cu — level meter (tick_meter) and RMS feed (update_input_rms) of the plugin as batched sm_90a reductions
 // behind the C ABI of include/wfstft.h (wf_meter_*).  SURVEY.md §8(f) rank 4 / §8(a) row a9.
 //
 // Reference semantics restated (paths relative to the reference tree):
@@ -627,8 +627,8 @@ int wf_meter_create(const wf_meter_config *cfg, wf_meter **out)
     WFM_C(cudaSetDevice(dev));
     cudaDeviceProp prop{};
     WFM_C(cudaGetDeviceProperties(&prop, dev));
-    if(prop.major < 10)
-        return bail(merr(m, WF_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_100a only", dev,
+    if(prop.major != 9 || prop.minor != 0) // sm_90a code runs on compute capability 9.0 only
+        return bail(merr(m, WF_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", dev,
                          prop.major, prop.minor));
     m->sm_count = prop.multiProcessorCount;
     WFM_C(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));

@@ -1,6 +1,6 @@
 // wf_team2048.cuh — N = 2048, one capture channel, spectrum output, FEW streams x MANY ticks (SURVEY §8(d) C3 "256 x 256").
 //
-// The warp-per-stream kernel (wf_fast2048.cuh) needs ~2400 streams to fill 148 SMs x 16 warps.  With fewer streams the only
+// The warp-per-stream kernel (wf_fast2048.cuh) needs ~2100 streams to fill 132 SMs x 16 warps.  With fewer streams the only
 // sequential part of a stream is the EMA / gate recurrence over ticks — the FFT of a tick is not.  Here a TEAM of W warps
 // (W = 4, 8, 16; 16/W teams per CTA, one CTA per SM) owns a stream and works on W consecutive ticks at once:
 //

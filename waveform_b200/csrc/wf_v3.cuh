@@ -674,8 +674,7 @@ __global__ void __launch_bounds__(v3::Geo3<N>::TN, v3::Geo3<N>::MINB)
                         split_pair(X, twp, j, m1, m2);
                         // EMA of the pair, packed: g*old + (g2*mag) with ONE fused rounding on the first product, as
                         // wf_fast2048.cuh and the reference's AVX2 path (src/source_avx2.cpp:154); the cluster flow's scalar
-                        // ema() below uses the same form, so R = 1 and R > 1 stay bit-identical.  (ptxas contracts a packed
-                        // mul.rn + add.rn pair into FFMA2 anyway: the two-rounding form cannot be expressed in f32x2.)
+                        // ema() below uses the same form, so R = 1 and R > 1 stay bit-identical.
                         pk::c64 old = pk::make(st[c][2 * j], st[c][2 * j + 1]);
                         pk::c64 m = pk::make(m1, m2);
                         if(XF && p.fast_peaks)

@@ -6,7 +6,7 @@
 namespace wf {
 namespace warp2 {
 
-constexpr int kMaxSmem = 227 * 1024; // opt-in shared memory per CTA on sm_100
+constexpr int kMaxSmem = 227 * 1024; // opt-in shared memory per CTA on sm_90
 
 template<int L, int P, bool EXTRA, bool DISP>
 cudaError_t launch(const KParams &kp, int grid, int *warps_io, cudaStream_t st, bool pdl, int device)

@@ -1,4 +1,4 @@
-// wf_wave.cu — waveform (oscilloscope) mode of the plugin (tick_waveform) as a batched sm_100a gather behind the C ABI of
+// wf_wave.cu — waveform (oscilloscope) mode of the plugin (tick_waveform) as a batched sm_90a gather behind the C ABI of
 // include/wfstft.h (wf_wave_*).  SURVEY.md §8(f) rank 4.
 //
 // Reference semantics restated (paths relative to the reference tree): src/source_generic.cpp:272-390 with the capture side
@@ -785,8 +785,8 @@ int wf_wave_create(const wf_wave_config *cfg, wf_wave **out)
     WFW_C(cudaSetDevice(dev));
     cudaDeviceProp prop{};
     WFW_C(cudaGetDeviceProperties(&prop, dev));
-    if(prop.major < 10)
-        return bail(werr(w, WF_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_100a only", dev, prop.major,
+    if(prop.major != 9 || prop.minor != 0) // sm_90a code runs on compute capability 9.0 only
+        return bail(werr(w, WF_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", dev, prop.major,
                          prop.minor));
     w->sm_count = prop.multiProcessorCount;
     if(2 * (size_t)cfg->width * sizeof(float) > 48 * 1024) // widths above 6144: both scrolling rings exceed the default 48 KB

@@ -1,7 +1,7 @@
 """ctypes binding of libwfstft.so (include/wfstft.h) — the product's C-ABI, nothing else.
 
 This module deliberately contains no DSP: every number comes out of the CUDA library.  If the
-library is missing, or there is no sm_100 device, construction fails loudly (no CPU fallback).
+library is missing, or there is no sm_90 device, construction fails loudly (no CPU fallback).
 
 Settings use the reference plugin's own setting keys (/root/reference/src/settings.hpp:29-135), so a
 caller (or a test) configures the engine exactly as it would configure the OBS source:
