@@ -222,7 +222,7 @@ void wf_host_free(void *p);
 /* Number of kernel launches this engine has issued (bench.py reports it as gpu_launches). */
 int64_t wf_launch_count(const wf_engine *e);
 /* Name (template arguments and launch geometry included) of the spectrum kernel the most recent wf_process* call
- * dispatched to, e.g. "stft2048_fast_kernel<16,1,1,0> grid 132 x 16 warps"; "" before the first call.  Valid until the
+ * dispatched to, e.g. "stft2048_fast_kernel<12,1,1,0> grid 132 x 12 warps"; "" before the first call.  Valid until the
  * next call on this engine.  bench.py reports it as roofline.kernel, the tests assert the routing with it. */
 const char *wf_last_kernel_name(const wf_engine *e);
 /* Device time (ms) of the kernel section of the most recent wf_process / wf_process_async / wf_peak_normalize call,

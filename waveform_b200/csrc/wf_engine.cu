@@ -48,7 +48,6 @@ struct wf_engine {
     bool lazy_hold = true;      // WF_LAZY_HOLD=0: always write the mirror (A/B tests)
     bool split_runs = true;     // WF_SPLIT=0: whole streams per warp in the N=2048 warp-per-stream kernel (A/B tests)
     bool force_generic = false; // WF_FORCE_GENERIC=1: bypass the specialised N=2048 kernel (A/B tests)
-    int fast_maxw = 16;         // WF_FAST_MAXW=12|16: which compiled variant of the N=2048 kernel (tuning knob)
     int fast_wpc_override = 0;  // WF_FAST_WPC=n: force warps per CTA (tuning knob)
     bool use_pdl = true;        // WF_NO_PDL=1: launch the fast kernel without programmatic dependent launch
     int wide_r = 0;             // WF_WIDE_R=1|2|4|8: force the cluster size of the wide kernel (1 = never use it); 0 = automatic
@@ -391,26 +390,17 @@ int launch_fast2048(wf_engine *e, const KParams &kp, cudaStream_t st)
 int dispatch_fast2048(wf_engine *e, const KParams &kp, cudaStream_t st, bool extra)
 {
     const bool tsm = kp.tsmooth != 0, gate = kp.gate != 0;
-    const int maxw = e->fast_maxw;
-#define WF_FAST_CASE(W, T, G, X)            \
-    if(maxw == W && tsm == T && gate == G && extra == X) \
-        return launch_fast2048<W, T, G, X>(e, kp, st);
-    WF_FAST_CASE(16, true, true, false)
-    WF_FAST_CASE(16, true, true, true)
-    WF_FAST_CASE(16, true, false, false)
-    WF_FAST_CASE(16, true, false, true)
-    WF_FAST_CASE(16, false, true, false)
-    WF_FAST_CASE(16, false, true, true)
-    WF_FAST_CASE(16, false, false, false)
-    WF_FAST_CASE(16, false, false, true)
-    WF_FAST_CASE(12, true, true, false)
-    WF_FAST_CASE(12, true, true, true)
-    WF_FAST_CASE(12, true, false, false)
-    WF_FAST_CASE(12, true, false, true)
-    WF_FAST_CASE(12, false, true, false)
-    WF_FAST_CASE(12, false, true, true)
-    WF_FAST_CASE(12, false, false, false)
-    WF_FAST_CASE(12, false, false, true)
+#define WF_FAST_CASE(T, G, X)                  \
+    if(tsm == T && gate == G && extra == X) \
+        return launch_fast2048<fast::kMaxWarpsPerCta, T, G, X>(e, kp, st);
+    WF_FAST_CASE(true, true, false)
+    WF_FAST_CASE(true, true, true)
+    WF_FAST_CASE(true, false, false)
+    WF_FAST_CASE(true, false, true)
+    WF_FAST_CASE(false, true, false)
+    WF_FAST_CASE(false, true, true)
+    WF_FAST_CASE(false, false, false)
+    WF_FAST_CASE(false, false, true)
 #undef WF_FAST_CASE
     return set_err(e, WF_ERR_INVALID_ARG, "fast2048 dispatch fell through");
 }
@@ -567,9 +557,6 @@ int wf_create(const wf_config *cfg, wf_engine **out)
     {
         const char *fg = getenv("WF_FORCE_GENERIC");
         e->force_generic = fg && fg[0] == '1';
-        const char *mw = getenv("WF_FAST_MAXW");
-        if(mw && (atoi(mw) == 12 || atoi(mw) == 16))
-            e->fast_maxw = atoi(mw);
         const char *np = getenv("WF_NO_PDL");
         e->use_pdl = !(np && np[0] == '1');
         const char *wr = getenv("WF_WIDE_R");
@@ -869,8 +856,9 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
         extra = (size_t)groups * 4 * (size_t)kp.scratch_q * sizeof(float);
     }
     const bool aligned16 = (((uintptr_t)kp.pcm & 15u) == 0) && ((b->stream_stride & 3) == 0) && ((b->hop & 3) == 0);
+    // (the fast kernel writes each dB row with one bulk copy, which needs a 16-byte aligned destination)
     const bool fast_ok = (N == 2048) && (cc == 1) && !t.cfg.stereo && kp.out_db && !kp.out_points && !kp.out_pixels &&
-                         !kp.out_min && aligned16 && !e->force_generic;
+                         !kp.out_min && aligned16 && (((uintptr_t)kp.out_db & 15u) == 0) && !e->force_generic;
     if(fast_ok)
     {
         const bool x = kp.slope || kp.rolloff || kp.normalize || kp.fast_peaks || kp.skip_mask || kp.out_peak || kp.g_tab;

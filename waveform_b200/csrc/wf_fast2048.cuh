@@ -2,14 +2,15 @@
 // channel, 16-byte aligned frames (hop % 4 == 0), spectrum output only.
 //
 // One WARP owns one stream and walks its frames; per frame:
-//   * the 8 KB PCM frame is staged HBM -> shared memory by a TMA bulk copy (cp.async.bulk + mbarrier),
-//     issued one frame ahead (during the previous frame's epilogue) so the warp never waits on DRAM;
+//   * the 8 KB PCM frame is staged HBM -> shared memory by a TMA bulk copy (cp.async.bulk + mbarrier) into a
+//     landing buffer of its own; the next frame is requested as soon as the lanes have this one in registers, so
+//     a whole frame of work hides its DRAM latency;
 //   * the packed 1024-point complex FFT is two radix-32 register passes (32 points per lane) with ONE
 //     padded shared-memory transpose between them (conflict-free 64-bit accesses);
 //   * the real-FFT split pass processes bins k and N/2-k TOGETHER (one twiddle multiply for two bins),
 //     after a half-size exchange so that each lane owns both bins of its 16 pairs;
-//   * |X| via MUFU.SQRT, EMA with state in registers across the stream's frames, dB via MUFU.LG2,
-//     32 coalesced 128-byte store instructions per frame.
+//   * |X| via MUFU.SQRT, EMA with state kept on chip across the stream's frames, dB via MUFU.LG2; the dB row is
+//     staged in the (then free) transpose buffer and leaves as ONE 4 KB bulk store (cp.async.bulk ... bulk_group).
 // Tables (window, inter-pass twiddles, split twiddles: 20 KB) live in shared memory once per CTA.
 //
 // Semantics are those of wf_kernels.cuh / src/source_generic.cpp:26-180; differences are confined to the
@@ -23,12 +24,16 @@ namespace fast {
 
 constexpr int kN = 2048;
 constexpr int kM = 1024;
-constexpr int kWarpBufBytes = 32 * 33 * 8; // padded transpose buffer, also the TMA landing zone (8192 B used)
-constexpr int kStateBytes = 16 * 32 * 8; // EMA state of the stream: [pair q][lane] -> (bin k1, bin k2)
-constexpr int kWarpBytes = kWarpBufBytes + kStateBytes + 16; // + mbarrier
+// Per warp, in this order: the TMA landing buffer of the next frame (8 KiB); the padded transpose buffer, which after
+// pass B stages the frame's dB row for its bulk store (8448 B); the mbarrier and the split-mode hand-over flag (16 B).
+// Every part is 16-byte aligned.  The EMA state of the stream lives in registers.
+constexpr int kLandBytes = kN * 4;
+constexpr int kXposeBytes = 32 * 33 * 8;
+constexpr int kWarpBytes = kLandBytes + kXposeBytes + 16;
 constexpr int kTableBytes = (1024 + 1024 + 512) * 8;
-constexpr int kMaxWarpsPerCta = 16; // 1 CTA/SM: 16 warps x 12.3 KB + 20 KB tables = 216 KB of shared memory
+constexpr int kMaxWarpsPerCta = 12; // 1 CTA/SM: 12 warps x 16.3 KB + 20 KB tables = 215 KB of shared memory, 168 registers/thread
 constexpr int smem_bytes(int warps_per_cta) { return kTableBytes + warps_per_cta * kWarpBytes; }
+static_assert(smem_bytes(kMaxWarpsPerCta) <= 227 * 1024, "one CTA per SM must fit");
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -66,6 +71,24 @@ __device__ __forceinline__ void fence_proxy_async()
 {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
+// TMA 1-D bulk copy shared -> global, one bulk async-group of the issuing thread per copy
+__device__ __forceinline__ void bulk_store_1d(void *dst_gmem, const void *src_smem, uint32_t bytes)
+{
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst_gmem), "r"(smem_u32(src_smem)), "r"(bytes)
+                 : "memory");
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+}
+// the issuing thread's bulk stores have read their shared-memory source (it may be overwritten)
+__device__ __forceinline__ void bulk_wait_read()
+{
+    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+}
+// the issuing thread's bulk stores have written global memory, and generic-proxy loads ordered after this see it
+__device__ __forceinline__ void bulk_wait_written()
+{
+    asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    asm volatile("fence.proxy.async.global;" ::: "memory");
+}
 __device__ __forceinline__ float sqrt_approx(float x)
 {
     float r;
@@ -95,12 +118,19 @@ __device__ __forceinline__ pk::c64 dbfs2(float m1, float m2, float db_min)
 
 } // namespace fast
 
-// One CTA per SM with up to MAXW warps (16 -> 128 registers/thread, 12 -> 168).  WIN is not a template
-// parameter: without a window the shared "window" table simply holds the magnitude normalisation constant.
+// One CTA per SM with up to MAXW warps.  WIN is not a template parameter: without a window the shared "window" table
+// simply holds the magnitude normalisation constant.
+//
+// Bulk-store ordering: lane 0 issues every row store and is the only thread that can wait for it.  The staging row is
+// overwritten only after cp.async.bulk.wait_group.read (the copy has read it).  A generic load of a row that a bulk
+// store wrote — the hold / quirk path reads the previous row, the next warp reads it after a split-mode hand-over —
+// comes after cp.async.bulk.wait_group 0 and a proxy fence.  The mirror write-back reads the last row from the staging
+// buffer, which still holds it.
 template<int MAXW, bool TSM, bool GATE, bool EXTRA>
 __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __grid_constant__ KParams p)
 {
     using namespace fast;
+    static_assert(MAXW <= kMaxWarpsPerCta, "shared memory holds at most kMaxWarpsPerCta warps");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float2 *s_win = reinterpret_cast<float2 *>(smem_raw);
     float2 *s_twA = s_win + 1024; // [k2][n1] = W_1024^(k2*n1)
@@ -109,9 +139,11 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
     const int lane = threadIdx.x & 31;
     const int warps_per_cta = blockDim.x >> 5;
     unsigned char *wbase = reinterpret_cast<unsigned char *>(s_twP + 512) + warp * kWarpBytes;
-    float2 *buf = reinterpret_cast<float2 *>(wbase);
-    float2 *sst = reinterpret_cast<float2 *>(wbase + kWarpBufBytes) + lane; // this lane's column of the state
-    uint64_t *mbar = reinterpret_cast<uint64_t *>(wbase + kWarpBufBytes + kStateBytes);
+    float2 *land = reinterpret_cast<float2 *>(wbase);
+    float2 *buf = reinterpret_cast<float2 *>(wbase + kLandBytes);
+    float *row = reinterpret_cast<float *>(buf); // staging row of the dB output, natural bin order
+    uint64_t *mbar = reinterpret_cast<uint64_t *>(wbase + kWarpBytes - 16);
+    pk::c64 st[16]; // EMA state of the stream: [pair q] -> (bin k1, bin k2) of this lane
 
     // ---- CTA prologue: tables -> shared, mbarriers ----
     // The window table carries the magnitude normalisation (2/sum(w))/2 so the epilogue needs no extra multiply.
@@ -154,7 +186,7 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
 
     // ---- work list of this warp ----
     // Whole streams, dealt round-robin (local index li = warp, warp + W, ...), leave the last round partly empty: 4096 streams
-    // are 27.7 per SM, i.e. 16 busy warps for one round and 11.7 for the second.  In split mode (p.split, at least one
+    // are 31.0 per SM on 132 SMs, i.e. 12 busy warps for two rounds and 7 for the third.  In split mode (p.split, at least one
     // stream per warp, more than one tick) the SM's n_local * T frames are cut into W equal runs of consecutive frames
     // instead: a warp's run is [tail of stream a][whole streams][head of stream b], and a stream is continued by the next
     // warp exactly as it would be by the next call (state, flags and mirror go through global memory).  Order inside a
@@ -210,7 +242,7 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
         int li, t0, t1;
         segment(0, li, t0, t1);
         mbar_expect_tx(mbar, kN * 4);
-        tma_load_1d(buf, p.pcm + (size_t)(blockIdx.x + li * G) * p.stream_stride + (size_t)t0 * p.hop, kN * 4, mbar);
+        tma_load_1d(land, p.pcm + (size_t)(blockIdx.x + li * G) * p.stream_stride + (size_t)t0 * p.hop, kN * 4, mbar);
     }
 
     for(int j = 0; j < nseg; ++j)
@@ -230,19 +262,19 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
         {
             // continuation of a stream whose first ticks the previous warp ran as its head segment
             // (atomics on the flag, fences around them: the hand-over is a release / acquire pair at CTA scope)
-            int *prev_done = reinterpret_cast<int *>(wbase - kWarpBytes + kWarpBufBytes + kStateBytes + 8);
+            int *prev_done = reinterpret_cast<int *>(reinterpret_cast<unsigned char *>(seg_done) - kWarpBytes);
             if(lane == 0)
                 while(atomicAdd(prev_done, 0) == 0)
                     ;
             __syncwarp();
             __threadfence_block();
         }
-        // ---- per-stream state: global (natural bin order) -> shared ([pair][lane]) ----
+        // ---- per-stream state: global (natural bin order) -> this lane's pairs ----
         {
             const float *sp = p.state + (size_t)s * B;
 #pragma unroll
             for(int q = 0; q < 16; ++q)
-                sst[q * 32] = make_float2(sp[lane + 32 * q], sp[(q == 0) ? k2_q0 : (kb + 32 * (31 - q))]);
+                st[q] = pk::make(sp[lane + 32 * q], sp[(q == 0) ? k2_q0 : (kb + 32 * (31 - q))]);
         }
         const unsigned char fl = p.flags[s];
         bool last_silent = (fl & 1u) != 0;
@@ -262,13 +294,31 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
             phase ^= 1u;
             pk::c64 v[32];
             unsigned long long nzbits = 0;
+            const pk::c64 *land64 = reinterpret_cast<const pk::c64 *>(land);
             const pk::c64 *buf64 = reinterpret_cast<const pk::c64 *>(buf);
             const pk::c64 *win64 = reinterpret_cast<const pk::c64 *>(s_win);
 #pragma unroll
             for(int pidx = 0; pidx < 32; ++pidx)
             {
-                v[pidx] = buf64[lane + 32 * pidx];
+                v[pidx] = land64[lane + 32 * pidx];
                 nzbits |= v[pidx];
+            }
+            // every lane has the frame in registers: the landing buffer takes the next frame (or the next segment's
+            // first frame), a whole frame of work ahead of its use
+            __syncwarp();
+            if(lane == 0)
+            {
+                const float *next = nullptr;
+                if(t + 1 < t1)
+                    next = pcm_s + (size_t)(t + 1) * p.hop;
+                else if(s_next >= 0)
+                    next = p.pcm + (size_t)s_next * p.stream_stride + (size_t)t0_next * p.hop;
+                if(next != nullptr)
+                {
+                    fence_proxy_async();
+                    mbar_expect_tx(mbar, kN * 4);
+                    tma_load_1d(land, next, kN * 4, mbar);
+                }
             }
 #pragma unroll
             for(int pidx = 0; pidx < 32; ++pidx)
@@ -283,8 +333,11 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
                 pk::dft_bitrev<32>(v);
                 if(pass == 0)
                 {
-                    // inter-pass twiddle W_1024^(n1 k2), then transpose through the (padded) shared buffer
-                    __syncwarp(); // every lane has read the frame before the buffer becomes the transpose area
+                    // inter-pass twiddle W_1024^(n1 k2), then transpose through the (padded) shared buffer, which still
+                    // stages the previous row until its bulk store has read it
+                    if(lane == 0)
+                        bulk_wait_read();
+                    __syncwarp();
 #pragma unroll
                     for(int k2 = 0; k2 < 32; ++k2)
                     {
@@ -297,27 +350,12 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
 #pragma unroll
                     for(int n1 = 0; n1 < 32; ++n1)
                         v[n1] = buf64[n1 * 33 + lane];
-                    __syncwarp(); // all generic-proxy accesses to buf are done: it can take the next frame
+                    __syncwarp(); // every lane has read the transpose: buf can stage this frame's row
                     // the next stream's EMA state (4 KB, one 128-byte line per lane) is pulled into L2 now, so that the
                     // synchronous state load at the top of the stream loop does not pay DRAM latency (matters when a
                     // stream has few frames: the 65536 x 1 layout loads a state per frame)
                     if(t + 1 == t1 && s_next >= 0 && t0_next == 0)
                         asm volatile("prefetch.global.L2 [%0];" ::"l"(p.state + (size_t)s_next * B + lane * 32));
-                    // prefetch the next frame (or the next stream's first frame) under pass B + epilogue
-                    if(lane == 0)
-                    {
-                        const float *next = nullptr;
-                        if(t + 1 < t1)
-                            next = pcm_s + (size_t)(t + 1) * p.hop;
-                        else if(s_next >= 0)
-                            next = p.pcm + (size_t)s_next * p.stream_stride + (size_t)t0_next * p.hop;
-                        if(next != nullptr)
-                        {
-                            fence_proxy_async();
-                            mbar_expect_tx(mbar, kN * 4);
-                            tma_load_1d(buf, next, kN * 4, mbar);
-                        }
-                    }
                 }
             }
             // now X[lane + 32 k1] = v[bitrev(k1)]
@@ -387,16 +425,15 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
                     pk::c64 m = pk::make(sqrt_approx(p1), sqrt_approx(p2)); // (|X[k1]|, |X[k2]|), normalised via the window
                     if(EXTRA && p.slope != nullptr)
                         m = pk::mul(m, pk::make(__ldg(p.slope + k1), __ldg(p.slope + k2)));
-                    pk::c64 *sst64 = reinterpret_cast<pk::c64 *>(sst);
                     if(TSM)
                     {
-                        pk::c64 old = sst64[q * 32];
+                        pk::c64 old = st[q];
                         if(EXTRA && p.fast_peaks)
                             old = pk::make(fmaxf(pk::re(m), pk::re(old)), fmaxf(pk::im(m), pk::im(old)));
                         // g*old + g2*new with one fused rounding, as the reference's AVX2 path (src/source_avx2.cpp:154)
                         m = pk::fma(pk::make(gt.x, gt.x), old, pk::mul(pk::make(gt.y, gt.y), m));
                     }
-                    sst64[q * 32] = m;
+                    st[q] = m;
                     float d1, d2;
                     pk::split(dbfs2(pk::re(m), pk::im(m), p.db_min), d1, d2);
                     if(EXTRA)
@@ -419,8 +456,8 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
                     }
                     if(GATE)
                         outs &= !(d1 > p.floor_m10) & !(d2 > p.floor_m10);
-                    stg_stream(odb + k1, d1);
-                    stg_stream(odb + k2, d2);
+                    row[k1] = d1;
+                    row[k2] = d2;
                 }
                 last_from_state = true;
             }
@@ -429,10 +466,18 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
                 // ---- rare path: tick returned early (hold, src/source_generic.cpp:138-139) or the channel was
                 //      skipped while the tick went on (stale dB re-converted, SURVEY appendix A quirk) ----
                 // Previous outputs: the row of tick t-1, or (t == 0) the engine's m_decibels mirror — which the previous
-                // call may have left implicit (hold_lazy: it is dbfs(state), and the state is in shared memory).
+                // call may have left implicit (hold_lazy: it is dbfs(state), and the state is on chip).  The row of tick
+                // t-1 may still be in flight in a bulk store (this warp's, or the previous warp's before a hand-over).
                 const float *prev_db = (t > 0) ? (odb - B) : hold_s;
                 const bool from_state = (t == 0) && hold_lazy;
-#pragma unroll 1
+                if(t > 0)
+                {
+                    if(lane == 0)
+                        bulk_wait_written();
+                    __syncwarp();
+                }
+                // (unrolled: the state registers cannot be indexed at run time)
+#pragma unroll
                 for(int q = 0; q < 16; ++q)
                 {
                     const int k1 = lane + 32 * q;
@@ -440,8 +485,9 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
                     float o1, o2;
                     if(from_state)
                     {
-                        const float2 stv = sst[q * 32];
-                        pk::split(dbfs2(stv.x, stv.y, p.db_min), o1, o2);
+                        float s1, s2;
+                        pk::split(st[q], s1, s2);
+                        pk::split(dbfs2(s1, s2, p.db_min), o1, o2);
                     }
                     else
                     {
@@ -472,11 +518,16 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
                     if(k1 >= 1)
                         peak = fmaxf(peak, o1);
                     peak = fmaxf(peak, o2);
-                    odb[k1] = o1;
-                    odb[k2] = o2;
+                    row[k1] = o1;
+                    row[k2] = o2;
                 }
                 last_from_state = false;
             }
+            // the row leaves in one bulk store: the lanes' stores to it must be visible to the async proxy first
+            fence_proxy_async();
+            __syncwarp();
+            if(lane == 0)
+                bulk_store_1d(odb, row, B * 4);
             if(GATE && !last_silent)
                 prev_out_silent = __all_sync(0xffffffffu, outs);
             if(p.out_silent != nullptr && lane == 0)
@@ -495,7 +546,6 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
         // ---- state back to the engine; m_decibels mirror for the next call's gate / hold paths ----
         {
             float *sp = p.state + (size_t)s * B;
-            const float *last = p.out_db + ((size_t)s * T + (t1 - 1)) * B;
             const bool plain = !EXTRA || (!p.normalize && p.rolloff == nullptr);
             // The mirror equals dbfs(state) after a normal tick without volume / roll-off post-processing: do not spend
             // 4 KB of HBM writes per stream on it, set bit 3 instead (the engine materialises it on demand, see
@@ -506,7 +556,8 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
             {
                 const int k1 = lane + 32 * q;
                 const int k2 = (q == 0) ? k2_q0 : (kb + 32 * (31 - q));
-                const float2 stv = sst[q * 32];
+                float2 stv;
+                pk::split(st[q], stv.x, stv.y);
                 sp[k1] = stv.x;
                 sp[k2] = stv.y;
                 if(p.write_hold && !lazy)
@@ -520,8 +571,8 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
                     }
                     else
                     {
-                        hold_s[k1] = last[k1];
-                        hold_s[k2] = last[k2];
+                        hold_s[k1] = row[k1]; // the last tick's row, still staged (its bulk store only reads it)
+                        hold_s[k2] = row[k2];
                     }
                 }
             }
@@ -531,6 +582,8 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
         if(t1 < T)
         {
             // head segment: hand the stream to the next warp (state, flags, mirror and output rows are written)
+            if(lane == 0)
+                bulk_wait_written();
             __threadfence_block();
             __syncwarp();
             if(lane == 0)
@@ -538,6 +591,9 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
         }
         __syncwarp();
     }
+    // no bulk store may still read the staging row when the CTA's shared memory is released
+    if(lane == 0)
+        bulk_wait_written();
 }
 
 } // namespace wf

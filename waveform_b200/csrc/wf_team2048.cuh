@@ -25,7 +25,10 @@ namespace wf {
 namespace team {
 constexpr int kCtlBytes = 64;  // per team: nz[16] | outs[16] (bytes)
 constexpr int kWarps = 16;
-constexpr int smem_bytes() { return fast::kTableBytes + kWarps * fast::kWarpBytes + kWarps * kCtlBytes; }
+constexpr int kWarpBufBytes = 32 * 33 * 8;                  // padded transpose buffer, also the TMA landing zone
+constexpr int kMagBytes = 1024 * 4;                         // the warp's tick: linear magnitudes
+constexpr int kWarpBytes = kWarpBufBytes + kMagBytes + 16;  // + mbarrier
+constexpr int smem_bytes() { return fast::kTableBytes + kWarps * kWarpBytes + kWarps * kCtlBytes; }
 
 __device__ __forceinline__ void bar_sync(int id, int nthreads)
 {
@@ -51,11 +54,11 @@ __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(con
     const int tm = warp / W; // team within the CTA
     const int wi = warp % W; // warp within the team = tick within a round (phase 1) = bin slice (phase 2)
     unsigned char *warps_base = reinterpret_cast<unsigned char *>(s_twP + 512);
-    unsigned char *wbase = warps_base + warp * kWarpBytes;
+    unsigned char *wbase = warps_base + warp * team::kWarpBytes;
     float2 *buf = reinterpret_cast<float2 *>(wbase);
-    float *mymag = reinterpret_cast<float *>(wbase + kWarpBufBytes); // this warp's tick: linear magnitudes [1024]
-    uint64_t *mbar = reinterpret_cast<uint64_t *>(wbase + kWarpBufBytes + kStateBytes);
-    unsigned char *ctl = warps_base + team::kWarps * kWarpBytes + tm * team::kCtlBytes;
+    float *mymag = reinterpret_cast<float *>(wbase + team::kWarpBufBytes); // this warp's tick: linear magnitudes [1024]
+    uint64_t *mbar = reinterpret_cast<uint64_t *>(wbase + team::kWarpBufBytes + team::kMagBytes);
+    unsigned char *ctl = warps_base + team::kWarps * team::kWarpBytes + tm * team::kCtlBytes;
     volatile unsigned char *ctl_nz = ctl;         // [W] frame of tick t0+i has a non-zero sample
     volatile unsigned char *ctl_outs = ctl + 16;  // [W] per-warp partial of the gate's all-bins test
     const int bar_id = 1 + tm;
@@ -260,7 +263,7 @@ __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(con
                     {
                         const int tt = t0 + i;
                         const float2 gt = (EXTRA && p.g_tab != nullptr) ? __ldg(p.g_tab + tt) : make_float2(p.g, p.g2);
-                        const float *mg = reinterpret_cast<const float *>(warps_base + (size_t)(tm * W + i) * kWarpBytes + kWarpBufBytes) + b0;
+                        const float *mg = reinterpret_cast<const float *>(warps_base + (size_t)(tm * W + i) * team::kWarpBytes + team::kWarpBufBytes) + b0;
                         float d[BPL];
 #pragma unroll
                         for(int j = 0; j < BPL; j += VEC)
@@ -398,7 +401,7 @@ __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(con
                 float d[BPL];
                 if(do_proc && !last_silent)
                 {
-                    const float *mg = reinterpret_cast<const float *>(warps_base + (size_t)(tm * W + i) * kWarpBytes + kWarpBufBytes) + b0;
+                    const float *mg = reinterpret_cast<const float *>(warps_base + (size_t)(tm * W + i) * team::kWarpBytes + team::kWarpBufBytes) + b0;
 #pragma unroll
                     for(int j = 0; j < BPL; j += VEC)
                     {
