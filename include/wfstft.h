@@ -255,6 +255,14 @@ typedef struct wf_meter_config {
     float gravity;            /* m_gravity */
     int32_t fast_peaks;       /* m_fast_peaks */
     int32_t floor_db;         /* m_floor: a channel below floor-10 dB counts as silent */
+    /* display stage (render_bars in meter mode, src/source.cpp:1478-1498, :1505-1509, :1548-1558): m_meter_val -> bar height
+     * in pixels.  A caller built against the previous header (struct_size = offsetof(wf_meter_config, height)) has no display
+     * settings; its engine then rejects out_pixels / out_min. */
+    int32_t height;           /* m_height */
+    int32_t ceiling_db;       /* m_ceiling (with floor_db: ceiling - floor < 1 -> 0 / -120 for the display, src/source.cpp:573-577) */
+    int32_t bar_width;        /* m_bar_width: cap radius = bar_width / 2 */
+    int32_t rounded_caps;     /* m_rounded_caps */
+    int32_t min_bar_height;   /* m_min_bar_height */
 } wf_meter_config;
 
 typedef struct wf_meter_batch {
@@ -272,6 +280,11 @@ typedef struct wf_meter_batch {
     float *out_lin;           /* optional [n_streams][n_ticks][capture_channels] m_meter_buf;
                                  INPUT_RMS: [n_streams][n_ticks] m_input_rms (feed it to wf_batch.input_rms) */
     uint8_t *out_silent;      /* optional [n_streams][n_ticks] m_last_silent after the tick; unused for INPUT_RMS */
+    /* optional display outputs (PEAK / RMS only; WF_ERR_INVALID_ARG for INPUT_RMS or an engine without display settings):
+     * what render_bars leaves in m_interp_bufs[0] in meter mode, i.e. bar heights in pixels measured from the top,
+     * lerp(border_top, border_bottom, clamp(ceiling - m_meter_val, 0, range) / range) */
+    float *out_pixels;        /* [n_streams][n_ticks][capture_channels] */
+    float *out_min;           /* [n_streams][n_ticks][2]: (miny, minpos) — first strict minimum, starting from (height, 0) */
 } wf_meter_batch;
 
 typedef struct wf_meter wf_meter;
@@ -311,6 +324,17 @@ typedef struct wf_wave_config {
     int32_t normalize_volume; /* m_normalize_volume */
     float volume_target;      /* m_volume_target */
     float max_gain;           /* m_max_gain */
+    /* display stage (render_curve in waveform mode, src/source.cpp:1360-1427 with init_interp :842-846 and the settings forced
+     * at :1129-1143: linear axis over the whole buffer, no mirroring).  Same meaning and clamps as in wf_config.  A caller built
+     * against the previous header (struct_size = offsetof(wf_wave_config, interp_mode)) has no display settings; its engine
+     * then rejects out_points / out_pixels / out_min. */
+    int32_t interp_mode;      /* wf_interp, m_interp_mode */
+    int32_t filter_mode;      /* wf_filter, m_filter_mode */
+    float filter_radius;      /* m_filter_radius */
+    int32_t height;           /* m_height */
+    int32_t floor_db;         /* m_floor */
+    int32_t ceiling_db;       /* m_ceiling */
+    int32_t channel_spacing;  /* m_channel_spacing (zeroed unless stereo, src/source.cpp:579-580) */
 } wf_wave_config;
 
 typedef struct wf_wave_batch {
@@ -322,8 +346,14 @@ typedef struct wf_wave_batch {
     int64_t stream_stride;
     int64_t channel_stride;
     const float *input_rms;   /* optional [n_streams][n_ticks] m_input_rms per tick (volume normalisation) */
-    float *out;               /* [n_streams][n_ticks][display_channels][width] m_decibels after the tick (oldest point first) */
+    float *out;               /* [n_streams][n_ticks][display_channels][width] m_decibels after the tick (oldest point first);
+                                 optional when out_points or out_pixels is set */
     uint8_t *out_silent;      /* optional [n_streams][n_ticks] m_last_silent after the tick */
+    /* optional display outputs, what render_curve computes from the tick's m_decibels rows (WF_ERR_INVALID_ARG on an engine
+     * without display settings or with width < 2): */
+    float *out_points;        /* [n_streams][n_ticks][display_channels][width] interpolated (+ Gaussian-smoothed) dB */
+    float *out_pixels;        /* same shape: m_interp_bufs after the dB -> pixel lerp/clamp (height measured from the top) */
+    float *out_min;           /* [n_streams][n_ticks][2]: (miny, minpos), first strict minimum over both channels from (cpos, 0) */
 } wf_wave_batch;
 
 typedef struct wf_wave wf_wave;
@@ -343,6 +373,10 @@ int wf_wave_reset(wf_wave *w);
  * points or a negative status. */
 int64_t wf_wave_preview_plan(const wf_wave_config *cfg, int32_t n_ticks, int32_t hop, int32_t *counts, int32_t *src,
                              int64_t capacity);
+/* The display stage's setup tables of a waveform engine, computed from a config without a device (like wf_preview_table):
+ * WF_TABLE_INTERP_INDICES (m_interp_indices, width floats), WF_TABLE_INTERP_WEIGHTS (m_interp_kernel.weights, width * taps)
+ * and WF_TABLE_GAUSS (m_kernel.weights).  Returns the element count (0: table not used) or a negative status. */
+int64_t wf_wave_preview_table(const wf_wave_config *cfg, int which, float *out, int64_t capacity);
 int64_t wf_wave_launch_count(const wf_wave *w);
 float wf_wave_last_kernel_ms(wf_wave *w);
 

@@ -61,3 +61,22 @@ for st, ch, hop in (({"width": 300, "meter_buf": 50, "channel_mode": "stereo"}, 
     a = w.process(x[:, :, : 4 * hop], 4, hop); b = w.process(torch.from_numpy(x[:, :, 4 * hop:]).cuda(), T - 4, hop)
     torch.cuda.synchronize()
     print("wave", st["width"], ch, hop, "ok silent ticks:", int(b["silent"].sum()), flush=True)
+# display stages: the waveform's render_curve in both kernels (with the Gaussian's scratch row, display-only calls) and the
+# meter's render_bars on its fused and three-kernel paths
+import os
+for chunk in ("1", "0"):
+    os.environ["WF_WAVE_CHUNK"] = chunk
+    for st, ch, hop in (({"width": 301, "meter_buf": 40, "channel_mode": "stereo", "filter_mode": "gauss"}, 1, 97),
+                        ({"width": 200, "meter_buf": 10, "interp_mode": "lanczos"}, 2, 800)):
+        w = WaveEngine(st, channels=ch, max_streams=3)
+        x = synth_pcm(3, ch, 12 * hop)
+        a = w.process(x[:, :, : 4 * hop], 4, hop, want_points=True, want_pixels=True)
+        b = w.process(torch.from_numpy(x[:, :, 4 * hop:]).cuda(), 8, hop, want_db=False, want_pixels=True)
+        torch.cuda.synchronize()
+        print("wave display", chunk, st["width"], ch, hop, "ok", float(b["min"][..., 0].mean()), flush=True)
+os.environ.pop("WF_WAVE_CHUNK")
+for hop in (441, 480):
+    m = MeterEngine({"meter_buf": 20, "rounded_caps": True}, channels=2, max_streams=3)
+    x = synth_pcm(3, 2, 9 * hop)
+    a = m.process(x, 9, hop, want_pixels=True)
+    print("meter display", hop, "ok", float(a["pixels"].mean()), flush=True)

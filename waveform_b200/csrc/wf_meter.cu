@@ -20,12 +20,14 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <new>
 #include <string>
 
+#include "wf_display.cuh"
 #include "wf_nvtx.hpp"
 #include "wf_tables.hpp"
 #include "wfstft.h"
@@ -53,7 +55,33 @@ struct MParams {
     float g, g2;
     int tsmooth, fast_peaks;
     float floor_m10, db_min;
+    // display stage (render_bars in meter mode), or null outputs
+    float *out_pixels, *out_min;
+    float ceiling_f, dbrange_f, px_lo, px_hi, px_cpos;
 };
+
+// render_bars in meter mode (src/source.cpp:1505-1509, :1548-1557): the bar height of each capture channel from its
+// m_meter_val (val0, val1 for c < cc) and the first strict minimum starting from (cpos, 0); `st` = s * n_ticks + t
+__device__ __forceinline__ void meter_pixels(const MParams &p, size_t st, float val0, float val1, int cc)
+{
+    float miny = p.px_cpos, minpos = 0.0f;
+    for(int c = 0; c < cc; ++c)
+    {
+        const float v = wf::display_pixel(c ? val1 : val0, p.ceiling_f, p.dbrange_f, p.px_lo, p.px_hi);
+        if(p.out_pixels)
+            p.out_pixels[st * cc + c] = v;
+        if(v < miny)
+        {
+            miny = v;
+            minpos = (float)c;
+        }
+    }
+    if(p.out_min)
+    {
+        p.out_min[2 * st] = miny;
+        p.out_min[2 * st + 1] = minpos;
+    }
+}
 
 // Row pointers of one (stream, channel): history ring first (timeline positions [0, W)), then this call's PCM.
 struct Row {
@@ -264,6 +292,7 @@ __global__ void meter_scan_kernel(const MParams p)
     for(int t = 0; t < p.n_ticks; ++t)
     {
         int silent_channels = 0;
+        float val0 = 0.0f, val1 = 0.0f;
         for(int c = 0; c < p.cc; ++c)
         {
             float out = p.raw[((size_t)s * p.n_ticks + t) * p.pc + c];
@@ -278,6 +307,7 @@ __global__ void meter_scan_kernel(const MParams p)
             const float val = (out > 0.0f) ? 20.0f * log10f(out) : p.db_min; // dbfs, src/source.hpp:293-299
             if(val < p.floor_m10)
                 ++silent_channels;
+            (c ? val1 : val0) = val;
             const size_t o = ((size_t)s * p.n_ticks + t) * p.cc + c;
             if(p.out_db)
                 p.out_db[o] = val;
@@ -285,6 +315,8 @@ __global__ void meter_scan_kernel(const MParams p)
                 p.out_lin[o] = out;
         }
         last_silent = silent_channels >= p.cc; // :264-269
+        if(p.out_pixels || p.out_min)
+            meter_pixels(p, (size_t)s * p.n_ticks + t, val0, val1, p.cc);
         if(p.out_silent)
             p.out_silent[(size_t)s * p.n_ticks + t] = last_silent ? 1 : 0;
     }
@@ -418,11 +450,13 @@ __global__ void __launch_bounds__(256) meter_fused_kernel(const MParams p)
     for(int t = threadIdx.x; t < T; t += blockDim.x)
     {
         int below = 0;
+        float val0 = 0.0f, val1 = 0.0f;
         for(int c = 0; c < cc; ++c)
         {
             const float out = raw[t * pc + c];
             const float val = (out > 0.0f) ? 20.0f * log10f(out) : p.db_min; // dbfs, src/source.hpp:293-299
             below += (val < p.floor_m10) ? 1 : 0;
+            (c ? val1 : val0) = val;
             const size_t o = ((size_t)s * T + t) * cc + c;
             if(p.out_db)
                 p.out_db[o] = val;
@@ -430,6 +464,8 @@ __global__ void __launch_bounds__(256) meter_fused_kernel(const MParams p)
                 p.out_lin[o] = out;
         }
         const bool silent = below >= cc; // :264-269
+        if(p.out_pixels || p.out_min)
+            meter_pixels(p, (size_t)s * T + t, val0, val1, cc);
         if(p.out_silent)
             p.out_silent[(size_t)s * T + t] = silent ? 1 : 0;
         if(t == T - 1)
@@ -487,6 +523,11 @@ struct wf_meter {
     float *d_partial = nullptr, *d_raw = nullptr, *s_pcm = nullptr, *s_db = nullptr, *s_lin = nullptr;
     unsigned char *s_silent = nullptr;
     size_t partial_cap = 0, raw_cap = 0, pcm_cap = 0, db_cap = 0, lin_cap = 0, silent_cap = 0;
+    // display stage: only when the config carried display settings (current struct size)
+    bool display = false;
+    float ceiling_f = 0.0f, dbrange_f = 1.0f, px_lo = 0.0f, px_hi = 0.0f, px_cpos = 0.0f;
+    float *s_pixels = nullptr, *s_min = nullptr;
+    size_t pixels_cap = 0, min_cap = 0;
 };
 
 namespace {
@@ -567,17 +608,31 @@ void wf_meter_config_init(wf_meter_config *c)
     c->gravity = 0.65f;
     c->fast_peaks = 0;
     c->floor_db = -65;
+    c->height = 225;
+    c->ceiling_db = 0;
+    c->bar_width = 24;
+    c->rounded_caps = 0;
+    c->min_bar_height = 0;
 }
 
 const char *wf_meter_last_error(const wf_meter *m) { return m ? m->last_error.c_str() : g_meter_create_error.c_str(); }
 
-int wf_meter_create(const wf_meter_config *cfg, wf_meter **out)
+int wf_meter_create(const wf_meter_config *cfg_in, wf_meter **out)
 {
-    if(!cfg || !out)
+    if(!cfg_in || !out)
         return WF_ERR_INVALID_ARG;
     *out = nullptr;
-    if(cfg->struct_size != sizeof(wf_meter_config))
+    // the current struct or the previous one, which ends before height: its display settings are absent
+    wf_meter_config cfg_v{};
+    if(cfg_in->struct_size == sizeof(wf_meter_config))
+        cfg_v = *cfg_in;
+    else if(cfg_in->struct_size == offsetof(wf_meter_config, height))
+        memcpy(&cfg_v, cfg_in, offsetof(wf_meter_config, height));
+    else
         return merr(nullptr, WF_ERR_ABI, "wf_meter_config.struct_size mismatch");
+    const bool display_settings = cfg_in->struct_size == sizeof(wf_meter_config);
+    cfg_v.struct_size = (uint32_t)sizeof(wf_meter_config);
+    const wf_meter_config *cfg = &cfg_v;
     if(cfg->capture_channels < 1 || cfg->capture_channels > 2 || cfg->max_streams < 1 || cfg->sample_rate < 16 ||
        cfg->mode < WF_METER_PEAK || cfg->mode > WF_METER_INPUT_RMS)
         return merr(nullptr, WF_ERR_INVALID_ARG, "bad meter config");
@@ -607,6 +662,30 @@ int wf_meter_create(const wf_meter_config *cfg, wf_meter **out)
     m->W = W;
     m->pc = (cfg->mode == WF_METER_INPUT_RMS) ? 1 : cfg->capture_channels;
     m->db_min = 20.0f * log10f(1.17549435e-38f); // DB_MIN, src/source.cpp:43
+    m->display = display_settings && cfg->mode != WF_METER_INPUT_RMS;
+    if(m->display)
+    {
+        // render_bars geometry in meter mode (src/source.cpp:1481-1494; m_stereo is forced off, :1115, so cpos = height and
+        // the channel spacing is 0) after the get_settings clamps (:573-577) and m_cap_radius = bar_width / 2 (:1297)
+        int ceiling = cfg->ceiling_db, floor = cfg->floor_db;
+        if((ceiling - floor) < 1)
+        {
+            ceiling = 0;
+            floor = -120;
+        }
+        const float cpos = (float)(cfg->height < 1 ? 225 : cfg->height);
+        const float cap_radius = (float)cfg->bar_width / 2.0f;
+        const float border_top = cfg->rounded_caps ? cap_radius : 0.0f;
+        float border_bottom = cfg->rounded_caps ? cpos - cap_radius : cpos;
+        if(cfg->min_bar_height > 0)
+            border_bottom -= cfg->min_bar_height;
+        border_bottom = std::clamp(border_bottom, border_top, cpos);
+        m->ceiling_f = (float)ceiling;
+        m->dbrange_f = (float)(ceiling - floor);
+        m->px_lo = border_top;
+        m->px_hi = border_bottom;
+        m->px_cpos = cpos;
+    }
     auto bail = [&](int code) {
         g_meter_create_error = m->last_error;
         wf_meter_destroy(m);
@@ -662,7 +741,7 @@ void wf_meter_destroy(wf_meter *m)
         cudaStreamSynchronize(m->stream);
     }
     void *ptrs[] = {m->d_part[0], m->d_part[1], m->d_hist[0], m->d_hist[1], m->d_buf, m->d_flags, m->d_partial, m->d_raw,
-                    m->s_pcm, m->s_db, m->s_lin, m->s_silent};
+                    m->s_pcm, m->s_db, m->s_lin, m->s_silent, m->s_pixels, m->s_min};
     for(void *q : ptrs)
         if(q)
             cudaFree(q);
@@ -677,13 +756,24 @@ void wf_meter_destroy(wf_meter *m)
 
 int32_t wf_meter_window(const wf_meter *m) { return m ? m->W : 0; }
 
-int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b, void *cuda_stream)
+int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b_in, void *cuda_stream)
 {
-    if(!m || !b)
+    if(!m || !b_in)
         return WF_ERR_INVALID_ARG;
     wf::NvtxRange nvtx("wf_meter_process");
-    if(b->struct_size != sizeof(wf_meter_batch))
-        return merr(m, WF_ERR_ABI, "wf_meter_batch.struct_size %u != %zu", b->struct_size, sizeof(wf_meter_batch));
+    // the current struct or the previous one (which ends before out_pixels: no display outputs)
+    wf_meter_batch bv{};
+    if(b_in->struct_size == sizeof(wf_meter_batch))
+        bv = *b_in;
+    else if(b_in->struct_size == offsetof(wf_meter_batch, out_pixels))
+        memcpy(&bv, b_in, offsetof(wf_meter_batch, out_pixels));
+    else
+        return merr(m, WF_ERR_ABI, "wf_meter_batch.struct_size %u != %zu", b_in->struct_size, sizeof(wf_meter_batch));
+    const wf_meter_batch *b = &bv;
+    if((b->out_pixels || b->out_min) && !m->display)
+        return merr(m, WF_ERR_INVALID_ARG, (m->cfg.mode == WF_METER_INPUT_RMS)
+                                               ? "display outputs do not exist for the RMS feed (INPUT_RMS)"
+                                               : "display outputs need an engine created with display settings");
     if(b->n_streams < 0 || b->n_ticks < 0 || b->hop < 1)
         return merr(m, WF_ERR_INVALID_ARG, "n_streams/n_ticks must be >= 0 and hop >= 1");
     if(b->first_stream < 0 || (int64_t)b->first_stream + b->n_streams > m->cfg.max_streams)
@@ -723,7 +813,7 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b, void *cuda_stre
     if((rc = mensure(m, &m->d_raw, &m->raw_cap, S * T * pc)))
         return rc;
     const float *d_pcm = b->pcm;
-    float *d_db = b->out_db, *d_lin = b->out_lin;
+    float *d_db = b->out_db, *d_lin = b->out_lin, *d_pixels = b->out_pixels, *d_min = b->out_min;
     unsigned char *d_silent = b->out_silent;
     if(!dev_ptrs)
     {
@@ -750,6 +840,18 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b, void *cuda_stre
             if((rc = mensure(m, &m->s_silent, &m->silent_cap, S * T)))
                 return rc;
             d_silent = m->s_silent;
+        }
+        if(b->out_pixels)
+        {
+            if((rc = mensure(m, &m->s_pixels, &m->pixels_cap, out_n)))
+                return rc;
+            d_pixels = m->s_pixels;
+        }
+        if(b->out_min)
+        {
+            if((rc = mensure(m, &m->s_min, &m->min_cap, S * T * 2)))
+                return rc;
+            d_min = m->s_min;
         }
     }
 
@@ -788,6 +890,13 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b, void *cuda_stre
     p.fast_peaks = m->cfg.fast_peaks;
     p.floor_m10 = (float)(m->cfg.floor_db - 10);
     p.db_min = m->db_min;
+    p.out_pixels = d_pixels;
+    p.out_min = d_min;
+    p.ceiling_f = m->ceiling_f;
+    p.dbrange_f = m->dbrange_f;
+    p.px_lo = m->px_lo;
+    p.px_hi = m->px_hi;
+    p.px_cpos = m->px_cpos;
 
     WFM_CUDA(m, cudaEventRecord(m->ev0, st));
     constexpr int kWarps = 8;
@@ -885,6 +994,10 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b, void *cuda_stre
             WFM_CUDA(m, cudaMemcpyAsync(b->out_lin, d_lin, out_n * sizeof(float), cudaMemcpyDeviceToHost, st));
         if(b->out_silent && !is_feed)
             WFM_CUDA(m, cudaMemcpyAsync(b->out_silent, d_silent, S * T, cudaMemcpyDeviceToHost, st));
+        if(b->out_pixels)
+            WFM_CUDA(m, cudaMemcpyAsync(b->out_pixels, d_pixels, out_n * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if(b->out_min)
+            WFM_CUDA(m, cudaMemcpyAsync(b->out_min, d_min, S * T * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
     }
     return WF_OK;
 }

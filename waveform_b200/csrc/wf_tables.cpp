@@ -410,4 +410,64 @@ int build_tables(const wf_config &cfg_in, Tables &t, const char **why)
     return WF_OK;
 }
 
+int build_wave_tables(const wf_wave_config &w, Tables &t, const char **why)
+{
+    t = Tables{};
+    auto fail = [&](const char *msg) {
+        if(why)
+            *why = msg;
+        return (int)WF_ERR_INVALID_ARG;
+    };
+    if(w.width < 2)
+        return fail("the waveform display stage needs width >= 2");
+    if(w.interp_mode < WF_INTERP_POINT || w.interp_mode > WF_INTERP_CATROM)
+        return fail("unknown interp_mode");
+    auto &c = t.cfg;
+    c.display_mode = WF_DISPLAY_CURVE;
+    c.width = w.width;
+    c.stereo = w.stereo ? 1 : 0;
+    c.interp_mode = w.interp_mode;
+    c.filter_mode = w.filter_mode;
+    c.filter_radius = w.filter_radius;
+    c.height = w.height;
+    c.floor_db = w.floor_db;
+    c.ceiling_db = w.ceiling_db;
+    c.channel_spacing = w.channel_spacing;
+    // get_settings clamps, src/source.cpp:573-580
+    if((c.ceiling_db - c.floor_db) < 1)
+    {
+        c.ceiling_db = 0;
+        c.floor_db = -120;
+    }
+    if(c.height < 1)
+        c.height = 225;
+    if(!c.stereo || (c.height - c.channel_spacing) < 1)
+        c.channel_spacing = 0;
+
+    t.N = c.width; // m_fft_size := m_width, src/source.cpp:1140
+    t.num_points = c.width;
+    t.display_channels = c.stereo ? 2 : 1;
+    t.db_min = 20.0f * std::log10(std::numeric_limits<float>::min());
+
+    // init_interp(m_width), src/source.cpp:842-846 and :859-863 (m_log_scale and m_mirror_freq_axis forced off, :1136-1137)
+    const unsigned sz = (unsigned)c.width;
+    const float lowbin = 0.0f, highbin = (float)(sz - 1);
+    t.interp_indices.resize(sz);
+    for(auto i = 0u; i < sz; ++i)
+        t.interp_indices[i] = std::clamp(std_lerp(lowbin, highbin, (float)i / (float)(sz - 1)), lowbin, highbin);
+    t.interp_weights.clear();
+    if(c.interp_mode == WF_INTERP_LANCZOS)
+        build_lanczos(t, 4);
+    else if(c.interp_mode == WF_INTERP_CATROM)
+        build_catrom(t, 0.5f);
+    build_gauss(t);
+
+    // render_curve geometry, src/source.cpp:1368-1373, 1410
+    const auto cpos = c.stereo ? (float)c.height / 2 : (float)c.height;
+    t.px_cpos = cpos;
+    t.px_lo = 0.0f;
+    t.px_hi = cpos - c.channel_spacing * 0.5f;
+    return WF_OK;
+}
+
 } // namespace wf

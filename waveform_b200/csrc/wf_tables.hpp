@@ -50,6 +50,12 @@ struct Tables {
 // Applies the get_settings clamps and builds every table.  Returns WF_OK or WF_ERR_INVALID_ARG.
 int build_tables(const wf_config &cfg, Tables &out, const char **why);
 
+// The display stage of the waveform mode: init_interp for DisplayMode::WAVEFORM (src/source.cpp:842-846: linear axis over
+// bins [0, width - 1], no mirroring, settings forced at :1129-1143), the interpolation kernel and Gaussian of the spectrum
+// path's builders, and render_curve's geometry (px_lo = 0, px_hi = cpos - channel_offset, px_cpos).  The get_settings clamps
+// of the display settings (floor / ceiling, channel spacing, height) land in out.cfg; N = num_points = width.
+int build_wave_tables(const wf_wave_config &cfg, Tables &out, const char **why);
+
 float gravity_for(const wf_config &cfg, float seconds); // WAVSource::get_gravity, src/source.hpp:301-312
 float std_lerp(float a, float b, float t);              // std::lerp as libstdc++ evaluates it
 

@@ -16,15 +16,19 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdarg>
+#include <cstddef>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <new>
 #include <string>
+#include <type_traits>
 #include <vector>
 
+#include "wf_display.cuh"
 #include "wf_nvtx.hpp"
+#include "wf_tables.hpp"
 #include "wfstft.h"
 
 namespace {
@@ -42,13 +46,255 @@ struct WParams {
     int n_streams, n_ticks, width, cc, dch, och, stereo, normalize;
     float vol_target, max_gain, db_min;
 };
+// The parameters of the kernels with the display stage (the plain kernels keep WParams, and with it their code):
+// tables of wf::build_wave_tables, the display outputs, render_curve's geometry.
+struct WDisp : WParams {
+    const float *interp_w;    // [width][taps] or null (point mode); 16-byte aligned
+    const float *interp_idx;  // [width]
+    const float *gauss_w;     // [2 * gauss_radius - 1] or null
+    float *out_points;        // [streams][ticks][dch][width] or null
+    float *out_pixels;        // same shape or null
+    float *out_min;           // [streams][ticks][2] or null
+    int taps, filter, gauss_radius, scratch_off; // scratch_off: floats of dynamic shared memory before the Gaussian's scratch row
+    int vec4;                 // width % 4 == 0 and 16-byte aligned display outputs: float4 stores
+    float gauss_sum, ceiling_f, dbrange_f, px_hi, px_cpos;
+};
 
 __device__ __forceinline__ float dbfs_dev(float mag, float db_min) { return (mag > 0.0f) ? 20.0f * log10f(mag) : db_min; }
 
-// One CTA per stream; the scrolling buffers live in shared memory as rings (head = oldest point).
-__global__ void __launch_bounds__(256) wave_kernel(const WParams p)
+// ---- display stage: render_curve in waveform mode (src/source.cpp:1375-1417) for the rows of one or more ticks ---------------
+// The operation order is the spectrum path's display_stage_tab / kernel_sum / weighted_avg (wf_kernels.cuh), which are pinned
+// against the reference; restated here because a waveform row is a window of a ring in shared memory, not a contiguous array.
+
+// One display row: element k is a[(a0 + k) mod cap] for k < split and b[k] from there on (the one-channel-shown-as-two layout's
+// second row: older points from the dB ring, the tick's own points raw); a silent row is DB_MIN throughout.  Built once per
+// (tick, channel, point group), so the taps only add k.
+struct RowSeg {
+    const float *a, *b;
+    int a0, cap, split;
+    bool sil;
+    float fill;
+    __device__ __forceinline__ float operator()(int k) const
+    {
+        if(sil)
+            return fill;
+        if(k < split)
+        {
+            const int x = a0 + k;
+            return a[x - ((x >= cap) ? cap : 0)];
+        }
+        return b[k];
+    }
+};
+
+// interpolated dB of display point i.  TAPS 0: point mode, the sample at (int)m_interp_indices[i] (:1393-1394; std::lerp puts
+// some indices just below an integer, so that is sample i - 1 there).  TAPS 4 / 8: Catmull-Rom / Lanczos, kernel_convolve
+// (src/filter.hpp:160-169): taps outside [0, width) are skipped, the rest summed in tap order; the weights come in 128-bit loads
+// (the table is 16-byte aligned and a point has 4 or 8 of them).
+template<int TAPS>
+__device__ __forceinline__ float wave_interp(const WDisp &p, const RowSeg &row, int i)
 {
-    extern __shared__ float ring[]; // [2][width]
+    const int index = (int)__ldg(p.interp_idx + i);
+    if constexpr(TAPS == 0)
+        return row(index);
+    else
+    {
+        float wt[TAPS];
+        const float4 *w4 = reinterpret_cast<const float4 *>(p.interp_w) + (size_t)i * (TAPS / 4);
+#pragma unroll
+        for(int q = 0; q < TAPS / 4; ++q)
+        {
+            const float4 v = __ldg(w4 + q);
+            wt[4 * q] = v.x;
+            wt[4 * q + 1] = v.y;
+            wt[4 * q + 2] = v.z;
+            wt[4 * q + 3] = v.w;
+        }
+        const int start = index - TAPS / 2 + 1;
+        float sum = 0.0f;
+#pragma unroll
+        for(int k = 0; k < TAPS; ++k)
+        {
+            const int j = start + k;
+            if((unsigned)j < (unsigned)p.width)
+                sum = __fadd_rn(sum, __fmul_rn(row(j), wt[k]));
+        }
+        return sum;
+    }
+}
+
+// weighted_avg (src/filter.hpp:133-158): the Gaussian, renormalised where it overhangs the row's ends
+__device__ __forceinline__ float wave_gauss(const WDisp &p, const float *raw, int i)
+{
+    const int n = p.width, start = (i - p.gauss_radius) + 1, stop = i + p.gauss_radius;
+    float sum = 0.0f;
+    if((start < 0) || (stop > n))
+    {
+        float wsum = 0.0f;
+        for(int k = max(start, 0); k < min(stop, n); ++k)
+        {
+            const float weight = __ldg(p.gauss_w + (k - start));
+            wsum = __fadd_rn(wsum, weight);
+            sum = __fadd_rn(sum, __fmul_rn(raw[k], weight));
+        }
+        return __fdiv_rn(sum, wsum);
+    }
+    for(int k = start; k < stop; ++k)
+        sum = __fadd_rn(sum, __fmul_rn(raw[k], __ldg(p.gauss_w + (k - start))));
+    return __fdiv_rn(sum, p.gauss_sum);
+}
+
+// stores points [i, i + V) of display channel d of tick t (one float4 per output when V = 4) and returns their arg-min key:
+// pixel heights are >= +0, so the float's bits order like the value, and the low word (channel, index) makes ties go to the
+// earliest point, as the sequential scan does
+template<int V>
+__device__ __forceinline__ unsigned long long wave_emit(const WDisp &p, int s, int t, int d, int i, const float (&db)[V])
+{
+    const size_t o = (((size_t)s * p.n_ticks + t) * p.dch + d) * p.width + i;
+    float px[V];
+    unsigned long long key = ~0ull;
+#pragma unroll
+    for(int u = 0; u < V; ++u)
+    {
+        px[u] = wf::display_pixel(db[u], p.ceiling_f, p.dbrange_f, 0.0f, p.px_hi);
+        key = min(key, ((unsigned long long)__float_as_uint(px[u]) << 32) | (unsigned)(d * p.width + i + u));
+    }
+    if constexpr(V == 4)
+    {
+        if(p.out_points != nullptr)
+            __stcs(reinterpret_cast<float4 *>(p.out_points + o), make_float4(db[0], db[1], db[2], db[3]));
+        if(p.out_pixels != nullptr)
+            __stcs(reinterpret_cast<float4 *>(p.out_pixels + o), make_float4(px[0], px[1], px[2], px[3]));
+    }
+    else
+    {
+        if(p.out_points != nullptr)
+            __stcs(p.out_points + o, db[0]);
+        if(p.out_pixels != nullptr)
+            __stcs(p.out_pixels + o, px[0]);
+    }
+    return key;
+}
+
+// Without the Gaussian: every (tick, channel, group of V points) of ticks [t0, t0 + K) at once.  A thread's items come in tick
+// order (the item index walks by nt; no division per item), so it folds its keys per tick before the shared atomic.
+template<int TAPS, int V, class Seg>
+__device__ __forceinline__ void wave_display_points(const WDisp &p, const Seg &seg, int s, int t0, int K,
+                                                    unsigned long long *s_min, int tid, int nt)
+{
+    const int Wv = p.width / V, per = p.dch * Wv;
+    int j = tid / per, r = tid - j * per, jc = -1;
+    unsigned long long key = ~0ull;
+    while(j < K)
+    {
+        const int d = (r >= Wv) ? 1 : 0, i = (r - d * Wv) * V;
+        if(j != jc)
+        {
+            if(jc >= 0)
+                atomicMin(&s_min[jc], key);
+            jc = j;
+            key = ~0ull;
+        }
+        const RowSeg row = seg(j, d);
+        float v[V];
+#pragma unroll
+        for(int u = 0; u < V; ++u)
+            v[u] = wave_interp<TAPS>(p, row, i + u);
+        key = min(key, wave_emit<V>(p, s, t0 + j, d, i, v));
+        r += nt;
+        while(r >= per)
+        {
+            r -= per;
+            ++j;
+        }
+    }
+    if(jc >= 0)
+        atomicMin(&s_min[jc], key);
+}
+
+// With the Gaussian: one tick at a time through the scratch row(s) (the Gaussian reads its neighbours' interpolated values).
+template<int TAPS, class Seg>
+__device__ __forceinline__ void wave_display_gauss(const WDisp &p, const Seg &seg, int s, int t0, int K, float *scratch,
+                                                   unsigned long long *s_min, int tid, int nt)
+{
+    const int W = p.width, per = p.dch * W;
+    for(int j = 0; j < K; ++j)
+    {
+        __syncthreads(); // the previous tick's scratch reads are done
+        for(int r = tid; r < per; r += nt)
+        {
+            const int d = (r >= W) ? 1 : 0;
+            scratch[r] = wave_interp<TAPS>(p, seg(j, d), r - d * W);
+        }
+        __syncthreads();
+        unsigned long long key = ~0ull;
+        for(int r = tid; r < per; r += nt)
+        {
+            const int d = (r >= W) ? 1 : 0, i = r - d * W;
+            const float v[1] = {wave_gauss(p, scratch + d * W, i)};
+            key = min(key, wave_emit<1>(p, s, t0 + j, d, i, v));
+        }
+        if(key != ~0ull)
+            atomicMin(&s_min[j], key);
+    }
+}
+
+// The display stage of ticks [t0, t0 + K) of stream s, K <= WCH_KMAX; seg(j, d) is the RowSeg of display channel d of tick
+// t0 + j.  Called by all threads of the CTA; s_min: K keys of shared memory; scratch: dch * width floats (Gaussian only).
+template<class Seg>
+__device__ __forceinline__ void wave_display(const WDisp &p, const Seg &seg, int s, int t0, int K, float *scratch,
+                                             unsigned long long *s_min, int tid, int nt)
+{
+    if(tid < K)
+        s_min[tid] = ~0ull;
+    __syncthreads();
+    if(p.filter)
+    {
+        if(p.taps == 0)
+            wave_display_gauss<0>(p, seg, s, t0, K, scratch, s_min, tid, nt);
+        else if(p.taps == 4)
+            wave_display_gauss<4>(p, seg, s, t0, K, scratch, s_min, tid, nt);
+        else
+            wave_display_gauss<8>(p, seg, s, t0, K, scratch, s_min, tid, nt);
+    }
+    else if(p.vec4)
+    {
+        if(p.taps == 0)
+            wave_display_points<0, 4>(p, seg, s, t0, K, s_min, tid, nt);
+        else if(p.taps == 4)
+            wave_display_points<4, 4>(p, seg, s, t0, K, s_min, tid, nt);
+        else
+            wave_display_points<8, 4>(p, seg, s, t0, K, s_min, tid, nt);
+    }
+    else
+    {
+        if(p.taps == 0)
+            wave_display_points<0, 1>(p, seg, s, t0, K, s_min, tid, nt);
+        else if(p.taps == 4)
+            wave_display_points<4, 1>(p, seg, s, t0, K, s_min, tid, nt);
+        else
+            wave_display_points<8, 1>(p, seg, s, t0, K, s_min, tid, nt);
+    }
+    __syncthreads();
+    if(p.out_min != nullptr && tid < K)
+    {
+        // miny starts at cpos and only a strictly smaller value replaces it; minpos is the index within its channel
+        const unsigned long long key = s_min[tid];
+        const float v = __uint_as_float((unsigned)(key >> 32));
+        const bool lt = v < p.px_cpos;
+        float *o = p.out_min + ((size_t)s * p.n_ticks + t0 + tid) * 2;
+        o[0] = lt ? v : p.px_cpos;
+        o[1] = lt ? (float)((int)(key & 0xffffffffu) % p.width) : 0.0f;
+    }
+}
+
+// One CTA per stream; the scrolling buffers live in shared memory as rings (head = oldest point).  DISP: with the display
+// stage after every tick (out may then be null).
+template<class P>
+__global__ void __launch_bounds__(256, std::is_same_v<P, WDisp> ? 4 : 0) wave_kernel(const P p)
+{
+    constexpr bool DISP = std::is_same_v<P, WDisp>;
+    extern __shared__ float ring[]; // [2][width] (DISP with the Gaussian: then the scratch row(s))
     const int W = p.width, tid = threadIdx.x, nt = blockDim.x;
     for(int s = blockIdx.x; s < p.n_streams; s += gridDim.x)
     {
@@ -148,16 +394,27 @@ __global__ void __launch_bounds__(256) wave_kernel(const WParams p)
             }
             __syncthreads();
             // the tick's row(s): buffer in time order
-            float *orow = p.out + ((size_t)s * p.n_ticks + t) * p.dch * W;
-            for(int d = 0; d < p.dch; ++d)
-                for(int i = tid; i < W; i += nt)
-                {
-                    int pos = head + i;
-                    pos -= (pos >= W) ? W : 0;
-                    __stcs(orow + d * W + i, ring[d * W + pos]);
-                }
+            if(!DISP || p.out != nullptr)
+            {
+                float *orow = p.out + ((size_t)s * p.n_ticks + t) * p.dch * W;
+                for(int d = 0; d < p.dch; ++d)
+                    for(int i = tid; i < W; i += nt)
+                    {
+                        int pos = head + i;
+                        pos -= (pos >= W) ? W : 0;
+                        __stcs(orow + d * W + i, ring[d * W + pos]);
+                    }
+            }
             if(p.out_silent != nullptr && tid == 0)
                 p.out_silent[(size_t)s * p.n_ticks + t] = last_silent ? 1 : 0;
+            if constexpr(DISP)
+            {
+                __shared__ unsigned long long s_min[1];
+                const int hd = head;
+                wave_display(
+                    p, [&](int, int d) { return RowSeg{ring + d * W, ring, hd, W, W, false, 0.0f}; }, s, t, 1,
+                    ring + p.scratch_off, s_min, tid, nt);
+            }
             __syncthreads();
         }
         for(int i = tid; i < 2 * W; i += nt)
@@ -196,9 +453,12 @@ struct WChunkTick {
 
 __device__ __forceinline__ int wrap2(int x, int cap) { return x - ((x >= cap) ? cap : 0); }
 
-template<int MODE>
-__global__ void __launch_bounds__(256, 5) wave_chunk_kernel(const WParams p)
+// DISP: the display stage runs over the rows of every chunk after they are stored (out may then be null).  Its instantiations
+// get 64 registers (4 CTAs per SM) instead of 48: the plain ones keep their budget.
+template<int MODE, class P>
+__global__ void __launch_bounds__(256, std::is_same_v<P, WDisp> ? 4 : 5) wave_chunk_kernel(const P p)
 {
+    constexpr bool DISP = std::is_same_v<P, WDisp>;
     extern __shared__ float wsm[];
     __shared__ WChunkTick s_cnt[2][WCH_KMAX];
     __shared__ int s_off[WCH_KMAX + 1];
@@ -421,7 +681,9 @@ __global__ void __launch_bounds__(256, 5) wave_chunk_kernel(const WParams p)
                 if(TWO)
                     wc1 += __shfl_sync(0xffffffffu, s1, Kc - 1);
             }
-            // rows of ticks [t, t+Kc): windows of E in time order
+            // rows of ticks [t, t+Kc): windows of E in time order (without `out`, MODE 3 still walks them for the state row)
+            const bool wr_out = !DISP || p.out != nullptr;
+            if(wr_out || MODE == 3)
             {
                 const bool wr_state1 = (MODE == 3) && (t + Kc == p.n_ticks);
                 if(vec)
@@ -463,7 +725,8 @@ __global__ void __launch_bounds__(256, 5) wave_chunk_kernel(const WParams p)
                             }
                         }
                         const float4 v = make_float4(e[0], e[1], e[2], e[3]);
-                        __stcs(reinterpret_cast<float4 *>(p.out + (((size_t)s * p.n_ticks + t + j) * DCH + d) * W + i), v);
+                        if(wr_out)
+                            __stcs(reinterpret_cast<float4 *>(p.out + (((size_t)s * p.n_ticks + t + j) * DCH + d) * W + i), v);
                         if(wr_state1 && d == 1 && j == Kc - 1)
                             *reinterpret_cast<float4 *>(st1 + i) = v;
                     }
@@ -473,7 +736,8 @@ __global__ void __launch_bounds__(256, 5) wave_chunk_kernel(const WParams p)
                         float4 *orow = reinterpret_cast<float4 *>(p.out + ((size_t)s * p.n_ticks + t + Kc - 1) * DCH * W);
                         for(int it = tid; it < per; it += nt)
                         {
-                            __stcs(orow + it, v);
+                            if(wr_out)
+                                __stcs(orow + it, v);
                             if(wr_state1 && it >= W4)
                                 reinterpret_cast<float4 *>(st1)[it - W4] = v;
                         }
@@ -495,13 +759,32 @@ __global__ void __launch_bounds__(256, 5) wave_chunk_kernel(const WParams p)
                             else
                                 v = ((d == 0) ? E0 : E1)[wrap2(base + rel, CAP)];
                         }
-                        __stcs(p.out + (((size_t)s * p.n_ticks + t + j) * DCH + d) * W + i, v);
+                        if(wr_out)
+                            __stcs(p.out + (((size_t)s * p.n_ticks + t + j) * DCH + d) * W + i, v);
                         if(wr_state1 && d == 1 && j == Kc - 1)
                             st1[i] = v;
                     }
                 }
+                if(!DISP && p.out_silent != nullptr && tid < Kc)
+                    p.out_silent[(size_t)s * p.n_ticks + t + tid] = (hit && tid == Kc - 1) ? 1 : 0;
+            }
+            if constexpr(DISP)
+            {
                 if(p.out_silent != nullptr && tid < Kc)
                     p.out_silent[(size_t)s * p.n_ticks + t + tid] = (hit && tid == Kc - 1) ? 1 : 0;
+                // the same windows of E (the silent row, at most the last one, is DB_MIN in the display channels)
+                __shared__ unsigned long long s_min[WCH_KMAX];
+                const int b0 = base, silent_j = hit ? Kc - 1 : -1;
+                wave_display(
+                    p,
+                    [&](int j, int d) {
+                        const int o1 = s_off[j + 1];
+                        const float *a = (DCH == 2 && MODE != 3 && d == 1) ? E1 : E0;
+                        if(MODE == 3 && d == 1)
+                            return RowSeg{a, N0 + (o1 - W), wrap2(b0 + o1, CAP), CAP, W + s_off[j] - o1, j == silent_j, p.db_min};
+                        return RowSeg{a, a, wrap2(b0 + o1, CAP), CAP, W, j == silent_j, p.db_min};
+                    },
+                    s, t, Kc, wsm + p.scratch_off, s_min, tid, nt);
             }
             last_silent = hit;
             if(hit)
@@ -613,6 +896,14 @@ struct wf_wave {
     cudaStream_t last_stream = nullptr;
     bool chunked = true;  // wave_chunk_kernel (WF_WAVE_CHUNK=0: the per-tick kernel, kept for A/B and bit-identity tests)
     int chunk_mode = 0, chunk_floats = 0, chunk_per_sm = 8;
+    // display stage: only when the config carried display settings (current struct size) and width >= 2
+    bool display = false;
+    wf::Tables tab;
+    float *d_tab = nullptr;       // interp weights | interp indices | Gaussian
+    int disp_scratch = 0;         // floats of Gaussian scratch (dch * width, or 0 without the filter)
+    int disp_per_sm = 4;          // resident CTAs of the DISP chunk kernel
+    float *s_points = nullptr, *s_pixels = nullptr, *s_min = nullptr;
+    size_t points_cap = 0, pixels_cap = 0, min_cap = 0;
 };
 
 namespace {
@@ -667,6 +958,42 @@ bool w_is_device_ptr(const void *p)
         return false;
     }
     return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+}
+
+// A config is either the current struct or the previous one, which ends before interp_mode: its display settings are absent.
+int wave_config_in(const wf_wave_config *in, wf_wave_config &c, bool &display_settings)
+{
+    if(in->struct_size == sizeof(wf_wave_config))
+    {
+        c = *in;
+        display_settings = true;
+        return WF_OK;
+    }
+    if(in->struct_size != offsetof(wf_wave_config, interp_mode))
+        return WF_ERR_ABI;
+    memset(&c, 0, sizeof(c));
+    memcpy(&c, in, offsetof(wf_wave_config, interp_mode));
+    c.struct_size = (uint32_t)sizeof(wf_wave_config);
+    display_settings = false;
+    return WF_OK;
+}
+
+// The limits of a waveform config that the clock and the buffers depend on (wf_wave_create, the previews): width in
+// [1, 8192] and a nanosecond step meter_ms * 10^6 / width of at least 1.
+bool wave_clock_ok(const wf_wave_config &c)
+{
+    return c.sample_rate >= 1 && c.width >= 1 && c.width <= 8192 && c.meter_ms >= 1 &&
+           ((uint64_t)c.meter_ms * 1000000ull) / (uint64_t)c.width != 0;
+}
+
+const void *chunk_kernel(int mode, bool disp)
+{
+    static const void *const k[2][4] = {
+        {(const void *)wave_chunk_kernel<0, WParams>, (const void *)wave_chunk_kernel<1, WParams>,
+         (const void *)wave_chunk_kernel<2, WParams>, (const void *)wave_chunk_kernel<3, WParams>},
+        {(const void *)wave_chunk_kernel<0, WDisp>, (const void *)wave_chunk_kernel<1, WDisp>,
+         (const void *)wave_chunk_kernel<2, WDisp>, (const void *)wave_chunk_kernel<3, WDisp>}};
+    return k[disp ? 1 : 0][mode];
 }
 
 // The tick-by-tick timestamp walk of tick_waveform (src/source_generic.cpp:303-339,358) for packets of `hop` samples that
@@ -732,22 +1059,38 @@ void wf_wave_config_init(wf_wave_config *c)
     c->normalize_volume = 0;
     c->volume_target = -8.0f;
     c->max_gain = 30.0f;
+    c->interp_mode = WF_INTERP_CATROM;
+    c->filter_mode = WF_FILTER_NONE;
+    c->filter_radius = 1.5f;
+    c->height = 225;
+    c->floor_db = -65;
+    c->ceiling_db = 0;
+    c->channel_spacing = 0;
 }
 
 const char *wf_wave_last_error(const wf_wave *w) { return w ? w->last_error.c_str() : g_wave_create_error.c_str(); }
 
-int wf_wave_create(const wf_wave_config *cfg, wf_wave **out)
+int wf_wave_create(const wf_wave_config *cfg_in, wf_wave **out)
 {
-    if(!cfg || !out)
+    if(!cfg_in || !out)
         return WF_ERR_INVALID_ARG;
     *out = nullptr;
-    if(cfg->struct_size != sizeof(wf_wave_config))
+    wf_wave_config cfg_v;
+    bool display_settings = false;
+    if(wave_config_in(cfg_in, cfg_v, display_settings) != WF_OK)
         return werr(nullptr, WF_ERR_ABI, "wf_wave_config.struct_size mismatch");
-    if(cfg->capture_channels < 1 || cfg->capture_channels > 2 || cfg->max_streams < 1 || cfg->sample_rate < 1 ||
-       cfg->width < 1 || cfg->width > 8192 || cfg->meter_ms < 1)
-        return werr(nullptr, WF_ERR_INVALID_ARG, "bad waveform config");
-    if(((uint64_t)cfg->meter_ms * 1000000ull) / (uint64_t)cfg->width == 0)
-        return werr(nullptr, WF_ERR_INVALID_ARG, "meter_ms too small for this width (step of 0 ns)");
+    const wf_wave_config *cfg = &cfg_v;
+    if(cfg->capture_channels < 1 || cfg->capture_channels > 2 || cfg->max_streams < 1 || !wave_clock_ok(*cfg))
+        return werr(nullptr, WF_ERR_INVALID_ARG, "bad waveform config (or meter_ms too small for this width: a step of 0 ns)");
+    // the display tables are built only for a config that passed the checks above (width <= 8192)
+    wf::Tables tab;
+    const bool display = display_settings && cfg->width >= 2;
+    if(display)
+    {
+        const char *why = "bad display settings";
+        if(wf::build_wave_tables(*cfg, tab, &why) != WF_OK)
+            return werr(nullptr, WF_ERR_INVALID_ARG, "%s", why);
+    }
     int ndev = 0;
     if(cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     {
@@ -789,8 +1132,19 @@ int wf_wave_create(const wf_wave_config *cfg, wf_wave **out)
         return bail(werr(w, WF_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", dev, prop.major,
                          prop.minor));
     w->sm_count = prop.multiProcessorCount;
-    if(2 * (size_t)cfg->width * sizeof(float) > 48 * 1024) // widths above 6144: both scrolling rings exceed the default 48 KB
-        WFW_C(cudaFuncSetAttribute(wave_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * (size_t)cfg->width * sizeof(float))));
+    w->display = display;
+    w->tab = std::move(tab);
+    // the Gaussian's scratch rows follow the kernel's own shared memory in the DISP kernels
+    w->disp_scratch = (display && w->tab.cfg.filter_mode == WF_FILTER_GAUSS) ? w->dch * cfg->width : 0;
+    {
+        const int ring_bytes = (int)((2 * (size_t)cfg->width + w->disp_scratch) * sizeof(float));
+        if(ring_bytes > 48 * 1024) // widths above 6144: both scrolling rings exceed the default 48 KB
+        {
+            WFW_C(cudaFuncSetAttribute(wave_kernel<WParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * (size_t)cfg->width * sizeof(float))));
+            if(display)
+                WFW_C(cudaFuncSetAttribute(wave_kernel<WDisp>, cudaFuncAttributeMaxDynamicSharedMemorySize, ring_bytes));
+        }
+    }
     {
         const char *e = getenv("WF_WAVE_CHUNK");
         w->chunked = !(e && e[0] == '0');
@@ -798,26 +1152,30 @@ int wf_wave_create(const wf_wave_config *cfg, wf_wave **out)
         w->chunk_mode = cfg->stereo ? (two ? 2 : 3) : (two ? 1 : 0);
         static const int mult[4] = {2, 4, 4, 3};
         w->chunk_floats = mult[w->chunk_mode] * cfg->width;
-        const int bytes = w->chunk_floats * (int)sizeof(float);
-        if(bytes > 48 * 1024)
+        for(int disp = 0; disp < (display ? 2 : 1); ++disp)
         {
-            switch(w->chunk_mode)
-            {
-            case 0: WFW_C(cudaFuncSetAttribute(wave_chunk_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)); break;
-            case 1: WFW_C(cudaFuncSetAttribute(wave_chunk_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)); break;
-            case 2: WFW_C(cudaFuncSetAttribute(wave_chunk_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)); break;
-            default: WFW_C(cudaFuncSetAttribute(wave_chunk_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)); break;
-            }
+            const void *k = chunk_kernel(w->chunk_mode, disp != 0);
+            const int bytes = (w->chunk_floats + (disp ? w->disp_scratch : 0)) * (int)sizeof(float);
+            if(bytes > 48 * 1024)
+                WFW_C(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+            int per_sm = 0;
+            WFW_C(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, 256, (size_t)bytes));
+            // one resident wave: streams are equal work, a partial second wave is a tail
+            (disp ? w->disp_per_sm : w->chunk_per_sm) = std::max(1, per_sm);
         }
-        int per_sm = 0;
-        switch(w->chunk_mode)
+    }
+    if(display)
+    {
+        const auto &t = w->tab;
+        const size_t n = t.interp_indices.size() + t.interp_weights.size() + t.gauss.size();
+        WFW_C(cudaMalloc((void **)&w->d_tab, n * sizeof(float)));
+        float *q = w->d_tab;
+        for(const auto *v : {&t.interp_weights, &t.interp_indices, &t.gauss}) // weights first: 16-byte aligned
         {
-        case 0: WFW_C(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wave_chunk_kernel<0>, 256, (size_t)bytes)); break;
-        case 1: WFW_C(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wave_chunk_kernel<1>, 256, (size_t)bytes)); break;
-        case 2: WFW_C(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wave_chunk_kernel<2>, 256, (size_t)bytes)); break;
-        default: WFW_C(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wave_chunk_kernel<3>, 256, (size_t)bytes)); break;
+            if(!v->empty())
+                WFW_C(cudaMemcpy(q, v->data(), v->size() * sizeof(float), cudaMemcpyHostToDevice));
+            q += v->size();
         }
-        w->chunk_per_sm = std::max(1, per_sm); // one resident wave: streams are equal work, a partial second wave is a tail
     }
     WFW_C(cudaStreamCreateWithFlags(&w->stream, cudaStreamNonBlocking));
     WFW_C(cudaEventCreate(&w->ev0));
@@ -846,7 +1204,8 @@ void wf_wave_destroy(wf_wave *w)
         if(w->last_stream && w->last_stream != w->stream)
             cudaStreamSynchronize(w->last_stream);
     }
-    void *ptrs[] = {w->d_state, w->d_flags, w->d_src, w->d_off, w->s_pcm, w->s_out, w->s_rms, w->s_silent};
+    void *ptrs[] = {w->d_state, w->d_flags, w->d_src, w->d_off, w->s_pcm, w->s_out, w->s_rms, w->s_silent,
+                    w->d_tab, w->s_points, w->s_pixels, w->s_min};
     for(void *q : ptrs)
         if(q)
             cudaFree(q);
@@ -866,22 +1225,32 @@ void wf_wave_destroy(wf_wave *w)
     delete w;
 }
 
-int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b, void *cuda_stream)
+int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b_in, void *cuda_stream)
 {
-    if(!w || !b)
+    if(!w || !b_in)
         return WF_ERR_INVALID_ARG;
     wf::NvtxRange nvtx("wf_wave_process");
-    if(b->struct_size != sizeof(wf_wave_batch))
-        return werr(w, WF_ERR_ABI, "wf_wave_batch.struct_size %u != %zu", b->struct_size, sizeof(wf_wave_batch));
+    // the current struct or the previous one (which ends before out_points: no display outputs)
+    wf_wave_batch bv{};
+    if(b_in->struct_size == sizeof(wf_wave_batch))
+        bv = *b_in;
+    else if(b_in->struct_size == offsetof(wf_wave_batch, out_points))
+        memcpy(&bv, b_in, offsetof(wf_wave_batch, out_points));
+    else
+        return werr(w, WF_ERR_ABI, "wf_wave_batch.struct_size %u != %zu", b_in->struct_size, sizeof(wf_wave_batch));
+    const wf_wave_batch *b = &bv;
     if(b->n_ticks < 0 || b->hop < 1)
         return werr(w, WF_ERR_INVALID_ARG, "n_ticks must be >= 0 and hop >= 1");
     if(b->n_streams != w->cfg.max_streams)
         return werr(w, WF_ERR_CAPACITY, "a waveform call must tick all %d streams of the engine (got %d): the clock is shared",
                     w->cfg.max_streams, b->n_streams);
+    const bool disp = b->out_points || b->out_pixels || b->out_min;
+    if(disp && !w->display)
+        return werr(w, WF_ERR_INVALID_ARG, "display outputs need an engine created with display settings (and width >= 2)");
     if(b->n_ticks == 0)
         return WF_OK;
-    if(!b->pcm || !b->out)
-        return werr(w, WF_ERR_INVALID_ARG, "pcm / out is null");
+    if(!b->pcm || !(b->out || b->out_points || b->out_pixels))
+        return werr(w, WF_ERR_INVALID_ARG, "pcm is null, or none of out / out_points / out_pixels is set");
     if(b->stream_stride < 0 || b->channel_stride < 0)
         return werr(w, WF_ERR_INVALID_ARG, "negative strides are not supported");
     if((long long)b->n_ticks * b->hop > 0x7fffffffLL)
@@ -932,7 +1301,7 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b, void *cuda_stream)
 
     const bool dev_ptrs = w_is_device_ptr(b->pcm);
     const float *d_pcm = b->pcm, *d_rms = b->input_rms;
-    float *d_out = b->out;
+    float *d_out = b->out, *d_points = b->out_points, *d_pixels = b->out_pixels, *d_min = b->out_min;
     unsigned char *d_silent = b->out_silent;
     const size_t out_n = S * T * w->dch * (size_t)W;
     if(!dev_ptrs)
@@ -942,9 +1311,30 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b, void *cuda_stream)
             return rc;
         WFW_CUDA(w, cudaMemcpyAsync(w->s_pcm, b->pcm, span * sizeof(float), cudaMemcpyHostToDevice, st));
         d_pcm = w->s_pcm;
-        if((rc = wensure(w, &w->s_out, &w->out_cap, out_n)))
-            return rc;
-        d_out = w->s_out;
+        if(b->out)
+        {
+            if((rc = wensure(w, &w->s_out, &w->out_cap, out_n)))
+                return rc;
+            d_out = w->s_out;
+        }
+        if(b->out_points)
+        {
+            if((rc = wensure(w, &w->s_points, &w->points_cap, out_n)))
+                return rc;
+            d_points = w->s_points;
+        }
+        if(b->out_pixels)
+        {
+            if((rc = wensure(w, &w->s_pixels, &w->pixels_cap, out_n)))
+                return rc;
+            d_pixels = w->s_pixels;
+        }
+        if(b->out_min)
+        {
+            if((rc = wensure(w, &w->s_min, &w->min_cap, S * T * 2)))
+                return rc;
+            d_min = w->s_min;
+        }
         if(b->input_rms)
         {
             if((rc = wensure(w, &w->s_rms, &w->rms_cap, S * T)))
@@ -981,28 +1371,55 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b, void *cuda_stream)
     p.vol_target = w->cfg.volume_target;
     p.max_gain = w->cfg.max_gain;
     p.db_min = w->db_min;
-    WFW_CUDA(w, cudaEventRecord(w->ev0, st));
-    const int grid = (int)std::min<size_t>(S, (size_t)w->sm_count * (w->chunked ? w->chunk_per_sm : 8));
-    if(w->chunked)
+    WDisp pd{};
+    if(disp)
     {
-        const size_t smem = (size_t)w->chunk_floats * sizeof(float);
-        switch(w->chunk_mode)
-        {
-        case 0: wave_chunk_kernel<0><<<grid, 256, smem, st>>>(p); break;
-        case 1: wave_chunk_kernel<1><<<grid, 256, smem, st>>>(p); break;
-        case 2: wave_chunk_kernel<2><<<grid, 256, smem, st>>>(p); break;
-        default: wave_chunk_kernel<3><<<grid, 256, smem, st>>>(p); break;
-        }
+        const auto &t = w->tab;
+        static_cast<WParams &>(pd) = p;
+        pd.interp_w = t.interp_weights.empty() ? nullptr : w->d_tab;
+        pd.interp_idx = w->d_tab + t.interp_weights.size();
+        pd.gauss_w = t.gauss.empty() ? nullptr : w->d_tab + t.interp_weights.size() + t.interp_indices.size();
+        pd.out_points = d_points;
+        pd.out_pixels = d_pixels;
+        pd.out_min = d_min;
+        pd.taps = t.interp_taps;
+        pd.filter = t.gauss.empty() ? 0 : 1;
+        pd.gauss_radius = t.gauss_radius;
+        pd.gauss_sum = t.gauss_sum;
+        pd.ceiling_f = (float)t.cfg.ceiling_db;
+        pd.dbrange_f = (float)(t.cfg.ceiling_db - t.cfg.floor_db);
+        pd.px_hi = t.px_hi;
+        pd.px_cpos = t.px_cpos;
+        pd.scratch_off = w->chunked ? w->chunk_floats : 2 * W;
+        pd.vec4 = ((W & 3) == 0) && ((reinterpret_cast<uintptr_t>(d_points) & 15) == 0) &&
+                  ((reinterpret_cast<uintptr_t>(d_pixels) & 15) == 0);
     }
+    WFW_CUDA(w, cudaEventRecord(w->ev0, st));
+    const int per_sm = w->chunked ? (disp ? w->disp_per_sm : w->chunk_per_sm) : 8;
+    const int grid = (int)std::min<size_t>(S, (size_t)w->sm_count * per_sm);
+    const size_t scratch = disp ? (size_t)w->disp_scratch * sizeof(float) : 0;
+    void *args[] = {disp ? (void *)&pd : (void *)&p};
+    if(w->chunked)
+        WFW_CUDA(w, cudaLaunchKernel(chunk_kernel(w->chunk_mode, disp), dim3(grid), dim3(256), args,
+                                     (size_t)w->chunk_floats * sizeof(float) + scratch, st));
+    else if(disp)
+        wave_kernel<WDisp><<<grid, 256, 2 * (size_t)W * sizeof(float) + scratch, st>>>(pd);
     else
-        wave_kernel<<<grid, 256, 2 * (size_t)W * sizeof(float), st>>>(p);
+        wave_kernel<WParams><<<grid, 256, 2 * (size_t)W * sizeof(float), st>>>(p);
     WFW_CUDA(w, cudaGetLastError());
     w->launches++;
     WFW_CUDA(w, cudaEventRecord(w->ev1, st));
     w->ev_valid = true;
     if(!dev_ptrs)
     {
-        WFW_CUDA(w, cudaMemcpyAsync(b->out, d_out, out_n * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if(b->out)
+            WFW_CUDA(w, cudaMemcpyAsync(b->out, d_out, out_n * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if(b->out_points)
+            WFW_CUDA(w, cudaMemcpyAsync(b->out_points, d_points, out_n * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if(b->out_pixels)
+            WFW_CUDA(w, cudaMemcpyAsync(b->out_pixels, d_pixels, out_n * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if(b->out_min)
+            WFW_CUDA(w, cudaMemcpyAsync(b->out_min, d_min, S * T * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
         if(b->out_silent)
             WFW_CUDA(w, cudaMemcpyAsync(b->out_silent, d_silent, S * T, cudaMemcpyDeviceToHost, st));
     }
@@ -1032,15 +1449,17 @@ int wf_wave_reset(wf_wave *w)
     return WF_OK;
 }
 
-int64_t wf_wave_preview_plan(const wf_wave_config *cfg, int32_t n_ticks, int32_t hop, int32_t *counts, int32_t *src,
+int64_t wf_wave_preview_plan(const wf_wave_config *cfg_in, int32_t n_ticks, int32_t hop, int32_t *counts, int32_t *src,
                              int64_t capacity)
 {
-    if(!cfg || n_ticks < 0 || hop < 1)
+    if(!cfg_in || n_ticks < 0 || hop < 1)
         return WF_ERR_INVALID_ARG;
-    if(cfg->struct_size != sizeof(wf_wave_config))
+    wf_wave_config cfg_v;
+    bool display_settings;
+    if(wave_config_in(cfg_in, cfg_v, display_settings) != WF_OK)
         return WF_ERR_ABI;
-    if(cfg->sample_rate < 1 || cfg->width < 1 || cfg->width > 8192 || cfg->meter_ms < 1 ||
-       ((uint64_t)cfg->meter_ms * 1000000ull) / (uint64_t)cfg->width == 0)
+    const wf_wave_config *cfg = &cfg_v;
+    if(!wave_clock_ok(*cfg))
         return WF_ERR_INVALID_ARG;
     wf_wave w; // host-only use: the same initial clock / start-up state wf_wave_create sets up
     w.cfg = *cfg;
@@ -1058,6 +1477,37 @@ int64_t wf_wave_preview_plan(const wf_wave_config *cfg, int32_t n_ticks, int32_t
         memcpy(src, s.data(), s.size() * sizeof(int));
     }
     return (int64_t)s.size();
+}
+
+int64_t wf_wave_preview_table(const wf_wave_config *cfg_in, int which, float *out, int64_t capacity)
+{
+    if(!cfg_in)
+        return WF_ERR_INVALID_ARG;
+    wf_wave_config cfg;
+    bool display_settings;
+    if(wave_config_in(cfg_in, cfg, display_settings) != WF_OK)
+        return WF_ERR_ABI;
+    if(which != WF_TABLE_INTERP_INDICES && which != WF_TABLE_INTERP_WEIGHTS && which != WF_TABLE_GAUSS)
+        return WF_ERR_INVALID_ARG;
+    if(!wave_clock_ok(cfg)) // the limits wf_wave_create applies, before anything is sized by width
+        return WF_ERR_INVALID_ARG;
+    if(!display_settings)
+        return 0; // an engine without display settings has no display tables
+    wf::Tables t;
+    const char *why = nullptr;
+    if(int rc = wf::build_wave_tables(cfg, t, &why); rc != WF_OK)
+        return rc;
+    const std::vector<float> &v = (which == WF_TABLE_INTERP_INDICES) ? t.interp_indices
+                                  : (which == WF_TABLE_INTERP_WEIGHTS) ? t.interp_weights
+                                                                       : t.gauss;
+    if(out)
+    {
+        if((int64_t)v.size() > capacity)
+            return WF_ERR_INVALID_ARG;
+        if(!v.empty())
+            memcpy(out, v.data(), v.size() * sizeof(float));
+    }
+    return (int64_t)v.size();
 }
 
 int64_t wf_wave_launch_count(const wf_wave *w) { return w ? w->launches : 0; }

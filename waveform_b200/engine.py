@@ -48,6 +48,7 @@ EXPORTS = [
     "wf_meter_process", "wf_meter_process_async", "wf_meter_reset", "wf_meter_launch_count", "wf_meter_last_kernel_ms",
     "wf_wave_config_init", "wf_wave_create", "wf_wave_destroy", "wf_wave_last_error", "wf_wave_process",
     "wf_wave_process_async", "wf_wave_reset", "wf_wave_launch_count", "wf_wave_last_kernel_ms", "wf_wave_preview_plan",
+    "wf_wave_preview_table",
 ]
 
 METER_PEAK, METER_RMS, METER_INPUT_RMS = 0, 1, 2
@@ -58,6 +59,8 @@ class WfMeterConfig(C.Structure):
         ("struct_size", C.c_uint32), ("device", C.c_int32), ("max_streams", C.c_int32), ("sample_rate", C.c_uint32),
         ("capture_channels", C.c_int32), ("mode", C.c_int32), ("meter_ms", C.c_int32), ("tsmoothing", C.c_int32),
         ("gravity", C.c_float), ("fast_peaks", C.c_int32), ("floor_db", C.c_int32),
+        ("height", C.c_int32), ("ceiling_db", C.c_int32), ("bar_width", C.c_int32), ("rounded_caps", C.c_int32),
+        ("min_bar_height", C.c_int32),
     ]
 
 
@@ -66,6 +69,8 @@ class WfWaveConfig(C.Structure):
         ("struct_size", C.c_uint32), ("device", C.c_int32), ("max_streams", C.c_int32), ("sample_rate", C.c_uint32),
         ("capture_channels", C.c_int32), ("stereo", C.c_int32), ("width", C.c_int32), ("meter_ms", C.c_int32),
         ("normalize_volume", C.c_int32), ("volume_target", C.c_float), ("max_gain", C.c_float),
+        ("interp_mode", C.c_int32), ("filter_mode", C.c_int32), ("filter_radius", C.c_float), ("height", C.c_int32),
+        ("floor_db", C.c_int32), ("ceiling_db", C.c_int32), ("channel_spacing", C.c_int32),
     ]
 
 
@@ -74,6 +79,7 @@ class WfWaveBatch(C.Structure):
         ("struct_size", C.c_uint32), ("n_streams", C.c_int32), ("n_ticks", C.c_int32), ("hop", C.c_int32),
         ("pcm", C.c_void_p), ("stream_stride", C.c_int64), ("channel_stride", C.c_int64),
         ("input_rms", C.c_void_p), ("out", C.c_void_p), ("out_silent", C.c_void_p),
+        ("out_points", C.c_void_p), ("out_pixels", C.c_void_p), ("out_min", C.c_void_p),
     ]
 
 
@@ -83,6 +89,7 @@ class WfMeterBatch(C.Structure):
         ("first_stream", C.c_int32), ("seconds", C.c_float),
         ("pcm", C.c_void_p), ("stream_stride", C.c_int64), ("channel_stride", C.c_int64),
         ("out_db", C.c_void_p), ("out_lin", C.c_void_p), ("out_silent", C.c_void_p),
+        ("out_pixels", C.c_void_p), ("out_min", C.c_void_p),
     ]
 
 
@@ -203,6 +210,8 @@ def load_library():
     L.wf_wave_last_kernel_ms.argtypes = [vp]
     L.wf_wave_preview_plan.restype = C.c_int64
     L.wf_wave_preview_plan.argtypes = [C.POINTER(WfWaveConfig), C.c_int32, C.c_int32, vp, vp, C.c_int64]
+    L.wf_wave_preview_table.restype = C.c_int64
+    L.wf_wave_preview_table.argtypes = [C.POINTER(WfWaveConfig), C.c_int, vp, C.c_int64]
     _lib = L
     return L
 
@@ -488,7 +497,8 @@ class Engine:
 
 def make_meter_config(settings: dict | None = None, sample_rate: int = 48000, channels: int = 2, max_streams: int = 1,
                       device: int = -1, mode: int | None = None) -> WfMeterConfig:
-    """Reference setting keys (meter_buf, rms_mode, temporal_smoothing, gravity, fast_peaks, floor;
+    """Reference setting keys (meter_buf, rms_mode, temporal_smoothing, gravity, fast_peaks, floor, and for the display
+    stage height, ceiling, bar_width, rounded_caps, min_bar_height;
     src/settings.hpp:29-135, defaults src/source.cpp:119-174) -> wf_meter_config."""
     L = load_library()
     c = WfMeterConfig()
@@ -503,6 +513,12 @@ def make_meter_config(settings: dict | None = None, sample_rate: int = 48000, ch
     c.gravity = float(s.pop("gravity", 0.65))
     c.fast_peaks = int(bool(s.pop("fast_peaks", False)))
     c.floor_db = int(s.pop("floor", -65))
+    # display stage (render_bars in meter mode)
+    c.height = int(s.pop("height", 225))
+    c.ceiling_db = int(s.pop("ceiling", 0))
+    c.bar_width = int(s.pop("bar_width", 24))
+    c.rounded_caps = int(bool(s.pop("rounded_caps", False)))
+    c.min_bar_height = int(s.pop("min_bar_height", 0))
     if s:
         raise KeyError(f"unsupported meter settings: {sorted(s)}")
     return c
@@ -548,9 +564,11 @@ class MeterEngine:
         count = self.cfg.max_streams - first_stream if count is None else count
         self._check(self.L.wf_meter_reset(self.h, first_stream, count))
 
-    def process(self, pcm, n_ticks: int, hop: int, *, first_stream=0, seconds=1.0 / 60.0, stream=None):
+    def process(self, pcm, n_ticks: int, hop: int, *, first_stream=0, seconds=1.0 / 60.0, stream=None, want_pixels=False):
         """pcm: [n_streams, capture_channels, >= n_ticks*hop] float32, numpy (host) or CUDA torch tensor.
-        Returns dict(db, lin, silent) — or dict(rms=[S, T]) for an INPUT_RMS engine."""
+        Returns dict(db, lin, silent) — or dict(rms=[S, T]) for an INPUT_RMS engine.  want_pixels adds the bar heights
+        render_bars draws, pixels=[S, T, capture_channels], and min=[S, T, 2] (miny, minpos).  CUDA tensors without an
+        explicit `stream` run on torch's current stream."""
         is_torch = hasattr(pcm, "data_ptr")
         if pcm.ndim == 2:
             pcm = pcm[None]
@@ -571,6 +589,10 @@ class MeterEngine:
         feed = self.cfg.mode == METER_INPUT_RMS
         out = {"rms": mk((S, n_ticks), f32)} if feed else {
             "db": mk((S, n_ticks, cc), f32), "lin": mk((S, n_ticks, cc), f32), "silent": mk((S, n_ticks), u8)}
+        if want_pixels:
+            out["pixels"], out["min"] = mk((S, n_ticks, cc), f32), mk((S, n_ticks, 2), f32)
+        if is_torch and stream is None:
+            stream = torch.cuda.current_stream(pcm.device).cuda_stream
         b = WfMeterBatch()
         b.struct_size = C.sizeof(WfMeterBatch)
         b.n_streams, b.n_ticks, b.hop, b.first_stream, b.seconds = S, n_ticks, hop, first_stream, seconds
@@ -578,6 +600,7 @@ class MeterEngine:
         b.out_db = None if feed else _ptr(out["db"])
         b.out_lin = _ptr(out["rms"]) if feed else _ptr(out["lin"])
         b.out_silent = None if feed else _ptr(out["silent"])
+        b.out_pixels, b.out_min = _ptr(out.get("pixels")), _ptr(out.get("min"))
         if stream is None:
             self._check(self.L.wf_meter_process(self.h, C.byref(b)))
         else:
@@ -587,7 +610,8 @@ class MeterEngine:
 
 def make_wave_config(settings: dict | None = None, sample_rate: int = 48000, channels: int = 2, max_streams: int = 1,
                      device: int = -1) -> WfWaveConfig:
-    """Reference setting keys (width, meter_buf, channel_mode, normalize_volume, volume_target, max_gain) -> wf_wave_config."""
+    """Reference setting keys (width, meter_buf, channel_mode, normalize_volume, volume_target, max_gain, and for the display
+    stage interp_mode, filter_mode, filter_radius, height, floor, ceiling, channel_spacing) -> wf_wave_config."""
     L = load_library()
     c = WfWaveConfig()
     L.wf_wave_config_init(C.byref(c))
@@ -601,6 +625,13 @@ def make_wave_config(settings: dict | None = None, sample_rate: int = 48000, cha
     c.normalize_volume = int(bool(s.pop("normalize_volume", False)))
     c.volume_target = float(s.pop("volume_target", -8.0))
     c.max_gain = float(s.pop("max_gain", 30.0))
+    c.interp_mode = INTERPS[s.pop("interp_mode", "catmull_rom")]
+    c.filter_mode = FILTERS[s.pop("filter_mode", "none")]
+    c.filter_radius = float(s.pop("filter_radius", 1.5))
+    c.height = int(s.pop("height", 225))
+    c.floor_db = int(s.pop("floor", -65))
+    c.ceiling_db = int(s.pop("ceiling", 0))
+    c.channel_spacing = int(s.pop("channel_spacing", 0))
     if s:
         raise KeyError(f"unsupported waveform settings: {sorted(s)}")
     return c
@@ -645,9 +676,13 @@ class WaveEngine:
     def reset(self):
         self._check(self.L.wf_wave_reset(self.h))
 
-    def process(self, pcm, n_ticks: int, hop: int, *, input_rms=None, stream=None):
+    def process(self, pcm, n_ticks: int, hop: int, *, input_rms=None, stream=None, want_db=True, want_points=False,
+                want_pixels=False):
         """pcm: [max_streams, capture_channels, >= n_ticks*hop] float32, numpy (host) or CUDA torch tensor.
-        Returns dict(out=[S, T, display_channels, width], silent=[S, T])."""
+        Returns dict(out=[S, T, display_channels, width], silent=[S, T]); want_points / want_pixels add what render_curve
+        computes from each tick's rows: points (interpolated + smoothed dB), pixels and min=[S, T, 2] (miny, minpos), all
+        [S, T, display_channels, width].  want_db=False leaves `out` out (a display-only call).  CUDA tensors without an
+        explicit `stream` run on torch's current stream."""
         is_torch = hasattr(pcm, "data_ptr")
         if pcm.ndim == 2:
             pcm = pcm[None]
@@ -669,12 +704,22 @@ class WaveEngine:
             f32, u8 = np.float32, np.uint8
             if input_rms is not None:
                 input_rms = np.ascontiguousarray(input_rms, dtype=np.float32)
-        out = {"out": mk((S, n_ticks, self.display_channels, self.cfg.width), f32), "silent": mk((S, n_ticks), u8)}
+        shape = (S, n_ticks, self.display_channels, self.cfg.width)
+        out = {"silent": mk((S, n_ticks), u8)}
+        if want_db:
+            out["out"] = mk(shape, f32)
+        if want_points:
+            out["points"] = mk(shape, f32)
+        if want_pixels:
+            out["pixels"], out["min"] = mk(shape, f32), mk((S, n_ticks, 2), f32)
+        if is_torch and stream is None:
+            stream = torch.cuda.current_stream(pcm.device).cuda_stream
         b = WfWaveBatch()
         b.struct_size = C.sizeof(WfWaveBatch)
         b.n_streams, b.n_ticks, b.hop = S, n_ticks, hop
         b.pcm, b.stream_stride, b.channel_stride = _ptr(pcm), cc * ns, ns
-        b.input_rms, b.out, b.out_silent = _ptr(input_rms), _ptr(out["out"]), _ptr(out["silent"])
+        b.input_rms, b.out, b.out_silent = _ptr(input_rms), _ptr(out.get("out")), _ptr(out["silent"])
+        b.out_points, b.out_pixels, b.out_min = _ptr(out.get("points")), _ptr(out.get("pixels")), _ptr(out.get("min"))
         if stream is None:
             self._check(self.L.wf_wave_process(self.h, C.byref(b)))
         else:
@@ -692,3 +737,19 @@ def preview_wave_plan(cfg: WfWaveConfig, n_ticks: int, hop: int):
     src = np.zeros(max(int(total), 1), np.int32)
     L.wf_wave_preview_plan(C.byref(cfg), n_ticks, hop, counts.ctypes.data, src.ctypes.data, int(total))
     return counts, src[: int(total)]
+
+
+def preview_wave_tables(cfg: WfWaveConfig) -> dict:
+    """The waveform display stage's tables for a config (wf_wave_preview_table) — host arithmetic only, no device."""
+    L = load_library()
+    out = {}
+    for which, name in ((TABLE_INTERP_INDICES, "interp_indices"), (TABLE_INTERP_WEIGHTS, "interp_weights"),
+                        (TABLE_GAUSS, "gauss")):
+        n = L.wf_wave_preview_table(C.byref(cfg), which, None, 0)
+        if n < 0:
+            raise WfError(int(n), L.wf_strerror(int(n)).decode())
+        arr = np.zeros(n, dtype=np.float32)
+        if n:
+            L.wf_wave_preview_table(C.byref(cfg), which, arr.ctypes.data, n)
+        out[name] = arr
+    return out
