@@ -8,15 +8,12 @@
 #include <cuda_runtime.h>
 
 #include <cmath>
-#include <cstdarg>
 #include <algorithm>
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
-#include <new>
 #include <string>
 #include <vector>
 
+#include "wf_host.hpp"
 #include "wf_kernels.cuh"
 #include "wf_fast2048.cuh"
 #include "wf_anyn.cuh"
@@ -31,15 +28,8 @@
 
 using namespace wf;
 
-struct wf_engine {
+struct wf_engine : HostCore {
     Tables tab;
-    int device = 0;
-    int sm_count = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    bool ev_valid = false;
-    std::string last_error;
-    int64_t launches = 0;
     std::string last_kernel;    // name of the spectrum kernel the most recent launch_range dispatched to (wf_last_kernel_name)
     bool hold_implicit = false; // some stream may carry flags bit 3 (m_decibels mirror left implicit by the N=2048 kernel)
     bool use_par16384 = true;   // WF_PAR16384=0: N=16384 stays on the CTA-per-tick kernel (A/B tests)
@@ -51,34 +41,23 @@ struct wf_engine {
     int fast_wpc_override = 0;  // WF_FAST_WPC=n: force warps per CTA (tuning knob)
     bool use_pdl = true;        // WF_NO_PDL=1: launch the fast kernel without programmatic dependent launch
     int wide_r = 0;             // WF_WIDE_R=1|2|4|8: force the cluster size of the wide kernel (1 = never use it); 0 = automatic
+    int team_w = 0;             // WF_TEAM_W=4|8|16: force the team size of wf_team2048.cuh; 1: never use it; 0 = automatic
+    bool use_v3 = true;         // WF_V3=0: fall back to the first-generation kernels (A/B tests)
 
     // device tables
-    float *d_window = nullptr, *d_slope = nullptr, *d_rolloff = nullptr;
-    float *d_tw = nullptr, *d_tw_post = nullptr;
-    float *d_tw1 = nullptr, *d_tw2 = nullptr, *d_tw0 = nullptr; // inter-pass twiddles of the CTA-per-tick kernel (wf_v3.cuh), N = 4096/8192/16384
-    // N=2048: the warp-per-stream kernel needs ~2400 streams to fill the GPU; with fewer streams AND long per-stream tick
-    // sequences (>= 32) the cluster kernel (wf_v3.cuh, up to 8 ticks of a stream in flight) is faster: measured 256x256
-    // 96 -> 145 M, 512x128 185 -> 202 M, 1024x64 286 vs 242 M spectra/s (profiles/r01_layouts.txt).  WF_FAST_MIN_STREAMS overrides.
-    int fast_min_streams = 768;
-    int team_w = 0;                            // WF_TEAM_W=4|8|16: force the team size of wf_team2048.cuh; 1: never use it; 0 = automatic
-    bool use_v3 = true;                        // WF_V3=0: fall back to the first-generation kernels (A/B tests)
-    float *d_interp_idx = nullptr, *d_interp_w = nullptr, *d_gauss = nullptr;
-    int *d_band_widths = nullptr, *d_band_offsets = nullptr;
+    DevBuf<float> d_window, d_slope, d_rolloff, d_tw, d_tw_post;
+    DevBuf<float> d_tw1, d_tw2, d_tw0; // inter-pass twiddles of the CTA-per-tick kernel (wf_v3.cuh), N = 4096/8192/16384
+    DevBuf<float> d_interp_idx, d_interp_w, d_gauss;
+    DevBuf<int> d_band_widths, d_band_offsets;
     // per-stream state
-    float *d_state = nullptr, *d_hold = nullptr;
-    unsigned char *d_flags = nullptr;
+    DevBuf<float> d_state, d_hold;
+    DevBuf<unsigned char> d_flags;
     // staging for host-pointer batches (grown on demand)
-    float *s_pcm = nullptr, *s_out_db = nullptr, *s_out_points = nullptr, *s_rms = nullptr, *s_peak = nullptr;
-    unsigned char *s_skip = nullptr, *s_silent = nullptr;
-    float *s_px = nullptr, *s_min = nullptr;
-    float *s_gtab = nullptr; // [n_frames][2] per-tick (g, 1-g) of a TV-exponential batch with frame_seconds
-    size_t s_gtab_cap = 0;
+    DevBuf<float> s_pcm, s_out_db, s_out_points, s_rms, s_peak, s_px, s_min;
+    DevBuf<unsigned char> s_skip, s_silent;
+    DevBuf<float> s_gtab; // [n_frames][2] per-tick (g, 1-g) of a TV-exponential batch with frame_seconds
     std::vector<float> h_gtab;
-    size_t s_px_cap = 0, s_min_cap = 0;
-    float *s_scratch = nullptr; // any-N kernel work buffers when N/2 complex points x 2 exceed shared memory
-    size_t s_scratch_cap = 0;
-    size_t s_pcm_cap = 0, s_out_db_cap = 0, s_out_points_cap = 0, s_rms_cap = 0, s_peak_cap = 0, s_skip_cap = 0,
-           s_silent_cap = 0;
+    DevBuf<float> s_scratch; // any-N kernel work buffers when N/2 complex points x 2 exceed shared memory
     // zero-copy verdict of the last host-pointer batch (live ticks reuse the same buffers every call)
     const void *zc_ptrs[9] = {};
     bool zc_ok = false, zc_dev = false, zc_valid = false;
@@ -89,57 +68,72 @@ struct wf_engine {
     cudaEvent_t chunk_in[kMaxChunks] = {}, chunk_k[kMaxChunks] = {}, ev_fork = nullptr, ev_join = nullptr;
 };
 
+// The engine's maintenance kernels (only this unit launches them).
+namespace wf {
+
+// Streams whose m_decibels mirror was left implicit by stft2048_fast_kernel (flags bit 3: mirror == dbfs(state), one
+// capture channel, one display channel) get it written out here, with the same MUFU.LG2 arithmetic the kernel used for
+// the outputs.  Run by the engine before anything else reads hold_db (other kernels, wf_get_state / wf_set_state).
+static __global__ void materialize_hold_kernel(const float *state, float *hold_db, unsigned char *flags, int n_streams, int B,
+                                               int och, float db_min)
+{
+    for(int s = blockIdx.x; s < n_streams; s += gridDim.x)
+    {
+        const unsigned char fl = flags[s];
+        if(!(fl & 8u))
+            continue;
+        for(int k = threadIdx.x; k < B; k += blockDim.x)
+        {
+            float l;
+            asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(l) : "f"(state[(size_t)s * B + k]));
+            hold_db[(size_t)s * och * B + k] = fmaxf(l * 6.02059991327962390f, db_min);
+        }
+        __syncthreads();
+        if(threadIdx.x == 0)
+            flags[s] = (unsigned char)(fl & ~8u);
+    }
+}
+
+// Timeout / hidden branch of tick_spectrum (src/source_generic.cpp:36-48) for streams [0, n_streams): a stream that is
+// already m_last_silent returns early there and keeps its buffers; the others get m_tsmooth_buf := 0, the DISPLAY rows of
+// m_decibels := DB_MIN (slot 1 of a 2ch->mono mix keeps its last linear magnitudes, :43-45) and m_last_silent := true.
+static __global__ void spectrum_reset_kernel(float *state, float *hold_db, unsigned char *flags, int n_streams, int ccB, int ochB,
+                                             int dchB, float db_min, unsigned char new_flags)
+{
+    for(int s = blockIdx.x; s < n_streams; s += gridDim.x)
+    {
+        if(flags[s] & 1u)
+            continue;
+        for(int i = threadIdx.x; i < ccB; i += blockDim.x)
+            state[(size_t)s * ccB + i] = 0.0f;
+        for(int i = threadIdx.x; i < dchB; i += blockDim.x)
+            hold_db[(size_t)s * ochB + i] = db_min;
+        __syncthreads();
+        if(threadIdx.x == 0)
+            flags[s] = new_flags;
+    }
+}
+
+// peak normalisation pass: out[row][k] += gain[t] for k >= 1 (row = (stream, frame, channel))
+static __global__ void peak_normalize_kernel(float *data, int n_streams, int n_frames, int rows_per_frame, int row_len,
+                                      const float *peak, float target_db, float max_gain)
+{
+    const long long rows = (long long)n_streams * n_frames * rows_per_frame;
+    for(long long r = blockIdx.x; r < rows; r += gridDim.x)
+    {
+        const int t = (int)((r / rows_per_frame) % n_frames);
+        const float gain = fminf(target_db - peak[t], max_gain);
+        float *row = data + r * row_len;
+        for(int k = 1 + threadIdx.x; k < row_len; k += blockDim.x)
+            row[k] += gain;
+    }
+}
+
+} // namespace wf
+
 namespace {
 
 thread_local std::string g_create_error;
-
-int set_err(wf_engine *e, int code, const char *fmt, ...)
-{
-    if(e)
-    {
-        char buf[512];
-        va_list ap;
-        va_start(ap, fmt);
-        vsnprintf(buf, sizeof(buf), fmt, ap);
-        va_end(ap);
-        e->last_error = buf;
-    }
-    return code;
-}
-
-#define WF_CUDA(e, call)                                                                                              \
-    do                                                                                                                \
-    {                                                                                                                 \
-        cudaError_t _err = (call);                                                                                    \
-        if(_err != cudaSuccess)                                                                                       \
-            return set_err((e), (_err == cudaErrorMemoryAllocation) ? WF_ERR_OOM : WF_ERR_CUDA, "%s failed: %s", #call, \
-                           cudaGetErrorString(_err));                                                                 \
-    } while(0)
-
-template<typename T>
-int upload(wf_engine *e, T **dst, const std::vector<T> &src)
-{
-    *dst = nullptr;
-    if(src.empty())
-        return WF_OK;
-    WF_CUDA(e, cudaMalloc((void **)dst, src.size() * sizeof(T)));
-    WF_CUDA(e, cudaMemcpy(*dst, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice));
-    return WF_OK;
-}
-
-template<typename T>
-int ensure(wf_engine *e, T **buf, size_t *cap, size_t need)
-{
-    if(need <= *cap)
-        return WF_OK;
-    if(*buf)
-        cudaFree(*buf);
-    *buf = nullptr;
-    *cap = 0;
-    WF_CUDA(e, cudaMalloc((void **)buf, need * sizeof(T)));
-    *cap = need;
-    return WF_OK;
-}
 
 bool is_pow2_kernel_size(int n)
 {
@@ -193,35 +187,6 @@ bool supported_fft_size(int n)
     return n <= 65536; // sizes whose work buffers exceed shared memory run from a global (L2) scratch
 }
 
-// 0 = pageable host (or unknown), 1 = device / managed, 2 = page-locked host memory the device can address directly
-int ptr_kind(const void *p)
-{
-    cudaPointerAttributes a{};
-    if(cudaPointerGetAttributes(&a, p) != cudaSuccess)
-    {
-        cudaGetLastError();
-        return 0;
-    }
-    if(a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged)
-        return 1;
-    if(a.type == cudaMemoryTypeHost && a.devicePointer == p) // unified addressing: the same pointer is valid on the device
-        return 2;
-    return 0;
-}
-
-bool is_device_ptr(const void *p)
-{
-    if(!p)
-        return false;
-    cudaPointerAttributes a{};
-    if(cudaPointerGetAttributes(&a, p) != cudaSuccess)
-    {
-        cudaGetLastError();
-        return false;
-    }
-    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
-}
-
 template<int N, int CC>
 int launch_fused(wf_engine *e, const KParams &kp, cudaStream_t st, size_t extra_smem)
 {
@@ -231,12 +196,12 @@ int launch_fused(wf_engine *e, const KParams &kp, cudaStream_t st, size_t extra_
     int dev = e->device & 63;
     if(smem > 48 * 1024 && configured[dev] < smem)
     {
-        WF_CUDA(e, cudaFuncSetAttribute(stft_fused_kernel<N, CC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        WF_CHECK(e, cudaFuncSetAttribute(stft_fused_kernel<N, CC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         configured[dev] = smem;
     }
     const int grid = (kp.n_streams + G::GROUPS - 1) / G::GROUPS;
     stft_fused_kernel<N, CC><<<grid, G::CTA, smem, st>>>(kp);
-    WF_CUDA(e, cudaGetLastError());
+    WF_CHECK(e, cudaGetLastError());
     e->launches++;
     e->last_kernel = "stft_fused_kernel<" + std::to_string(N) + "," + std::to_string(CC) + ">";
     return WF_OK;
@@ -282,7 +247,7 @@ int dispatch_n(wf_engine *e, const KParams &kp, cudaStream_t st, size_t extra)
             const bool feat = kp.slope || kp.rolloff || kp.normalize || kp.fast_peaks || kp.skip_mask || kp.g_tab;
             const int x = feat ? 3 : (kp.out_peak ? 1 : 0);
             const int r = pick_v3_r(e, kp);
-            WF_CUDA(e, v3_launch(e->tab.N, CC, r, x, kp, e->d_tw1, e->d_tw2, e->d_tw0, st, display, e->device));
+            WF_CHECK(e, v3_launch(e->tab.N, CC, r, x, kp, e->d_tw1, e->d_tw2, e->d_tw0, st, display, e->device));
             e->launches++;
             e->last_kernel = "stft_v3_kernel<" + std::to_string(e->tab.N) + "," + std::to_string(CC) + "," + std::to_string(r) +
                              "," + std::to_string(x) + ">";
@@ -291,7 +256,7 @@ int dispatch_n(wf_engine *e, const KParams &kp, cudaStream_t st, size_t extra)
         const int R = pick_wide_r(e, kp, display);
         if(R > 1)
         {
-            WF_CUDA(e, wide_launch(e->tab.N, CC, R, kp, st, display, e->device));
+            WF_CHECK(e, wide_launch(e->tab.N, CC, R, kp, st, display, e->device));
             e->launches++;
             e->last_kernel = "stft_wide_kernel<" + std::to_string(e->tab.N) + "," + std::to_string(CC) + "," + std::to_string(R) + ">";
             return WF_OK;
@@ -313,27 +278,26 @@ int dispatch_n(wf_engine *e, const KParams &kp, cudaStream_t st, size_t extra)
     // any other multiple of 16: run-time mixed-radix kernel
     AnyPlan plan;
     if(!make_any_plan(e->tab.N, &plan))
-        return set_err(e, WF_ERR_UNSUPPORTED_FFT_SIZE, "fft_size %d has no kernel", e->tab.N);
+        return fail(e, WF_ERR_UNSUPPORTED_FFT_SIZE, "fft_size %d has no kernel", e->tab.N);
     const bool in_smem = (size_t)plan.M * 16 + extra <= 200 * 1024;
     int grid = std::min(kp.n_streams, e->sm_count * (in_smem ? 8 : 2));
     size_t smem = in_smem ? (size_t)plan.M * 16 + extra : extra;
     plan.scratch = nullptr;
     if(!in_smem)
     {
-        int rc = ensure(e, &e->s_scratch, &e->s_scratch_cap, (size_t)grid * 2 * plan.M * 2);
-        if(rc)
+        if(int rc = e->s_scratch.reserve(e, (size_t)grid * 2 * plan.M * 2))
             return rc;
-        plan.scratch = reinterpret_cast<float2 *>(e->s_scratch);
+        plan.scratch = reinterpret_cast<float2 *>(e->s_scratch.p);
     }
     static thread_local size_t configured[64] = {0};
     const int dev = e->device & 63;
     if(smem > 48 * 1024 && configured[dev] < smem)
     {
-        WF_CUDA(e, cudaFuncSetAttribute(stft_anyn_kernel<CC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        WF_CHECK(e, cudaFuncSetAttribute(stft_anyn_kernel<CC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         configured[dev] = smem;
     }
     stft_anyn_kernel<CC><<<grid, kAnyThreads, smem, st>>>(kp, plan);
-    WF_CUDA(e, cudaGetLastError());
+    WF_CHECK(e, cudaGetLastError());
     e->launches++;
     e->last_kernel = "stft_anyn_kernel<" + std::to_string(CC) + "> N=" + std::to_string(e->tab.N);
     return WF_OK;
@@ -357,7 +321,7 @@ int launch_fast2048(wf_engine *e, const KParams &kp, cudaStream_t st)
     const int dev = e->device & 63;
     if(!configured[dev])
     {
-        WF_CUDA(e, cudaFuncSetAttribute(stft2048_fast_kernel<MAXW, TSM, GATE, EXTRA>,
+        WF_CHECK(e, cudaFuncSetAttribute(stft2048_fast_kernel<MAXW, TSM, GATE, EXTRA>,
                                         cudaFuncAttributeMaxDynamicSharedMemorySize, fast::smem_bytes(MAXW)));
         configured[dev] = true;
     }
@@ -378,7 +342,7 @@ int launch_fast2048(wf_engine *e, const KParams &kp, cudaStream_t st)
     attr[0].val.programmaticStreamSerializationAllowed = e->use_pdl ? 1 : 0;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    WF_CUDA(e, cudaLaunchKernelEx(&cfg, stft2048_fast_kernel<MAXW, TSM, GATE, EXTRA>, kp));
+    WF_CHECK(e, cudaLaunchKernelEx(&cfg, stft2048_fast_kernel<MAXW, TSM, GATE, EXTRA>, kp));
     e->launches++;
     e->last_kernel = "stft2048_fast_kernel<" + std::to_string(MAXW) + "," + std::to_string((int)TSM) + "," + std::to_string((int)GATE) +
                      "," + std::to_string((int)EXTRA) + "> grid " + std::to_string(grid) + " x " + std::to_string(wpc) + " warps";
@@ -402,18 +366,7 @@ int dispatch_fast2048(wf_engine *e, const KParams &kp, cudaStream_t st, bool ext
     WF_FAST_CASE(false, false, false)
     WF_FAST_CASE(false, false, true)
 #undef WF_FAST_CASE
-    return set_err(e, WF_ERR_INVALID_ARG, "fast2048 dispatch fell through");
-}
-
-int fill_device(wf_engine *e, float *p, long long n, float v, cudaStream_t st)
-{
-    if(n <= 0)
-        return WF_OK;
-    int blocks = (int)std::min<long long>((n + 255) / 256, 1184);
-    fill_kernel<<<blocks, 256, 0, st>>>(p, n, v);
-    WF_CUDA(e, cudaGetLastError());
-    e->launches++;
-    return WF_OK;
+    return fail(e, WF_ERR_INVALID_ARG, "fast2048 dispatch fell through");
 }
 
 // Write out every implicit m_decibels mirror (see materialize_hold_kernel) before something other than the N=2048
@@ -426,7 +379,7 @@ int materialize_hold(wf_engine *e, cudaStream_t st)
     const int S = t.cfg.max_streams;
     materialize_hold_kernel<<<std::min(S, e->sm_count * 8), 256, 0, st>>>(e->d_state, e->d_hold, e->d_flags, S, t.B,
                                                                           t.output_channels, t.db_min);
-    WF_CUDA(e, cudaGetLastError());
+    WF_CHECK(e, cudaGetLastError());
     e->launches++;
     e->hold_implicit = false;
     return WF_OK;
@@ -437,13 +390,13 @@ int init_state(wf_engine *e, int first, int count, cudaStream_t st)
 {
     const Tables &t = e->tab;
     const int cc = t.cfg.capture_channels, och = t.output_channels, B = t.B;
-    WF_CUDA(e, cudaMemsetAsync(e->d_state + (size_t)first * cc * B, 0, (size_t)count * cc * B * sizeof(float), st));
+    WF_CHECK(e, cudaMemsetAsync(e->d_state + (size_t)first * cc * B, 0, (size_t)count * cc * B * sizeof(float), st));
     int rc = fill_device(e, e->d_hold + (size_t)first * och * B, (long long)count * och * B, t.db_min, st);
     if(rc)
         return rc;
     // flags: bit0 last_silent; bit1/2: previous outputs all <= floor-10 (DB_MIN is)
     const bool below = !(t.db_min > (float)(t.cfg.floor_db - 10));
-    WF_CUDA(e, cudaMemsetAsync(e->d_flags + first, below ? 6 : 0, (size_t)count, st));
+    WF_CHECK(e, cudaMemsetAsync(e->d_flags + first, below ? 6 : 0, (size_t)count, st));
     return WF_OK;
 }
 
@@ -520,130 +473,54 @@ int wf_create(const wf_config *cfg, wf_engine **out)
     *out = nullptr;
     if(cfg->struct_size != sizeof(wf_config))
         return WF_ERR_ABI;
-    wf_engine *e = new(std::nothrow) wf_engine();
-    if(!e)
-        return WF_ERR_OOM;
-    auto bail = [&](int code) {
-        g_create_error = e->last_error; // readable through wf_last_error(NULL) after the engine is gone
-        wf_destroy(e);
-        return code;
-    };
+    return create_engine(out, g_create_error, wf_destroy, [&](wf_engine *e) -> int {
+        const char *why = nullptr;
+        int rc = build_tables(*cfg, e->tab, &why);
+        if(rc != WF_OK)
+            return fail(e, rc, "%s", why ? why : "bad config");
+        if(!supported_fft_size(e->tab.N))
+            return fail(e, WF_ERR_UNSUPPORTED_FFT_SIZE, "fft_size %d unsupported", e->tab.N);
+        if((rc = open_device(e, cfg->device)))
+            return rc;
+        e->force_generic = env_flag("WF_FORCE_GENERIC", false);
+        e->use_pdl = !env_flag("WF_NO_PDL", false);
+        e->wide_r = env_int("WF_WIDE_R", 0);
+        e->use_v3 = env_flag("WF_V3", true);
+        e->team_w = env_int("WF_TEAM_W", 0);
+        e->zero_copy = env_flag("WF_ZERO_COPY", true);
+        e->use_par16384 = env_flag("WF_PAR16384", true);
+        e->use_warp2 = env_flag("WF_WARP2", true);
+        e->use_warp2_display = env_flag("WF_WARP2_DISPLAY", true);
+        e->lazy_hold = env_flag("WF_LAZY_HOLD", true);
+        e->split_runs = env_flag("WF_SPLIT", true);
+        e->fast_wpc_override = env_int("WF_FAST_WPC", 0);
 
-    const char *why = nullptr;
-    int rc = build_tables(*cfg, e->tab, &why);
-    if(rc != WF_OK)
-    {
-        set_err(e, rc, "%s", why ? why : "bad config");
-        return bail(rc);
-    }
-    if(!supported_fft_size(e->tab.N))
-        return bail(set_err(e, WF_ERR_UNSUPPORTED_FFT_SIZE, "fft_size %d unsupported", e->tab.N));
+        const Tables &t = e->tab;
+        std::vector<float> tw1, tw2, tw0; // stay empty (and d_tw1 null) for sizes without the CTA-per-tick kernel
+        if(v3_supported(t.N))
+            v3_build_twiddles(t.N, tw1, tw2, tw0);
+        for(auto [buf, v] : {std::pair{&e->d_window, &t.window}, {&e->d_slope, &t.slope}, {&e->d_rolloff, &t.rolloff},
+                             {&e->d_tw, &t.tw}, {&e->d_tw_post, &t.tw_post}, {&e->d_tw1, &tw1}, {&e->d_tw2, &tw2},
+                             {&e->d_tw0, &tw0}, {&e->d_interp_idx, &t.interp_indices}, {&e->d_interp_w, &t.interp_weights},
+                             {&e->d_gauss, &t.gauss}})
+            if((rc = buf->upload(e, *v)))
+                return rc;
+        for(auto [buf, v] : {std::pair{&e->d_band_widths, &t.band_widths}, {&e->d_band_offsets, &t.band_offsets}})
+            if((rc = buf->upload(e, *v)))
+                return rc;
 
-    int ndev = 0;
-    if(cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-    {
-        cudaGetLastError();
-        return bail(set_err(e, WF_ERR_NO_DEVICE, "no CUDA device"));
-    }
-    int dev = cfg->device;
-    if(dev < 0)
-    {
-        if(cudaGetDevice(&dev) != cudaSuccess)
-            return bail(set_err(e, WF_ERR_CUDA, "cudaGetDevice failed"));
-    }
-    if(dev >= ndev)
-        return bail(set_err(e, WF_ERR_INVALID_ARG, "device %d out of range (%d devices)", dev, ndev));
-    e->device = dev;
-    {
-        const char *fg = getenv("WF_FORCE_GENERIC");
-        e->force_generic = fg && fg[0] == '1';
-        const char *np = getenv("WF_NO_PDL");
-        e->use_pdl = !(np && np[0] == '1');
-        const char *wr = getenv("WF_WIDE_R");
-        if(wr)
-            e->wide_r = atoi(wr);
-        const char *fms = getenv("WF_FAST_MIN_STREAMS");
-        if(fms)
-            e->fast_min_streams = atoi(fms);
-        const char *v3 = getenv("WF_V3");
-        e->use_v3 = !(v3 && v3[0] == '0');
-        const char *tw = getenv("WF_TEAM_W");
-        if(tw)
-            e->team_w = atoi(tw);
-        const char *zc = getenv("WF_ZERO_COPY");
-        e->zero_copy = !(zc && zc[0] == '0');
-        const char *p16 = getenv("WF_PAR16384");
-        e->use_par16384 = !(p16 && p16[0] == '0');
-        const char *w2 = getenv("WF_WARP2");
-        e->use_warp2 = !(w2 && w2[0] == '0');
-        const char *w2d = getenv("WF_WARP2_DISPLAY");
-        e->use_warp2_display = !(w2d && w2d[0] == '0');
-        const char *lh = getenv("WF_LAZY_HOLD");
-        e->lazy_hold = !(lh && lh[0] == '0');
-        const char *sp = getenv("WF_SPLIT");
-        e->split_runs = !(sp && sp[0] == '0');
-        const char *wo = getenv("WF_FAST_WPC");
-        if(wo)
-            e->fast_wpc_override = atoi(wo);
-    }
-
-#define WF_TRY(x)                 \
-    do                            \
-    {                             \
-        int _rc = (x);            \
-        if(_rc != WF_OK)          \
-            return bail(_rc);     \
-    } while(0)
-#define WF_CUDA_C(call)                                                                                      \
-    do                                                                                                       \
-    {                                                                                                        \
-        cudaError_t _err = (call);                                                                           \
-        if(_err != cudaSuccess)                                                                              \
-            return bail(set_err(e, (_err == cudaErrorMemoryAllocation) ? WF_ERR_OOM : WF_ERR_CUDA, "%s: %s", \
-                                #call, cudaGetErrorString(_err)));                                           \
-    } while(0)
-
-    WF_CUDA_C(cudaSetDevice(dev));
-    cudaDeviceProp prop{};
-    WF_CUDA_C(cudaGetDeviceProperties(&prop, dev));
-    e->sm_count = prop.multiProcessorCount;
-    if(prop.major != 9 || prop.minor != 0) // sm_90a code runs on compute capability 9.0 only
-        return bail(set_err(e, WF_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", dev,
-                            prop.major, prop.minor));
-    WF_CUDA_C(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
-    WF_CUDA_C(cudaEventCreate(&e->ev0));
-    WF_CUDA_C(cudaEventCreate(&e->ev1));
-
-    const Tables &t = e->tab;
-    WF_TRY(upload(e, &e->d_window, t.window));
-    WF_TRY(upload(e, &e->d_slope, t.slope));
-    WF_TRY(upload(e, &e->d_rolloff, t.rolloff));
-    WF_TRY(upload(e, &e->d_tw, t.tw));
-    WF_TRY(upload(e, &e->d_tw_post, t.tw_post));
-    if(v3_supported(t.N))
-    {
-        std::vector<float> tw1, tw2, tw0;
-        v3_build_twiddles(t.N, tw1, tw2, tw0);
-        WF_TRY(upload(e, &e->d_tw1, tw1));
-        WF_TRY(upload(e, &e->d_tw2, tw2));
-        WF_TRY(upload(e, &e->d_tw0, tw0));
-    }
-    WF_TRY(upload(e, &e->d_interp_idx, t.interp_indices));
-    WF_TRY(upload(e, &e->d_interp_w, t.interp_weights));
-    WF_TRY(upload(e, &e->d_gauss, t.gauss));
-    WF_TRY(upload(e, &e->d_band_widths, t.band_widths));
-    WF_TRY(upload(e, &e->d_band_offsets, t.band_offsets));
-
-    const size_t S = (size_t)t.cfg.max_streams;
-    WF_CUDA_C(cudaMalloc((void **)&e->d_state, S * t.cfg.capture_channels * t.B * sizeof(float)));
-    WF_CUDA_C(cudaMalloc((void **)&e->d_hold, S * t.output_channels * t.B * sizeof(float)));
-    WF_CUDA_C(cudaMalloc((void **)&e->d_flags, S));
-    WF_TRY(init_state(e, 0, (int)S, e->stream));
-    WF_CUDA_C(cudaStreamSynchronize(e->stream));
-#undef WF_TRY
-#undef WF_CUDA_C
-    *out = e;
-    return WF_OK;
+        const size_t S = (size_t)t.cfg.max_streams;
+        if((rc = e->d_state.reserve(e, S * t.cfg.capture_channels * t.B)))
+            return rc;
+        if((rc = e->d_hold.reserve(e, S * t.output_channels * t.B)))
+            return rc;
+        if((rc = e->d_flags.reserve(e, S)))
+            return rc;
+        if((rc = init_state(e, 0, (int)S, e->stream)))
+            return rc;
+        WF_CHECK(e, cudaStreamSynchronize(e->stream));
+        return WF_OK;
+    });
 }
 
 void wf_destroy(wf_engine *e)
@@ -655,12 +532,6 @@ void wf_destroy(wf_engine *e)
         cudaSetDevice(e->device);
         cudaStreamSynchronize(e->stream);
     }
-    void *ptrs[] = {e->d_window, e->d_slope, e->d_rolloff, e->d_tw, e->d_tw_post, e->d_tw1, e->d_tw2, e->d_tw0, e->d_interp_idx, e->d_interp_w,
-                    e->d_gauss, e->d_band_widths, e->d_band_offsets, e->d_state, e->d_hold, e->d_flags, e->s_pcm,
-                    e->s_out_db, e->s_out_points, e->s_rms, e->s_peak, e->s_skip, e->s_silent, e->s_scratch, e->s_px, e->s_min, e->s_gtab};
-    for(void *p : ptrs)
-        if(p)
-            cudaFree(p);
     for(auto ev : e->chunk_in)
         if(ev)
             cudaEventDestroy(ev);
@@ -675,12 +546,6 @@ void wf_destroy(wf_engine *e)
         cudaStreamDestroy(e->s_h2d);
     if(e->s_d2h)
         cudaStreamDestroy(e->s_d2h);
-    if(e->ev0)
-        cudaEventDestroy(e->ev0);
-    if(e->ev1)
-        cudaEventDestroy(e->ev1);
-    if(e->stream)
-        cudaStreamDestroy(e->stream);
     delete e;
 }
 
@@ -785,9 +650,9 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
     kp.input_rms = rms ? rms + (size_t)s0 * T : nullptr;
     kp.skip_mask = skip ? skip + (size_t)s0 * T : nullptr;
     kp.window = e->d_window;
-    kp.window2 = reinterpret_cast<const float2 *>(e->d_window);
-    kp.tw = reinterpret_cast<const float2 *>(e->d_tw);
-    kp.tw_post = reinterpret_cast<const float2 *>(e->d_tw_post);
+    kp.window2 = reinterpret_cast<const float2 *>(e->d_window.p);
+    kp.tw = reinterpret_cast<const float2 *>(e->d_tw.p);
+    kp.tw_post = reinterpret_cast<const float2 *>(e->d_tw_post.p);
     kp.slope = e->d_slope;
     kp.rolloff = e->d_rolloff;
     const size_t slot = (size_t)b->first_stream + (size_t)s0;
@@ -886,7 +751,7 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
         {
             const int tpc = 16 / W;
             const int grid = std::min(e->sm_count, kp.n_streams); // streams are dealt to SMs first, then to an SM's teams
-            WF_CUDA(e, team2048_launch(W, x, kp, grid, st, e->use_pdl, e->device));
+            WF_CHECK(e, team2048_launch(W, x, kp, grid, st, e->use_pdl, e->device));
             e->launches++;
             e->last_kernel = "stft2048_team_kernel<" + std::to_string(W) + "," + std::to_string((int)x) + "> grid " + std::to_string(grid) +
                              " x " + std::to_string(tpc) + " teams";
@@ -905,7 +770,7 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
     if(par_ok)
     {
         const bool x = kp.slope || kp.rolloff || kp.normalize || kp.fast_peaks || kp.skip_mask || kp.out_peak || kp.g_tab;
-        WF_CUDA(e, par16384_launch(x, kp, e->d_tw1, e->d_tw2, e->d_tw0, st, e->device));
+        WF_CHECK(e, par16384_launch(x, kp, e->d_tw1, e->d_tw2, e->d_tw0, st, e->device));
         e->launches++;
         e->last_kernel = "stft16384_parity_kernel<" + std::to_string((int)x) + "> " + std::to_string(kp.n_streams) + " clusters of 2";
         return WF_OK;
@@ -937,7 +802,7 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
         const cudaError_t rc = warp2_launch(N, x, disp, kp, grid, &wpc, st, e->use_pdl, e->device, &name);
         if(rc != cudaErrorInvalidConfiguration) // (a curve too long for one warp's share of shared memory falls through)
         {
-            WF_CUDA(e, rc);
+            WF_CHECK(e, rc);
             e->launches++;
             e->last_kernel = std::string(name) + " N=" + std::to_string(N) + " grid " + std::to_string(grid) + " x " + std::to_string(wpc) + " warps";
             return WF_OK;
@@ -952,36 +817,35 @@ int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
         return WF_ERR_INVALID_ARG;
     NvtxRange nvtx("wf_process");
     if(b->struct_size != sizeof(wf_batch))
-        return set_err(e, WF_ERR_ABI, "wf_batch.struct_size %u != %zu", b->struct_size, sizeof(wf_batch));
+        return fail(e, WF_ERR_ABI, "wf_batch.struct_size %u != %zu", b->struct_size, sizeof(wf_batch));
     const Tables &t = e->tab;
     const int cc = t.cfg.capture_channels, dch = t.display_channels, B = t.B, N = t.N;
     if(b->n_streams < 0 || b->n_frames < 0 || b->hop < 1)
-        return set_err(e, WF_ERR_INVALID_ARG, "n_streams/n_frames must be >= 0 and hop >= 1");
+        return fail(e, WF_ERR_INVALID_ARG, "n_streams/n_frames must be >= 0 and hop >= 1");
     if(b->first_stream < 0 || (int64_t)b->first_stream + b->n_streams > t.cfg.max_streams)
-        return set_err(e, WF_ERR_CAPACITY, "streams [%d, %d) exceed max_streams %d", b->first_stream,
+        return fail(e, WF_ERR_CAPACITY, "streams [%d, %d) exceed max_streams %d", b->first_stream,
                        b->first_stream + b->n_streams, t.cfg.max_streams);
     if(b->n_streams == 0 || b->n_frames == 0)
         return WF_OK;
     if(!b->pcm)
-        return set_err(e, WF_ERR_INVALID_ARG, "pcm is null");
+        return fail(e, WF_ERR_INVALID_ARG, "pcm is null");
     if(b->stream_stride < 0 || b->channel_stride < 0)
-        return set_err(e, WF_ERR_INVALID_ARG, "negative strides are not supported");
+        return fail(e, WF_ERR_INVALID_ARG, "negative strides are not supported");
     if(t.cfg.normalize_volume && !b->input_rms)
-        return set_err(e, WF_ERR_INVALID_ARG, "normalize_volume is set but the batch carries no input_rms (m_input_rms per tick: "
+        return fail(e, WF_ERR_INVALID_ARG, "normalize_volume is set but the batch carries no input_rms (m_input_rms per tick: "
                                               "wf_meter in WF_METER_INPUT_RMS mode, or the host's own update_input_rms)");
     if((b->out_points || b->out_pixels || b->out_min) && t.num_points <= 0)
-        return set_err(e, WF_ERR_INVALID_ARG, "display outputs requested but the engine has no display points");
+        return fail(e, WF_ERR_INVALID_ARG, "display outputs requested but the engine has no display points");
 
-    WF_CUDA(e, cudaSetDevice(e->device));
+    WF_CHECK(e, cudaSetDevice(e->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : e->stream;
     const size_t S = (size_t)b->n_streams, T = (size_t)b->n_frames;
     // per-tick gravity (TVEXPONENTIAL only): evaluated on the host exactly as get_gravity(seconds) does, one pair per tick
     const float *d_gtab = nullptr;
     if(b->frame_seconds != nullptr && t.cfg.tsmoothing == WF_TSMOOTH_TVEXPONENTIAL)
     {
-        int rcg = ensure(e, &e->s_gtab, &e->s_gtab_cap, 2 * T);
-        if(rcg)
-            return rcg;
+        if(int rc = e->s_gtab.reserve(e, 2 * T))
+            return rc;
         e->h_gtab.resize(2 * T);
         for(size_t i = 0; i < T; ++i)
         {
@@ -989,7 +853,7 @@ int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
             e->h_gtab[2 * i] = g;
             e->h_gtab[2 * i + 1] = 1.0f - g;
         }
-        WF_CUDA(e, cudaMemcpyAsync(e->s_gtab, e->h_gtab.data(), 2 * T * sizeof(float), cudaMemcpyHostToDevice, st));
+        WF_CHECK(e, cudaMemcpyAsync(e->s_gtab, e->h_gtab.data(), 2 * T * sizeof(float), cudaMemcpyHostToDevice, st));
         d_gtab = e->s_gtab;
     }
     bool dev_ptrs = false;
@@ -1018,7 +882,7 @@ int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
 
     if(dev_ptrs)
     {
-        WF_CUDA(e, cudaEventRecord(e->ev0, st));
+        WF_CHECK(e, cudaEventRecord(e->ev0, st));
         if(b->out_peak)
         {
             int rc = fill_device(e, b->out_peak, (long long)T, -INFINITY, st);
@@ -1029,7 +893,7 @@ int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
                               b->out_silent, b->out_peak, b->out_pixels, b->out_min, d_gtab);
         if(rc)
             return rc;
-        WF_CUDA(e, cudaEventRecord(e->ev1, st));
+        WF_CHECK(e, cudaEventRecord(e->ev1, st));
         e->ev_valid = true;
         return WF_OK;
     }
@@ -1039,80 +903,45 @@ int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
     //      real overlap, pageable memory still works but serialises) ----
     const size_t per_stream_span = (size_t)(cc - 1) * (size_t)b->channel_stride + (T - 1) * (size_t)b->hop + (size_t)N;
     const size_t span = (S - 1) * (size_t)b->stream_stride + per_stream_span;
+    // device buffer of each host buffer the batch carries (null where the batch has none)
     int rc;
-    if((rc = ensure(e, &e->s_pcm, &e->s_pcm_cap, span)))
+    auto stage = [&](auto &buf, const void *host, size_t n) -> decltype(buf.p) {
+        if(!host || rc)
+            return nullptr;
+        rc = buf.reserve(e, n);
+        return buf.p;
+    };
+    rc = e->s_pcm.reserve(e, span);
+    float *d_out_db = stage(e->s_out_db, b->out_db, S * T * dch * B);
+    float *d_out_points = stage(e->s_out_points, b->out_points, S * T * dch * t.num_points);
+    float *d_rms = stage(e->s_rms, b->input_rms, S * T);
+    unsigned char *d_skip = stage(e->s_skip, b->skip_mask, S * T);
+    unsigned char *d_silent = stage(e->s_silent, b->out_silent, S * T);
+    float *d_peak = stage(e->s_peak, b->out_peak, T);
+    float *d_px = stage(e->s_px, b->out_pixels, S * T * dch * t.num_points);
+    float *d_min = stage(e->s_min, b->out_min, S * T * 2);
+    if(rc)
         return rc;
-    float *d_out_db = nullptr, *d_out_points = nullptr, *d_rms = nullptr, *d_peak = nullptr;
-    unsigned char *d_skip = nullptr, *d_silent = nullptr;
-    if(b->out_db)
-    {
-        if((rc = ensure(e, &e->s_out_db, &e->s_out_db_cap, S * T * dch * B)))
-            return rc;
-        d_out_db = e->s_out_db;
-    }
-    if(b->out_points)
-    {
-        if((rc = ensure(e, &e->s_out_points, &e->s_out_points_cap, S * T * dch * t.num_points)))
-            return rc;
-        d_out_points = e->s_out_points;
-    }
-    if(b->input_rms)
-    {
-        if((rc = ensure(e, &e->s_rms, &e->s_rms_cap, S * T)))
-            return rc;
-        d_rms = e->s_rms;
-    }
-    if(b->skip_mask)
-    {
-        if((rc = ensure(e, &e->s_skip, &e->s_skip_cap, S * T)))
-            return rc;
-        d_skip = e->s_skip;
-    }
-    if(b->out_silent)
-    {
-        if((rc = ensure(e, &e->s_silent, &e->s_silent_cap, S * T)))
-            return rc;
-        d_silent = e->s_silent;
-    }
-    if(b->out_peak)
-    {
-        if((rc = ensure(e, &e->s_peak, &e->s_peak_cap, T)))
-            return rc;
-        d_peak = e->s_peak;
-    }
-    float *d_px = nullptr, *d_min = nullptr;
-    if(b->out_pixels)
-    {
-        if((rc = ensure(e, &e->s_px, &e->s_px_cap, S * T * dch * t.num_points)))
-            return rc;
-        d_px = e->s_px;
-    }
-    if(b->out_min)
-    {
-        if((rc = ensure(e, &e->s_min, &e->s_min_cap, S * T * 2)))
-            return rc;
-        d_min = e->s_min;
-    }
     if(!e->s_h2d)
     {
-        WF_CUDA(e, cudaStreamCreateWithFlags(&e->s_h2d, cudaStreamNonBlocking));
-        WF_CUDA(e, cudaStreamCreateWithFlags(&e->s_d2h, cudaStreamNonBlocking));
+        WF_CHECK(e, cudaStreamCreateWithFlags(&e->s_h2d, cudaStreamNonBlocking));
+        WF_CHECK(e, cudaStreamCreateWithFlags(&e->s_d2h, cudaStreamNonBlocking));
         for(auto &ev : e->chunk_in)
-            WF_CUDA(e, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+            WF_CHECK(e, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
         for(auto &ev : e->chunk_k)
-            WF_CUDA(e, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-        WF_CUDA(e, cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
-        WF_CUDA(e, cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming));
+            WF_CHECK(e, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        WF_CHECK(e, cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
+        WF_CHECK(e, cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming));
     }
     const size_t in_bytes = span * sizeof(float);
     int nchunks = (int)std::min<size_t>(std::min<size_t>(wf_engine::kMaxChunks, S), std::max<size_t>(1, in_bytes >> 25));
     const int per = (int)((S + nchunks - 1) / nchunks);
     nchunks = (int)((S + per - 1) / per);
 
-    WF_CUDA(e, cudaEventRecord(e->ev0, st));
-    WF_CUDA(e, cudaEventRecord(e->ev_fork, st));
-    WF_CUDA(e, cudaStreamWaitEvent(e->s_h2d, e->ev_fork, 0));
-    WF_CUDA(e, cudaStreamWaitEvent(e->s_d2h, e->ev_fork, 0));
+    WF_CHECK(e, cudaEventRecord(e->ev0, st));
+    WF_CHECK(e, cudaEventRecord(e->ev_fork, st));
+    WF_CHECK(e, cudaStreamWaitEvent(e->s_h2d, e->ev_fork, 0));
+    WF_CHECK(e, cudaStreamWaitEvent(e->s_d2h, e->ev_fork, 0));
     if(d_peak)
     {
         if((rc = fill_device(e, d_peak, (long long)T, -INFINITY, st)))
@@ -1124,44 +953,44 @@ int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
         const int cnt = std::min<int>(per, (int)S - s0);
         const size_t off = (size_t)s0 * (size_t)b->stream_stride;
         const size_t cspan = (size_t)(cnt - 1) * (size_t)b->stream_stride + per_stream_span;
-        WF_CUDA(e, cudaMemcpyAsync(e->s_pcm + off, b->pcm + off, cspan * sizeof(float), cudaMemcpyHostToDevice, e->s_h2d));
+        WF_CHECK(e, cudaMemcpyAsync(e->s_pcm + off, b->pcm + off, cspan * sizeof(float), cudaMemcpyHostToDevice, e->s_h2d));
         if(d_rms)
-            WF_CUDA(e, cudaMemcpyAsync(d_rms + (size_t)s0 * T, b->input_rms + (size_t)s0 * T, (size_t)cnt * T * sizeof(float),
+            WF_CHECK(e, cudaMemcpyAsync(d_rms + (size_t)s0 * T, b->input_rms + (size_t)s0 * T, (size_t)cnt * T * sizeof(float),
                                        cudaMemcpyHostToDevice, e->s_h2d));
         if(d_skip)
-            WF_CUDA(e, cudaMemcpyAsync(d_skip + (size_t)s0 * T, b->skip_mask + (size_t)s0 * T, (size_t)cnt * T,
+            WF_CHECK(e, cudaMemcpyAsync(d_skip + (size_t)s0 * T, b->skip_mask + (size_t)s0 * T, (size_t)cnt * T,
                                        cudaMemcpyHostToDevice, e->s_h2d));
-        WF_CUDA(e, cudaEventRecord(e->chunk_in[c], e->s_h2d));
-        WF_CUDA(e, cudaStreamWaitEvent(st, e->chunk_in[c], 0));
+        WF_CHECK(e, cudaEventRecord(e->chunk_in[c], e->s_h2d));
+        WF_CHECK(e, cudaStreamWaitEvent(st, e->chunk_in[c], 0));
         if((rc = launch_range(e, b, st, s0, cnt, e->s_pcm, d_rms, d_skip, d_out_db, d_out_points, d_silent, d_peak, d_px,
                               d_min, d_gtab)))
             return rc;
-        WF_CUDA(e, cudaEventRecord(e->chunk_k[c], st));
-        WF_CUDA(e, cudaStreamWaitEvent(e->s_d2h, e->chunk_k[c], 0));
+        WF_CHECK(e, cudaEventRecord(e->chunk_k[c], st));
+        WF_CHECK(e, cudaStreamWaitEvent(e->s_d2h, e->chunk_k[c], 0));
         if(b->out_db)
-            WF_CUDA(e, cudaMemcpyAsync(b->out_db + (size_t)s0 * T * dch * B, d_out_db + (size_t)s0 * T * dch * B,
+            WF_CHECK(e, cudaMemcpyAsync(b->out_db + (size_t)s0 * T * dch * B, d_out_db + (size_t)s0 * T * dch * B,
                                        (size_t)cnt * T * dch * B * sizeof(float), cudaMemcpyDeviceToHost, e->s_d2h));
         if(b->out_points)
-            WF_CUDA(e, cudaMemcpyAsync(b->out_points + (size_t)s0 * T * dch * t.num_points,
+            WF_CHECK(e, cudaMemcpyAsync(b->out_points + (size_t)s0 * T * dch * t.num_points,
                                        d_out_points + (size_t)s0 * T * dch * t.num_points,
                                        (size_t)cnt * T * dch * t.num_points * sizeof(float), cudaMemcpyDeviceToHost, e->s_d2h));
         if(b->out_silent)
-            WF_CUDA(e, cudaMemcpyAsync(b->out_silent + (size_t)s0 * T, d_silent + (size_t)s0 * T, (size_t)cnt * T,
+            WF_CHECK(e, cudaMemcpyAsync(b->out_silent + (size_t)s0 * T, d_silent + (size_t)s0 * T, (size_t)cnt * T,
                                        cudaMemcpyDeviceToHost, e->s_d2h));
         if(b->out_pixels)
-            WF_CUDA(e, cudaMemcpyAsync(b->out_pixels + (size_t)s0 * T * dch * t.num_points,
+            WF_CHECK(e, cudaMemcpyAsync(b->out_pixels + (size_t)s0 * T * dch * t.num_points,
                                        d_px + (size_t)s0 * T * dch * t.num_points,
                                        (size_t)cnt * T * dch * t.num_points * sizeof(float), cudaMemcpyDeviceToHost, e->s_d2h));
         if(b->out_min)
-            WF_CUDA(e, cudaMemcpyAsync(b->out_min + (size_t)s0 * T * 2, d_min + (size_t)s0 * T * 2,
+            WF_CHECK(e, cudaMemcpyAsync(b->out_min + (size_t)s0 * T * 2, d_min + (size_t)s0 * T * 2,
                                        (size_t)cnt * T * 2 * sizeof(float), cudaMemcpyDeviceToHost, e->s_d2h));
     }
-    WF_CUDA(e, cudaEventRecord(e->ev1, st));
+    WF_CHECK(e, cudaEventRecord(e->ev1, st));
     e->ev_valid = true;
     if(b->out_peak) // complete only after the last chunk's kernel
-        WF_CUDA(e, cudaMemcpyAsync(b->out_peak, d_peak, T * sizeof(float), cudaMemcpyDeviceToHost, e->s_d2h));
-    WF_CUDA(e, cudaEventRecord(e->ev_join, e->s_d2h));
-    WF_CUDA(e, cudaStreamWaitEvent(st, e->ev_join, 0)); // the caller's stream completes when the results are home
+        WF_CHECK(e, cudaMemcpyAsync(b->out_peak, d_peak, T * sizeof(float), cudaMemcpyDeviceToHost, e->s_d2h));
+    WF_CHECK(e, cudaEventRecord(e->ev_join, e->s_d2h));
+    WF_CHECK(e, cudaStreamWaitEvent(st, e->ev_join, 0)); // the caller's stream completes when the results are home
     return WF_OK;
 }
 
@@ -1170,7 +999,7 @@ int wf_process(wf_engine *e, const wf_batch *b)
     int rc = wf_process_async(e, b, nullptr);
     if(rc)
         return rc;
-    WF_CUDA(e, cudaStreamSynchronize(e->stream));
+    WF_CHECK(e, cudaStreamSynchronize(e->stream));
     return WF_OK;
 }
 
@@ -1178,8 +1007,8 @@ int wf_synchronize(wf_engine *e)
 {
     if(!e)
         return WF_ERR_INVALID_ARG;
-    WF_CUDA(e, cudaSetDevice(e->device));
-    WF_CUDA(e, cudaStreamSynchronize(e->stream));
+    WF_CHECK(e, cudaSetDevice(e->device));
+    WF_CHECK(e, cudaStreamSynchronize(e->stream));
     return WF_OK;
 }
 
@@ -1188,10 +1017,10 @@ int wf_reset_state(wf_engine *e, int32_t first, int32_t count)
     if(!e)
         return WF_ERR_INVALID_ARG;
     if(first < 0 || count < 0 || (int64_t)first + count > e->tab.cfg.max_streams)
-        return set_err(e, WF_ERR_CAPACITY, "reset range out of bounds");
+        return fail(e, WF_ERR_CAPACITY, "reset range out of bounds");
     if(count == 0)
         return WF_OK;
-    WF_CUDA(e, cudaSetDevice(e->device));
+    WF_CHECK(e, cudaSetDevice(e->device));
     // on the device, per stream, so that a stream that is already silent keeps its buffers exactly as the reference's
     // early return does (src/source_generic.cpp:38-39)
     const Tables &t = e->tab;
@@ -1201,9 +1030,9 @@ int wf_reset_state(wf_engine *e, int32_t first, int32_t count)
     spectrum_reset_kernel<<<std::min(count, e->sm_count * 8), 256, 0, e->stream>>>(
         e->d_state + (size_t)first * t.cfg.capture_channels * B, e->d_hold + (size_t)first * t.output_channels * B, e->d_flags + first,
         count, (int)(t.cfg.capture_channels * B), (int)(t.output_channels * B), (int)(t.display_channels * B), t.db_min, fl);
-    WF_CUDA(e, cudaGetLastError());
+    WF_CHECK(e, cudaGetLastError());
     e->launches++;
-    WF_CUDA(e, cudaStreamSynchronize(e->stream));
+    WF_CHECK(e, cudaStreamSynchronize(e->stream));
     return WF_OK;
 }
 
@@ -1213,22 +1042,22 @@ int wf_get_state(wf_engine *e, int32_t first, int32_t count, float *tsmooth, flo
         return WF_ERR_INVALID_ARG;
     const Tables &t = e->tab;
     if(first < 0 || count < 0 || (int64_t)first + count > t.cfg.max_streams)
-        return set_err(e, WF_ERR_CAPACITY, "state range out of bounds");
-    WF_CUDA(e, cudaSetDevice(e->device));
+        return fail(e, WF_ERR_CAPACITY, "state range out of bounds");
+    WF_CHECK(e, cudaSetDevice(e->device));
     {
         const int rc = materialize_hold(e, e->stream);
         if(rc)
             return rc;
     }
-    WF_CUDA(e, cudaStreamSynchronize(e->stream));
+    WF_CHECK(e, cudaStreamSynchronize(e->stream));
     const size_t cc = (size_t)t.cfg.capture_channels, och = (size_t)t.output_channels, B = (size_t)t.B;
     if(tsmooth)
-        WF_CUDA(e, cudaMemcpy(tsmooth, e->d_state + first * cc * B, count * cc * B * sizeof(float), cudaMemcpyDeviceToHost));
+        WF_CHECK(e, cudaMemcpy(tsmooth, e->d_state + first * cc * B, count * cc * B * sizeof(float), cudaMemcpyDeviceToHost));
     if(hold_db)
-        WF_CUDA(e, cudaMemcpy(hold_db, e->d_hold + first * och * B, count * och * B * sizeof(float), cudaMemcpyDeviceToHost));
+        WF_CHECK(e, cudaMemcpy(hold_db, e->d_hold + first * och * B, count * och * B * sizeof(float), cudaMemcpyDeviceToHost));
     if(flags)
     {
-        WF_CUDA(e, cudaMemcpy(flags, e->d_flags + first, (size_t)count, cudaMemcpyDeviceToHost));
+        WF_CHECK(e, cudaMemcpy(flags, e->d_flags + first, (size_t)count, cudaMemcpyDeviceToHost));
         for(int i = 0; i < count; ++i)
             flags[i] &= 1u;
     }
@@ -1242,22 +1071,22 @@ int wf_set_state(wf_engine *e, int32_t first, int32_t count, const float *tsmoot
         return WF_ERR_INVALID_ARG;
     const Tables &t = e->tab;
     if(first < 0 || count < 0 || (int64_t)first + count > t.cfg.max_streams)
-        return set_err(e, WF_ERR_CAPACITY, "state range out of bounds");
-    WF_CUDA(e, cudaSetDevice(e->device));
+        return fail(e, WF_ERR_CAPACITY, "state range out of bounds");
+    WF_CHECK(e, cudaSetDevice(e->device));
     {
         const int rc = materialize_hold(e, e->stream);
         if(rc)
             return rc;
     }
-    WF_CUDA(e, cudaStreamSynchronize(e->stream));
+    WF_CHECK(e, cudaStreamSynchronize(e->stream));
     const size_t cc = (size_t)t.cfg.capture_channels, och = (size_t)t.output_channels, B = (size_t)t.B;
     if(tsmooth)
-        WF_CUDA(e, cudaMemcpy(e->d_state + first * cc * B, tsmooth, count * cc * B * sizeof(float), cudaMemcpyHostToDevice));
+        WF_CHECK(e, cudaMemcpy(e->d_state + first * cc * B, tsmooth, count * cc * B * sizeof(float), cudaMemcpyHostToDevice));
     std::vector<unsigned char> fl((size_t)count);
-    WF_CUDA(e, cudaMemcpy(fl.data(), e->d_flags + first, (size_t)count, cudaMemcpyDeviceToHost));
+    WF_CHECK(e, cudaMemcpy(fl.data(), e->d_flags + first, (size_t)count, cudaMemcpyDeviceToHost));
     if(hold_db)
     {
-        WF_CUDA(e, cudaMemcpy(e->d_hold + first * och * B, hold_db, count * och * B * sizeof(float), cudaMemcpyHostToDevice));
+        WF_CHECK(e, cudaMemcpy(e->d_hold + first * och * B, hold_db, count * och * B * sizeof(float), cudaMemcpyHostToDevice));
         const float thr = (float)(t.cfg.floor_db - 10);
         for(int s = 0; s < count; ++s)
         {
@@ -1283,7 +1112,7 @@ int wf_set_state(wf_engine *e, int32_t first, int32_t count, const float *tsmoot
     if(flags)
         for(int s = 0; s < count; ++s)
             fl[s] = (unsigned char)((fl[s] & ~1u) | (flags[s] & 1u));
-    WF_CUDA(e, cudaMemcpy(e->d_flags + first, fl.data(), (size_t)count, cudaMemcpyHostToDevice));
+    WF_CHECK(e, cudaMemcpy(e->d_flags + first, fl.data(), (size_t)count, cudaMemcpyHostToDevice));
     return WF_OK;
 }
 
@@ -1291,11 +1120,11 @@ int wf_peak_normalize(wf_engine *e, float *data, int32_t n_streams, int32_t n_fr
                       const float *peak, float target_db, float max_gain, void *cuda_stream)
 {
     if(!e || !data || !peak || n_streams < 0 || n_frames < 0 || row_len < 1)
-        return e ? set_err(e, WF_ERR_INVALID_ARG, "bad peak_normalize arguments") : WF_ERR_INVALID_ARG;
+        return e ? fail(e, WF_ERR_INVALID_ARG, "bad peak_normalize arguments") : WF_ERR_INVALID_ARG;
     NvtxRange nvtx("wf_peak_normalize");
     if(n_streams == 0 || n_frames == 0)
         return WF_OK;
-    WF_CUDA(e, cudaSetDevice(e->device));
+    WF_CHECK(e, cudaSetDevice(e->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : e->stream;
     const int rows_per_frame = e->tab.display_channels;
     const size_t total = (size_t)n_streams * n_frames * rows_per_frame * row_len;
@@ -1305,36 +1134,35 @@ int wf_peak_normalize(wf_engine *e, float *data, int32_t n_streams, int32_t n_fr
     if(!dev)
     {
         int rc;
-        if((rc = ensure(e, &e->s_out_db, &e->s_out_db_cap, total)))
+        if((rc = e->s_out_db.reserve(e, total)))
             return rc;
-        if((rc = ensure(e, &e->s_peak, &e->s_peak_cap, (size_t)n_frames)))
+        if((rc = e->s_peak.reserve(e, (size_t)n_frames)))
             return rc;
-        WF_CUDA(e, cudaMemcpyAsync(e->s_out_db, data, total * sizeof(float), cudaMemcpyHostToDevice, st));
-        WF_CUDA(e, cudaMemcpyAsync(e->s_peak, peak, (size_t)n_frames * sizeof(float), cudaMemcpyHostToDevice, st));
+        WF_CHECK(e, cudaMemcpyAsync(e->s_out_db, data, total * sizeof(float), cudaMemcpyHostToDevice, st));
+        WF_CHECK(e, cudaMemcpyAsync(e->s_peak, peak, (size_t)n_frames * sizeof(float), cudaMemcpyHostToDevice, st));
         d_data = e->s_out_db;
         d_peak = e->s_peak;
     }
     else if(!is_device_ptr(peak))
     {
-        int rc;
-        if((rc = ensure(e, &e->s_peak, &e->s_peak_cap, (size_t)n_frames)))
+        if(int rc = e->s_peak.reserve(e, (size_t)n_frames))
             return rc;
-        WF_CUDA(e, cudaMemcpyAsync(e->s_peak, peak, (size_t)n_frames * sizeof(float), cudaMemcpyHostToDevice, st));
+        WF_CHECK(e, cudaMemcpyAsync(e->s_peak, peak, (size_t)n_frames * sizeof(float), cudaMemcpyHostToDevice, st));
         d_peak = e->s_peak;
     }
-    WF_CUDA(e, cudaEventRecord(e->ev0, st));
+    WF_CHECK(e, cudaEventRecord(e->ev0, st));
     const long long rows = (long long)n_streams * n_frames * rows_per_frame;
     const int grid = (int)std::min<long long>(rows, (long long)e->sm_count * 16);
     peak_normalize_kernel<<<grid, 256, 0, st>>>(d_data, n_streams, n_frames, rows_per_frame, row_len, d_peak, target_db,
                                                 max_gain);
-    WF_CUDA(e, cudaGetLastError());
+    WF_CHECK(e, cudaGetLastError());
     e->launches++;
-    WF_CUDA(e, cudaEventRecord(e->ev1, st));
+    WF_CHECK(e, cudaEventRecord(e->ev1, st));
     e->ev_valid = true;
     if(!dev)
     {
-        WF_CUDA(e, cudaMemcpyAsync(data, d_data, total * sizeof(float), cudaMemcpyDeviceToHost, st));
-        WF_CUDA(e, cudaStreamSynchronize(st));
+        WF_CHECK(e, cudaMemcpyAsync(data, d_data, total * sizeof(float), cudaMemcpyDeviceToHost, st));
+        WF_CHECK(e, cudaStreamSynchronize(st));
     }
     return WF_OK;
 }
@@ -1360,16 +1188,6 @@ int64_t wf_launch_count(const wf_engine *e) { return e ? e->launches : 0; }
 
 const char *wf_last_kernel_name(const wf_engine *e) { return e ? e->last_kernel.c_str() : ""; }
 
-float wf_last_kernel_ms(wf_engine *e)
-{
-    if(!e || !e->ev_valid)
-        return -1.0f;
-    if(cudaEventSynchronize(e->ev1) != cudaSuccess)
-        return -1.0f;
-    float ms = -1.0f;
-    if(cudaEventElapsedTime(&ms, e->ev0, e->ev1) != cudaSuccess)
-        return -1.0f;
-    return ms;
-}
+float wf_last_kernel_ms(wf_engine *e) { return last_kernel_ms(e); }
 
 } // extern "C"

@@ -1,0 +1,104 @@
+// wf_host.cu — the parts of the shared host layer (wf_host.hpp) that cannot live in the header: fill_kernel, and the
+// functions around CUDA calls that all three engines make the same way.
+#include "wf_host.hpp"
+
+#include <algorithm>
+#include <cstdarg>
+#include <cstdio>
+
+namespace wf {
+
+static __global__ void fill_kernel(float *p, long long n, float v)
+{
+    for(long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        p[i] = v;
+}
+
+HostCore::~HostCore()
+{
+    if(ev0)
+        cudaEventDestroy(ev0);
+    if(ev1)
+        cudaEventDestroy(ev1);
+    if(stream)
+        cudaStreamDestroy(stream);
+}
+
+int fail(HostCore *c, int code, const char *fmt, ...)
+{
+    if(c)
+    {
+        char buf[512];
+        va_list ap;
+        va_start(ap, fmt);
+        vsnprintf(buf, sizeof(buf), fmt, ap);
+        va_end(ap);
+        c->last_error = buf;
+    }
+    return code;
+}
+
+int open_device(HostCore *c, int requested)
+{
+    int ndev = 0;
+    if(cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+    {
+        cudaGetLastError();
+        return fail(c, WF_ERR_NO_DEVICE, "no CUDA device (this engine has no CPU fallback)");
+    }
+    int dev = requested;
+    if(dev < 0 && cudaGetDevice(&dev) != cudaSuccess)
+        return fail(c, WF_ERR_CUDA, "cudaGetDevice failed");
+    if(dev >= ndev)
+        return fail(c, WF_ERR_INVALID_ARG, "device %d out of range (%d devices)", dev, ndev);
+    c->device = dev;
+    WF_CHECK(c, cudaSetDevice(dev));
+    cudaDeviceProp prop{};
+    WF_CHECK(c, cudaGetDeviceProperties(&prop, dev));
+    if(prop.major != 9 || prop.minor != 0) // sm_90a code runs on compute capability 9.0 only
+        return fail(c, WF_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", dev, prop.major,
+                    prop.minor);
+    c->sm_count = prop.multiProcessorCount;
+    WF_CHECK(c, cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
+    WF_CHECK(c, cudaEventCreate(&c->ev0));
+    WF_CHECK(c, cudaEventCreate(&c->ev1));
+    return WF_OK;
+}
+
+int ptr_kind(const void *p)
+{
+    cudaPointerAttributes a{};
+    if(cudaPointerGetAttributes(&a, p) != cudaSuccess)
+    {
+        cudaGetLastError();
+        return 0;
+    }
+    if(a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged)
+        return 1;
+    if(a.type == cudaMemoryTypeHost && a.devicePointer == p) // unified addressing: the same pointer is valid on the device
+        return 2;
+    return 0;
+}
+
+int fill_device(HostCore *c, float *p, long long n, float v, cudaStream_t st)
+{
+    if(n <= 0)
+        return WF_OK;
+    const int blocks = (int)std::min<long long>((n + 255) / 256, 1184);
+    fill_kernel<<<blocks, 256, 0, st>>>(p, n, v);
+    WF_CHECK(c, cudaGetLastError());
+    c->launches++;
+    return WF_OK;
+}
+
+float last_kernel_ms(HostCore *c)
+{
+    if(!c || !c->ev_valid || cudaEventSynchronize(c->ev1) != cudaSuccess)
+        return -1.0f;
+    float ms = -1.0f;
+    if(cudaEventElapsedTime(&ms, c->ev0, c->ev1) != cudaSuccess)
+        return -1.0f;
+    return ms;
+}
+
+} // namespace wf

@@ -1,0 +1,224 @@
+// wf_host.hpp — the host layer the three C-ABI engines share: spectrum (wf_engine.cu), level meter / RMS feed
+// (wf_meter.cu) and waveform (wf_wave.cu).  Device, stream, timing events and error reporting (HostCore), grow-only device
+// buffers, pointer classification, struct-size compatibility, environment knobs and the staging of host buffers.  What
+// cannot live in a header (fill_kernel and the functions around CUDA calls) is in wf_host.cu.
+#pragma once
+
+#include <cuda_runtime.h>
+
+#include <cstddef>
+#include <cstdint>
+#include <cstdlib>
+#include <cstring>
+#include <new>
+#include <string>
+#include <utility>
+#include <vector>
+
+#include "wfstft.h"
+
+namespace wf {
+
+// What every engine owns besides its tables and kernels; the engine structs derive from it.  The destructor releases the
+// stream and the events: the engines' *_destroy synchronise the stream before the handle goes, so nothing is freed while a
+// kernel may still use it.
+struct HostCore {
+    int device = 0, sm_count = 0;
+    cudaStream_t stream = nullptr;            // the engine's own stream (calls without a caller stream)
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr; // around the kernels of the last call (wf_*last_kernel_ms)
+    bool ev_valid = false;
+    int64_t launches = 0;
+    std::string last_error;
+
+    HostCore() = default;
+    HostCore(const HostCore &) = delete;
+    HostCore &operator=(const HostCore &) = delete;
+    ~HostCore();
+};
+
+// Keeps the message for wf_*last_error (when there is an engine) and returns `code`.
+int fail(HostCore *c, int code, const char *fmt, ...) __attribute__((format(printf, 3, 4)));
+
+// Returns WF_ERR_OOM / WF_ERR_CUDA from the calling function, with the failing call and CUDA's reason as the message,
+// unless `call` succeeds.
+#define WF_CHECK(core, call)                                                                                       \
+    do                                                                                                             \
+    {                                                                                                              \
+        const cudaError_t _err = (call);                                                                           \
+        if(_err != cudaSuccess)                                                                                    \
+            return ::wf::fail((core), (_err == cudaErrorMemoryAllocation) ? WF_ERR_OOM : WF_ERR_CUDA, "%s failed: %s", \
+                              #call, cudaGetErrorString(_err));                                                    \
+    } while(0)
+
+// Allocates an engine, runs its create steps and hands it out.  When a step fails, the engine's message stays readable
+// through the engine kind's wf_*last_error(NULL) (`create_error`) and `destroy` releases what was set up.
+template<class E, class Init>
+int create_engine(E **out, std::string &create_error, void (*destroy)(E *), Init &&init)
+{
+    E *e = new(std::nothrow) E();
+    if(!e)
+        return WF_ERR_OOM;
+    const int rc = init(e);
+    if(rc != WF_OK)
+    {
+        create_error = e->last_error;
+        destroy(e);
+        return rc;
+    }
+    *out = e;
+    return WF_OK;
+}
+
+// Device `requested` (< 0: the current one) for a new engine: it must exist and be sm_90.  Makes it current, stores its SM
+// count and creates the engine's stream and timing events.  WF_ERR_NO_DEVICE without a CUDA device or on another
+// architecture, WF_ERR_INVALID_ARG for a device number out of range, WF_ERR_CUDA / WF_ERR_OOM when a CUDA call fails.
+int open_device(HostCore *c, int requested);
+
+// 0 = pageable host memory (or unknown), 1 = device / managed memory, 2 = page-locked host memory the device can address
+// directly under the same pointer
+int ptr_kind(const void *p);
+inline bool is_device_ptr(const void *p) { return p && ptr_kind(p) == 1; }
+
+// p[0, n) := v on `st` (fill_kernel); counts as one launch of the engine.
+int fill_device(HostCore *c, float *p, long long n, float v, cudaStream_t st);
+
+// Milliseconds between the events around the last call's kernels, -1 before the first call or when the events fail.
+float last_kernel_ms(HostCore *c);
+
+// A device buffer that only grows: reserve(n) keeps the allocation when it holds n elements already, else frees it and
+// allocates exactly n (the contents are not kept).  Freed with its owner.
+template<class T>
+struct DevBuf {
+    T *p = nullptr;
+    size_t cap = 0;
+
+    DevBuf() = default;
+    DevBuf(DevBuf &&o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+    DevBuf &operator=(DevBuf &&o) noexcept
+    {
+        std::swap(p, o.p);
+        std::swap(cap, o.cap);
+        return *this;
+    }
+    ~DevBuf()
+    {
+        if(p)
+            cudaFree(p);
+    }
+    operator T *() const { return p; }
+
+    int reserve(HostCore *c, size_t n)
+    {
+        if(n <= cap)
+            return WF_OK;
+        if(p)
+            cudaFree(p);
+        p = nullptr;
+        cap = 0;
+        WF_CHECK(c, cudaMalloc((void **)&p, n * sizeof(T)));
+        cap = n;
+        return WF_OK;
+    }
+    // a table uploaded once at create time; an empty table leaves the buffer null
+    int upload(HostCore *c, const std::vector<T> &v)
+    {
+        if(v.empty())
+            return WF_OK;
+        if(int rc = reserve(c, v.size()))
+            return rc;
+        WF_CHECK(c, cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+        return WF_OK;
+    }
+};
+
+// A caller's struct of the current size, or of the previous ABI's size (`prev_size`: it ends before the fields added
+// since, which then read as zero).  False for any other struct_size.  `out` carries the current struct_size either way.
+template<class T>
+bool accept_struct(const T *in, size_t prev_size, T &out, bool *is_current = nullptr)
+{
+    const bool cur = in->struct_size == sizeof(T);
+    if(!cur && in->struct_size != prev_size)
+        return false;
+    out = T{};
+    memcpy(&out, in, cur ? sizeof(T) : prev_size);
+    out.struct_size = (uint32_t)sizeof(T);
+    if(is_current)
+        *is_current = cur;
+    return true;
+}
+
+// Environment knobs (A/B switches for tests and tools).  A flag that is on by default is switched off by a value starting
+// with '0'; one that is off by default is switched on by a value starting with '1'.
+inline bool env_flag(const char *name, bool dflt)
+{
+    const char *v = getenv(name);
+    return v ? (dflt ? v[0] != '0' : v[0] == '1') : dflt;
+}
+inline int env_int(const char *name, int dflt)
+{
+    const char *v = getenv(name);
+    return v ? atoi(v) : dflt;
+}
+
+// Host buffers of one meter / waveform call, staged through the engine's grow-only device buffers on stream `st`.  With
+// `host` false (the call passed device pointers) every buffer passes through as it is.  in() uploads an input at once and
+// returns its device copy; out() returns device space for an output, and finish() copies the outputs back, after the
+// launch, in the order they were declared.  Null buffers pass through.  After a failure later declarations do nothing and
+// `rc` holds the status, which the caller checks before it launches.
+class Staging {
+  public:
+    Staging(HostCore *c, cudaStream_t st, bool host) : core(c), st(st), host(host) {}
+    int rc = WF_OK;
+
+    template<class T>
+    const T *in(DevBuf<T> &buf, const T *src, size_t n)
+    {
+        if(!take(buf, src, n))
+            return src;
+        rc = copy(buf.p, src, n * sizeof(T), cudaMemcpyHostToDevice);
+        return buf.p;
+    }
+    template<class T>
+    T *out(DevBuf<T> &buf, T *dst, size_t n)
+    {
+        if(!take(buf, dst, n))
+            return dst;
+        back[n_back++] = {dst, buf.p, n * sizeof(T)};
+        return buf.p;
+    }
+    int finish()
+    {
+        for(int i = 0; i < n_back; ++i)
+            if(int r = copy(back[i].host, back[i].dev, back[i].bytes, cudaMemcpyDeviceToHost))
+                return r;
+        return WF_OK;
+    }
+
+  private:
+    struct Back {
+        void *host;
+        const void *dev;
+        size_t bytes;
+    };
+    HostCore *core;
+    cudaStream_t st;
+    bool host;
+    Back back[8];
+    int n_back = 0;
+
+    template<class T>
+    bool take(DevBuf<T> &buf, const void *p, size_t n)
+    {
+        if(rc || !host || !p)
+            return false;
+        rc = buf.reserve(core, n);
+        return rc == WF_OK;
+    }
+    int copy(void *dst, const void *src, size_t bytes, cudaMemcpyKind kind)
+    {
+        WF_CHECK(core, cudaMemcpyAsync(dst, src, bytes, kind, st));
+        return WF_OK;
+    }
+};
+
+} // namespace wf

@@ -289,27 +289,31 @@ def _ptr(x):
     return x.ctypes.data
 
 
-class Engine:
-    def __init__(self, settings: dict | None = None, sample_rate: int = 48000, channels: int = 2,
-                 max_streams: int = 1, device: int = -1, config: WfConfig | None = None):
-        self.L = load_library()
-        self.cfg = config if config is not None else make_config(settings, sample_rate, channels, max_streams, device)
-        h = C.c_void_p()
-        rc = self.L.wf_create(C.byref(self.cfg), C.byref(h))
-        if rc != WF_OK:
-            raise WfError(rc, f"{self.L.wf_strerror(rc).decode()}: {self.L.wf_last_error(None).decode()}")
-        self.h = h
-        self.info = WfInfo()
-        self._check(self.L.wf_get_info(self.h, C.byref(self.info)))
+class _Handle:
+    """What the three engine handles share: creation, error reporting, release, launch count and kernel time.  `_prefix`
+    selects the engine kind's C functions (wf_*, wf_meter_*, wf_wave_*)."""
 
-    # ---- plumbing ----
+    _prefix = "wf"
+
+    def _fn(self, name):
+        return getattr(self.L, f"{self._prefix}_{name}")
+
+    def _create(self, cfg):
+        self.L = load_library()
+        self.cfg = cfg
+        h = C.c_void_p()
+        rc = self._fn("create")(C.byref(cfg), C.byref(h))
+        if rc != WF_OK:
+            raise WfError(rc, f"{self.L.wf_strerror(rc).decode()}: {self._fn('last_error')(None).decode()}")
+        self.h = h
+
     def _check(self, rc):
         if rc != WF_OK:
-            raise WfError(rc, f"{self.L.wf_strerror(rc).decode()}: {self.L.wf_last_error(self.h).decode()}")
+            raise WfError(rc, f"{self.L.wf_strerror(rc).decode()}: {self._fn('last_error')(self.h).decode()}")
 
     def close(self):
         if getattr(self, "h", None):
-            self.L.wf_destroy(self.h)
+            self._fn("destroy")(self.h)
             self.h = None
 
     def __del__(self):
@@ -317,6 +321,61 @@ class Engine:
             self.close()
         except Exception:
             pass
+
+    @property
+    def launch_count(self) -> int:
+        return int(self._fn("launch_count")(self.h))
+
+    def last_kernel_ms(self) -> float:
+        return float(self._fn("last_kernel_ms")(self.h))
+
+
+class _Inputs:
+    """The shared prelude of the engines' process(): `pcm` as [S, channels, samples] (a 2-D array is one stream), checked
+    against the engine's channel count and the samples the call needs.  A numpy array becomes contiguous float32 (host
+    path); a torch tensor must be a contiguous float32 CUDA tensor (device path), and `stream` is then torch's current
+    stream.  new() allocates an output and aux() brings an optional per-tick input to the same side as pcm."""
+
+    def __init__(self, pcm, channels: int, need: int, who: str = "engine"):
+        self.is_torch = hasattr(pcm, "data_ptr")
+        if pcm.ndim == 2:
+            pcm = pcm[None]
+        self.S, self.cc, self.ns = pcm.shape
+        if self.cc != channels:
+            raise ValueError(f"pcm has {self.cc} channels, {who} captures {channels}")
+        if self.ns < need:
+            raise ValueError(f"need {need} samples per channel, got {self.ns}")
+        self.stream = None
+        if self.is_torch:
+            import torch
+            assert pcm.is_cuda and pcm.dtype == torch.float32 and pcm.is_contiguous()
+            self.f32, self.u8 = torch.float32, torch.uint8
+            self.stream = torch.cuda.current_stream(pcm.device).cuda_stream
+        else:
+            pcm = np.ascontiguousarray(pcm, dtype=np.float32)
+            self.f32, self.u8 = np.float32, np.uint8
+        self.pcm = pcm
+
+    def new(self, shape, dtype):
+        if self.is_torch:
+            import torch
+            return torch.empty(shape, dtype=dtype, device=self.pcm.device)
+        return np.empty(shape, dtype=dtype)
+
+    def aux(self, x, dtype):
+        if x is None:
+            return None
+        if self.is_torch:
+            return x.to(device=self.pcm.device, dtype=dtype).contiguous()
+        return np.ascontiguousarray(x, dtype=dtype)
+
+
+class Engine(_Handle):
+    def __init__(self, settings: dict | None = None, sample_rate: int = 48000, channels: int = 2,
+                 max_streams: int = 1, device: int = -1, config: WfConfig | None = None):
+        self._create(config if config is not None else make_config(settings, sample_rate, channels, max_streams, device))
+        self.info = WfInfo()
+        self._check(self.L.wf_get_info(self.h, C.byref(self.info)))
 
     # ---- facts ----
     @property
@@ -365,13 +424,6 @@ class Engine:
         self.L.wf_get_table(self.h, which, out.ctypes.data, n)
         return out
 
-    @property
-    def launch_count(self) -> int:
-        return int(self.L.wf_launch_count(self.h))
-
-    def last_kernel_ms(self) -> float:
-        return float(self.L.wf_last_kernel_ms(self.h))
-
     def last_kernel_name(self) -> str:
         return self.L.wf_last_kernel_name(self.h).decode()
 
@@ -403,34 +455,11 @@ class Engine:
                 frame_seconds=None):
         """pcm: [n_streams, capture_channels, samples] float32 — numpy (host path, staged inside the C call)
         or a CUDA torch tensor (device path, outputs are CUDA tensors)."""
-        is_torch = hasattr(pcm, "data_ptr")
-        if pcm.ndim == 2:
-            pcm = pcm[None]
-        S, cc, ns = pcm.shape
-        if cc != self.capture_channels:
-            raise ValueError(f"pcm has {cc} channels, engine captures {self.capture_channels}")
-        need = (n_frames - 1) * hop + self.fft_size
-        if ns < need:
-            raise ValueError(f"need {need} samples per channel, got {ns}")
+        x = _Inputs(pcm, self.capture_channels, (n_frames - 1) * hop + self.fft_size)
+        S, cc, ns, mk, f32, u8 = x.S, x.cc, x.ns, x.new, x.f32, x.u8
+        input_rms, skip_mask = x.aux(input_rms, f32), x.aux(skip_mask, u8)
         dch, B, P = self.display_channels, self.bins, self.num_points
         out = {}
-        if is_torch:
-            import torch
-            assert pcm.is_cuda and pcm.dtype == torch.float32 and pcm.is_contiguous()
-            mk = lambda shape, dt: torch.empty(shape, dtype=dt, device=pcm.device)
-            f32, u8 = torch.float32, torch.uint8
-            if input_rms is not None:
-                input_rms = input_rms.to(device=pcm.device, dtype=f32).contiguous()
-            if skip_mask is not None:
-                skip_mask = skip_mask.to(device=pcm.device, dtype=u8).contiguous()
-        else:
-            pcm = np.ascontiguousarray(pcm, dtype=np.float32)
-            mk = lambda shape, dt: np.empty(shape, dtype=dt)
-            f32, u8 = np.float32, np.uint8
-            if input_rms is not None:
-                input_rms = np.ascontiguousarray(input_rms, dtype=np.float32)
-            if skip_mask is not None:
-                skip_mask = np.ascontiguousarray(skip_mask, dtype=np.uint8)
         if want_db:
             out["db"] = mk((S, n_frames, dch, B), f32)
         if want_points:
@@ -445,19 +474,15 @@ class Engine:
         # CUDA tensors: launch on torch's CURRENT stream, so the kernel is ordered after whatever produced `pcm` and before
         # whatever consumes the outputs (torch semantics: asynchronous, stream-ordered).  Host arrays: the engine's own
         # stream, synchronised before returning.
-        stream = None
-        if is_torch:
-            import torch
-            stream = torch.cuda.current_stream(pcm.device).cuda_stream
         fs = None
         if frame_seconds is not None:  # per-tick `seconds` (always a host array), see wf_batch.frame_seconds
             fs = np.ascontiguousarray(frame_seconds, dtype=np.float32)
             assert fs.shape == (n_frames,)
-        self.process_raw(_ptr(pcm), S, n_frames, hop, cc * ns, ns, first_stream=first_stream, seconds=seconds,
+        self.process_raw(_ptr(x.pcm), S, n_frames, hop, cc * ns, ns, first_stream=first_stream, seconds=seconds,
                          input_rms=_ptr(input_rms), skip_mask=_ptr(skip_mask), out_db=_ptr(out.get("db")),
                          out_points=_ptr(out.get("points")), out_silent=_ptr(out.get("silent")),
                          out_peak=_ptr(out.get("peak")), out_pixels=_ptr(out.get("pixels")), out_min=_ptr(out.get("min")),
-                         stream=stream, sync=not is_torch, frame_seconds=None if fs is None else fs.ctypes.data)
+                         stream=x.stream, sync=not x.is_torch, frame_seconds=None if fs is None else fs.ctypes.data)
         return out
 
     def synchronize(self):
@@ -524,41 +549,15 @@ def make_meter_config(settings: dict | None = None, sample_rate: int = 48000, ch
     return c
 
 
-class MeterEngine:
+class MeterEngine(_Handle):
     """Level meter (tick_meter) / RMS feed (update_input_rms) on the GPU: ctypes over wf_meter_*; no DSP here."""
+
+    _prefix = "wf_meter"
 
     def __init__(self, settings: dict | None = None, sample_rate: int = 48000, channels: int = 2, max_streams: int = 1,
                  device: int = -1, mode: int | None = None):
-        self.L = load_library()
-        self.cfg = make_meter_config(settings, sample_rate, channels, max_streams, device, mode)
-        h = C.c_void_p()
-        rc = self.L.wf_meter_create(C.byref(self.cfg), C.byref(h))
-        if rc != WF_OK:
-            raise WfError(rc, f"{self.L.wf_strerror(rc).decode()}: {self.L.wf_meter_last_error(None).decode()}")
-        self.h = h
+        self._create(make_meter_config(settings, sample_rate, channels, max_streams, device, mode))
         self.window = int(self.L.wf_meter_window(self.h))
-
-    def _check(self, rc):
-        if rc != WF_OK:
-            raise WfError(rc, f"{self.L.wf_strerror(rc).decode()}: {self.L.wf_meter_last_error(self.h).decode()}")
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.wf_meter_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    @property
-    def launch_count(self) -> int:
-        return int(self.L.wf_meter_launch_count(self.h))
-
-    def last_kernel_ms(self) -> float:
-        return float(self.L.wf_meter_last_kernel_ms(self.h))
 
     def reset(self, first_stream=0, count=None):
         count = self.cfg.max_streams - first_stream if count is None else count
@@ -569,34 +568,19 @@ class MeterEngine:
         Returns dict(db, lin, silent) — or dict(rms=[S, T]) for an INPUT_RMS engine.  want_pixels adds the bar heights
         render_bars draws, pixels=[S, T, capture_channels], and min=[S, T, 2] (miny, minpos).  CUDA tensors without an
         explicit `stream` run on torch's current stream."""
-        is_torch = hasattr(pcm, "data_ptr")
-        if pcm.ndim == 2:
-            pcm = pcm[None]
-        S, cc, ns = pcm.shape
-        if cc != self.cfg.capture_channels:
-            raise ValueError(f"pcm has {cc} channels, meter captures {self.cfg.capture_channels}")
-        if ns < n_ticks * hop:
-            raise ValueError(f"need {n_ticks * hop} samples per channel, got {ns}")
-        if is_torch:
-            import torch
-            assert pcm.is_cuda and pcm.dtype == torch.float32 and pcm.is_contiguous()
-            mk = lambda shape, dt: torch.empty(shape, dtype=dt, device=pcm.device)
-            f32, u8 = torch.float32, torch.uint8
-        else:
-            pcm = np.ascontiguousarray(pcm, dtype=np.float32)
-            mk = lambda shape, dt: np.empty(shape, dtype=dt)
-            f32, u8 = np.float32, np.uint8
+        x = _Inputs(pcm, self.cfg.capture_channels, n_ticks * hop, "meter")
+        S, cc, ns, mk, f32, u8 = x.S, x.cc, x.ns, x.new, x.f32, x.u8
         feed = self.cfg.mode == METER_INPUT_RMS
         out = {"rms": mk((S, n_ticks), f32)} if feed else {
             "db": mk((S, n_ticks, cc), f32), "lin": mk((S, n_ticks, cc), f32), "silent": mk((S, n_ticks), u8)}
         if want_pixels:
             out["pixels"], out["min"] = mk((S, n_ticks, cc), f32), mk((S, n_ticks, 2), f32)
-        if is_torch and stream is None:
-            stream = torch.cuda.current_stream(pcm.device).cuda_stream
+        if stream is None:
+            stream = x.stream
         b = WfMeterBatch()
         b.struct_size = C.sizeof(WfMeterBatch)
         b.n_streams, b.n_ticks, b.hop, b.first_stream, b.seconds = S, n_ticks, hop, first_stream, seconds
-        b.pcm, b.stream_stride, b.channel_stride = _ptr(pcm), cc * ns, ns
+        b.pcm, b.stream_stride, b.channel_stride = _ptr(x.pcm), cc * ns, ns
         b.out_db = None if feed else _ptr(out["db"])
         b.out_lin = _ptr(out["rms"]) if feed else _ptr(out["lin"])
         b.out_silent = None if feed else _ptr(out["silent"])
@@ -637,41 +621,15 @@ def make_wave_config(settings: dict | None = None, sample_rate: int = 48000, cha
     return c
 
 
-class WaveEngine:
+class WaveEngine(_Handle):
     """Waveform (oscilloscope) mode (tick_waveform) on the GPU: ctypes over wf_wave_*; no DSP here."""
+
+    _prefix = "wf_wave"
 
     def __init__(self, settings: dict | None = None, sample_rate: int = 48000, channels: int = 2, max_streams: int = 1,
                  device: int = -1):
-        self.L = load_library()
-        self.cfg = make_wave_config(settings, sample_rate, channels, max_streams, device)
-        h = C.c_void_p()
-        rc = self.L.wf_wave_create(C.byref(self.cfg), C.byref(h))
-        if rc != WF_OK:
-            raise WfError(rc, f"{self.L.wf_strerror(rc).decode()}: {self.L.wf_wave_last_error(None).decode()}")
-        self.h = h
+        self._create(make_wave_config(settings, sample_rate, channels, max_streams, device))
         self.display_channels = 2 if self.cfg.stereo else 1
-
-    def _check(self, rc):
-        if rc != WF_OK:
-            raise WfError(rc, f"{self.L.wf_strerror(rc).decode()}: {self.L.wf_wave_last_error(self.h).decode()}")
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.wf_wave_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    @property
-    def launch_count(self) -> int:
-        return int(self.L.wf_wave_launch_count(self.h))
-
-    def last_kernel_ms(self) -> float:
-        return float(self.L.wf_wave_last_kernel_ms(self.h))
 
     def reset(self):
         self._check(self.L.wf_wave_reset(self.h))
@@ -683,27 +641,9 @@ class WaveEngine:
         computes from each tick's rows: points (interpolated + smoothed dB), pixels and min=[S, T, 2] (miny, minpos), all
         [S, T, display_channels, width].  want_db=False leaves `out` out (a display-only call).  CUDA tensors without an
         explicit `stream` run on torch's current stream."""
-        is_torch = hasattr(pcm, "data_ptr")
-        if pcm.ndim == 2:
-            pcm = pcm[None]
-        S, cc, ns = pcm.shape
-        if cc != self.cfg.capture_channels:
-            raise ValueError(f"pcm has {cc} channels, engine captures {self.cfg.capture_channels}")
-        if ns < n_ticks * hop:
-            raise ValueError(f"need {n_ticks * hop} samples per channel, got {ns}")
-        if is_torch:
-            import torch
-            assert pcm.is_cuda and pcm.dtype == torch.float32 and pcm.is_contiguous()
-            mk = lambda shape, dt: torch.empty(shape, dtype=dt, device=pcm.device)
-            f32, u8 = torch.float32, torch.uint8
-            if input_rms is not None:
-                input_rms = input_rms.to(device=pcm.device, dtype=f32).contiguous()
-        else:
-            pcm = np.ascontiguousarray(pcm, dtype=np.float32)
-            mk = lambda shape, dt: np.empty(shape, dtype=dt)
-            f32, u8 = np.float32, np.uint8
-            if input_rms is not None:
-                input_rms = np.ascontiguousarray(input_rms, dtype=np.float32)
+        x = _Inputs(pcm, self.cfg.capture_channels, n_ticks * hop)
+        S, cc, ns, mk, f32, u8 = x.S, x.cc, x.ns, x.new, x.f32, x.u8
+        input_rms = x.aux(input_rms, f32)
         shape = (S, n_ticks, self.display_channels, self.cfg.width)
         out = {"silent": mk((S, n_ticks), u8)}
         if want_db:
@@ -712,12 +652,12 @@ class WaveEngine:
             out["points"] = mk(shape, f32)
         if want_pixels:
             out["pixels"], out["min"] = mk(shape, f32), mk((S, n_ticks, 2), f32)
-        if is_torch and stream is None:
-            stream = torch.cuda.current_stream(pcm.device).cuda_stream
+        if stream is None:
+            stream = x.stream
         b = WfWaveBatch()
         b.struct_size = C.sizeof(WfWaveBatch)
         b.n_streams, b.n_ticks, b.hop = S, n_ticks, hop
-        b.pcm, b.stream_stride, b.channel_stride = _ptr(pcm), cc * ns, ns
+        b.pcm, b.stream_stride, b.channel_stride = _ptr(x.pcm), cc * ns, ns
         b.input_rms, b.out, b.out_silent = _ptr(input_rms), _ptr(out.get("out")), _ptr(out["silent"])
         b.out_points, b.out_pixels, b.out_min = _ptr(out.get("points")), _ptr(out.get("pixels")), _ptr(out.get("min"))
         if stream is None:
