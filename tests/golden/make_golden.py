@@ -180,8 +180,55 @@ def main_stall():
         print("stall", name, "N", N, "skipped ticks", skipped, "db at first skipped tick: max", float(db[J].max()))
 
 
+# Reference yardsticks for the float64 tests (tests/test_fp64_reference.py, tests/test_gpu_fp64.py): one small case per
+# FFT plan family of the engine, with what the reference's generic (FFTW) path produced.  Its error against the float64
+# restatement (tests/fp64_spectrum.py) is the figure a GPU kernel is held to at that size.
+FP64_CASES = {
+    "2048": dict(settings={"fft_size": 2048, "window": "hann"}, channels=1),
+    "1456": dict(settings={"fft_size": 1456, "window": "hann"}, channels=1),              # 2^4 7 13
+    "1664": dict(settings={"fft_size": 1664, "window": "blackman_harris"}, channels=1),   # 2^7 13
+    "1408": dict(settings={"fft_size": 1408, "window": "hann"}, channels=1),              # 2^7 11
+    "1792": dict(settings={"fft_size": 1792, "window": "hamming"}, channels=1),           # 2^8 7
+    "800": dict(settings={"fft_size": 800, "window": "blackman"}, channels=1),            # 2^5 5^2
+    "4096_stereo": dict(settings={"fft_size": 4096, "window": "hann", "channel_mode": "stereo"}, channels=2),
+    "16384": dict(settings={"fft_size": 16384, "window": "hann"}, channels=1),
+    "40000": dict(settings={"fft_size": 40000, "window": "hann"}, channels=1),            # 2^6 5^4
+    "65344": dict(settings={"fft_size": 65344, "window": "hann"}, channels=1),            # 2^6 1021
+    "65488": dict(settings={"fft_size": 65488, "window": "hann"}, channels=1),            # 2^4 4093
+}
+FP64_T = 3
+
+
+def _savez_fixed(path, **arrays):
+    """np.savez_compressed with a fixed member timestamp, so that a regeneration is byte for byte the same file."""
+    import zipfile
+
+    with zipfile.ZipFile(path, "w", compression=zipfile.ZIP_DEFLATED) as zf:
+        for key, val in arrays.items():
+            info = zipfile.ZipInfo(key + ".npy", date_time=(1980, 1, 1, 0, 0, 0))
+            info.compress_type = zipfile.ZIP_DEFLATED
+            with zf.open(info, "w", force_zip64=True) as f:
+                np.lib.format.write_array(f, np.asanyarray(val), allow_pickle=False)
+
+
+def main_fp64():
+    for name, c in FP64_CASES.items():
+        ref = RefSource(c["settings"], impl=IMPL_GENERIC, channels=c["channels"])
+        N, cc, T = ref.fft_size, ref.capture_channels, FP64_T
+        hop = N // 2
+        pcm = synth_pcm(1, cc, (T - 1) * hop + N, seed=0xF640 + N)[0]
+        r = ref.run_stft(pcm, T, hop, seconds=1.0 / 60.0, want_points=False, fma3=False)
+        _savez_fixed(OUT / f"fp64_{name}.npz", settings=json.dumps(c["settings"]), channels=c["channels"], hop=hop,
+                     n_frames=T, seconds=1.0 / 60.0, pcm=pcm, db=r["db"], silent=r["silent"],
+                     db_min=np.float32(ref.db_min))
+        print("fp64", name, "N", N, "db", r["db"].shape)
+
+
 if __name__ == "__main__":
     import sys
+    if "--fp64-only" in sys.argv:
+        main_fp64()
+        sys.exit(0)
     if "--stall-only" in sys.argv:
         main_stall()
         sys.exit(0)
@@ -193,3 +240,4 @@ if __name__ == "__main__":
         main_wave()
     if "--meter-only" not in sys.argv and "--wave-only" not in sys.argv:
         main_stall()
+        main_fp64()

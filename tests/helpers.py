@@ -103,21 +103,3 @@ def device_pcm(n_streams: int, channels: int, n_samples: int, seed: int = 0xB200
         zero = ((b + 3 * s) % zero_every) == 0          # [S, nb]
         blk[zero[:, None, :].expand(n_streams, channels, nb)] = 0.0
     return pcm
-
-
-def fp64_truth_db(pcm, window, window_sum, n_frames, hop, g, db_min=-758.59564):
-    """Double-precision ground truth of the plain pipeline (window -> DFT -> |X| 2/sum(w) -> EMA -> dBFS) for one mono
-    stream, from the SAME float32 window table (so that only the arithmetic differs): SURVEY.md §7 'both
-    implementations' error vs fp64 truth'.  pcm: [samples] float32."""
-    N = len(window)
-    w = window.astype(np.float64)
-    coef = 2.0 / float(window_sum)
-    state = np.zeros(N // 2)
-    out = np.empty((n_frames, N // 2))
-    for t in range(n_frames):
-        x = pcm[t * hop: t * hop + N].astype(np.float64) * w
-        mag = np.abs(np.fft.rfft(x)[: N // 2]) * coef
-        state = g * state + (1.0 - g) * mag
-        with np.errstate(divide="ignore"):
-            out[t] = np.where(state > 0, 20.0 * np.log10(np.maximum(state, 1e-300)), db_min)
-    return out

@@ -129,12 +129,13 @@ def test_fp64_arbiter_reference_and_oracle():
     """SURVEY §4(ii)/§7: the error of the reference's FFTW path (golden vectors) and of the oracle's own fp32 FFT against
     a double-precision ground truth computed from the same float32 window table.  Both are ~1e-7 normwise; the GPU
     variant of this test (tests/test_gpu_scale.py) holds the CUDA path to the same yardstick."""
-    from helpers import fp64_truth_db
+    from fp64_spectrum import Fp64Spectrum
 
     z, settings = _load(Path(__file__).parent / "golden" / "case_c3_mono_2048_hann.npz")
     T, hop = int(z["n_frames"]), int(z["hop"])
-    truth = fp64_truth_db(z["pcm"][0], z["window"], float(z["window_sum"]), T, hop, g=np.float64(np.float32(0.65)))
-    got = OracleSource(settings, channels=1).run_stft(z["pcm"], T, hop)["db"][:, 0]
+    o = OracleSource(settings, channels=1)
+    truth = Fp64Spectrum(settings, channels=1).run(z["pcm"], T, hop, o.gravity(float(z["seconds"])))["db"][:, 0]
+    got = o.run_stft(z["pcm"], T, hop, seconds=float(z["seconds"]))["db"][:, 0]
     lin = lambda d: np.power(10.0, np.asarray(d, np.float64) / 20.0)
     peak = lin(truth).max(axis=-1, keepdims=True)
     err_ref = (np.abs(lin(z["db"][:, 0]) - lin(truth)) / peak).max()
