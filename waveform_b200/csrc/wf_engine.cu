@@ -9,6 +9,9 @@
 
 #include <cmath>
 #include <algorithm>
+#include <array>
+#include <cstdio>
+#include <utility>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -28,21 +31,27 @@
 
 using namespace wf;
 
+// Environment knobs of the spectrum engine, read at wf_create: A/B switches for tests and tools.  None changes a result.
+struct SpectrumKnobs {
+    bool force_generic = env_flag("WF_FORCE_GENERIC", false); // bypass the specialised N=2048 kernels
+    bool v3 = env_flag("WF_V3", true);             // 0: the first-generation kernels instead of the CTA-per-tick kernel
+    int wide_r = env_int("WF_WIDE_R", 0);          // 1|2|4|8: cluster size of the wide and CTA-per-tick kernels (1 = no
+                                                   // wide kernel); 0 = automatic
+    int team_w = env_int("WF_TEAM_W", 0);          // 4|8|16: team size of wf_team2048.cuh; 1 = never a team; 0 = automatic
+    bool par16384 = env_flag("WF_PAR16384", true); // 0: N=16384 stays on the CTA-per-tick kernel
+    bool warp2 = env_flag("WF_WARP2", true);       // 0: non-power-of-two sizes stay on the any-N kernel
+    bool warp2_display = env_flag("WF_WARP2_DISPLAY", true); // 0: display outputs stay on the CTA-per-tick / any-N kernels
+    bool split = env_flag("WF_SPLIT", true);       // 0: whole streams per warp in the N=2048 warp-per-stream kernel
+    bool zero_copy = env_flag("WF_ZERO_COPY", true); // 0: always stage host buffers through device memory
+};
+
 struct wf_engine : HostCore {
     Tables tab;
     std::string last_kernel;    // name of the spectrum kernel the most recent launch_range dispatched to (wf_last_kernel_name)
-    bool hold_implicit = false; // some stream may carry flags bit 3 (m_decibels mirror left implicit by the N=2048 kernel)
-    bool use_par16384 = true;   // WF_PAR16384=0: N=16384 stays on the CTA-per-tick kernel (A/B tests)
-    bool use_warp2_display = true; // WF_WARP2_DISPLAY=0: display outputs stay on the CTA-per-tick / any-N kernels (A/B tests)
-    bool use_warp2 = true;      // WF_WARP2=0: non-power-of-two sizes stay on the first-generation any-N kernel (A/B tests)
-    bool lazy_hold = true;      // WF_LAZY_HOLD=0: always write the mirror (A/B tests)
-    bool split_runs = true;     // WF_SPLIT=0: whole streams per warp in the N=2048 warp-per-stream kernel (A/B tests)
-    bool force_generic = false; // WF_FORCE_GENERIC=1: bypass the specialised N=2048 kernel (A/B tests)
-    int fast_wpc_override = 0;  // WF_FAST_WPC=n: force warps per CTA (tuning knob)
-    bool use_pdl = true;        // WF_NO_PDL=1: launch the fast kernel without programmatic dependent launch
-    int wide_r = 0;             // WF_WIDE_R=1|2|4|8: force the cluster size of the wide kernel (1 = never use it); 0 = automatic
-    int team_w = 0;             // WF_TEAM_W=4|8|16: force the team size of wf_team2048.cuh; 1: never use it; 0 = automatic
-    bool use_v3 = true;         // WF_V3=0: fall back to the first-generation kernels (A/B tests)
+    bool hold_implicit = false; // some stream may carry flags bit 3 (m_decibels mirror left implicit by the N=2048 kernels)
+    SpectrumKnobs knobs;
+    Warp2Plan warp2;            // compiled warp-per-stream plan of this fft size (L == 0: none)
+    AnyPlan any{};              // run-time plan of the any-N kernel (sizes without a templated kernel)
 
     // device tables
     DevBuf<float> d_window, d_slope, d_rolloff, d_tw, d_tw_post;
@@ -61,7 +70,6 @@ struct wf_engine : HostCore {
     // zero-copy verdict of the last host-pointer batch (live ticks reuse the same buffers every call)
     const void *zc_ptrs[9] = {};
     bool zc_ok = false, zc_dev = false, zc_valid = false;
-    bool zero_copy = true; // WF_ZERO_COPY=0: always stage host buffers through device memory
     // copy/compute pipeline for host-pointer batches
     static constexpr int kMaxChunks = 16;
     cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
@@ -187,24 +195,45 @@ bool supported_fft_size(int n)
     return n <= 65536; // sizes whose work buffers exceed shared memory run from a global (L2) scratch
 }
 
-template<int N, int CC>
-int launch_fused(wf_engine *e, const KParams &kp, cudaStream_t st, size_t extra_smem)
+// What one call runs: the kernel family, its template arguments and the launch shape the host picks for it.  The shapes of
+// the parity, CTA-per-tick, wide and fused kernels follow from their template arguments.
+enum class Family { fast, team, parity, warp2, v3, wide, fused, anyn };
+struct Route {
+    Family family;
+    int x = 0;                      // EXTRA: options in use (0 / 1); the CTA-per-tick kernel: 0, 1 (out_peak only) or 3
+    bool tsm = false, gate = false; // fast: temporal smoothing, silence gate
+    int w = 0;                      // fast, warp2: warps per CTA; team: warps per stream
+    int r = 1;                      // v3, wide: CTAs per cluster
+    int grid = 0;                   // fast, team, warp2, any-N: CTAs
+    size_t smem = 0;                // warp2, any-N: dynamic shared memory bytes
+    bool scratch = false;           // any-N: work buffers in an L2 scratch instead of shared memory
+    bool display = false;           // warp2: the display variant
+    int disp_tab_bytes = 0, disp_bytes = 0; // warp2 with display outputs: per-CTA tables, per-warp rows
+};
+
+// What routing needs to know about one call, worked out once from its KParams.
+struct CallFacts {
+    bool display;   // curve points, pixels or minimum requested
+    bool opts;      // slope, roll-off, volume, fast peaks, skip mask, peak output or per-tick gravity in use
+    int v3_x;       // the CTA-per-tick kernel's level of options: 0, 1 (peak output only) or 3
+    bool aligned16; // frames can be loaded in 16-byte units (pcm, stream stride and hop)
+    bool db16;      // out_db is 16-byte aligned (the N=2048 kernels write each dB row with one bulk copy)
+};
+
+CallFacts call_facts(const KParams &kp)
 {
-    using G = Geo<N>;
-    const size_t smem = (size_t)G::GROUPS * G::BUF * sizeof(float2) + extra_smem;
-    static thread_local size_t configured[64] = {0};
-    int dev = e->device & 63;
-    if(smem > 48 * 1024 && configured[dev] < smem)
-    {
-        WF_CHECK(e, cudaFuncSetAttribute(stft_fused_kernel<N, CC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured[dev] = smem;
-    }
-    const int grid = (kp.n_streams + G::GROUPS - 1) / G::GROUPS;
-    stft_fused_kernel<N, CC><<<grid, G::CTA, smem, st>>>(kp);
-    WF_CHECK(e, cudaGetLastError());
-    e->launches++;
-    e->last_kernel = "stft_fused_kernel<" + std::to_string(N) + "," + std::to_string(CC) + ">";
-    return WF_OK;
+    const bool opts_but_peak = kp.slope || kp.rolloff || kp.normalize || kp.fast_peaks || kp.skip_mask || kp.g_tab;
+    return {.display = kp.out_points || kp.out_pixels || kp.out_min,
+            .opts = opts_but_peak || kp.out_peak,
+            .v3_x = opts_but_peak ? 3 : (kp.out_peak ? 1 : 0),
+            .aligned16 = (((uintptr_t)kp.pcm & 15u) == 0) && ((kp.stream_stride & 3) == 0) && ((kp.hop & 3) == 0),
+            .db16 = ((uintptr_t)kp.out_db & 15u) == 0};
+}
+
+// Shared memory of the display stage in the fused and any-N kernels: [groups][2][dch <= 2][num_points] floats
+size_t display_smem(const KParams &kp, const CallFacts &f, int groups)
+{
+    return f.display ? (size_t)groups * 4 * (size_t)kp.scratch_q * sizeof(float) : 0;
 }
 
 // Cluster size of the wide kernel (wf_wide.cuh) for this launch, 1 = use the one-group-per-stream kernel.
@@ -212,12 +241,12 @@ int launch_fused(wf_engine *e, const KParams &kp, cudaStream_t st, size_t extra_
 int pick_wide_r(const wf_engine *e, const KParams &kp, bool display)
 {
     const int N = e->tab.N;
-    if(!wide_supported(N) || e->wide_r == 1)
+    if(!wide_supported(N) || e->knobs.wide_r == 1)
         return 1;
     if(wide_smem_bytes(N, kp.dch, kp.scratch_q, display) > 227 * 1024)
         return 1;
-    if(e->wide_r == 2 || e->wide_r == 4 || e->wide_r == 8)
-        return e->wide_r;
+    if(e->knobs.wide_r == 2 || e->knobs.wide_r == 4 || e->knobs.wide_r == 8)
+        return e->knobs.wide_r;
     int r = 1;
     while(r < 8 && (long long)kp.n_streams * r < 2LL * e->sm_count && 2 * r <= kp.n_frames)
         r *= 2;
@@ -228,84 +257,18 @@ int pick_wide_r(const wf_engine *e, const KParams &kp, bool display)
 // (= 8 ticks in flight) per stream.
 int pick_v3_r(const wf_engine *e, const KParams &kp)
 {
-    const int rmin = v3_min_cluster(e->tab.N);
-    if(e->wide_r == 1 || e->wide_r == 2 || e->wide_r == 4 || e->wide_r == 8)
-        return std::max(rmin, e->wide_r);
+    const int rmin = v3_min_cluster(e->tab.N), wide_r = e->knobs.wide_r;
+    if(wide_r == 1 || wide_r == 2 || wide_r == 4 || wide_r == 8)
+        return std::max(rmin, wide_r);
     int r = rmin;
     while(r < 8 && (long long)kp.n_streams * r * 3 < 5LL * e->sm_count && 2 * r <= kp.n_frames) // per-tick overhead grows with R
         r *= 2;
     return r;
 }
 
-template<int CC>
-int dispatch_n(wf_engine *e, const KParams &kp, cudaStream_t st, size_t extra)
-{
-    {
-        const bool display = kp.out_points || kp.out_pixels || kp.out_min;
-        if(e->use_v3 && e->d_tw1 != nullptr && v3_smem_bytes(e->tab.N, kp.dch, kp.scratch_q, display, CC, 8) <= 227 * 1024)
-        {
-            const bool feat = kp.slope || kp.rolloff || kp.normalize || kp.fast_peaks || kp.skip_mask || kp.g_tab;
-            const int x = feat ? 3 : (kp.out_peak ? 1 : 0);
-            const int r = pick_v3_r(e, kp);
-            WF_CHECK(e, v3_launch(e->tab.N, CC, r, x, kp, e->d_tw1, e->d_tw2, e->d_tw0, st, display, e->device));
-            e->launches++;
-            e->last_kernel = "stft_v3_kernel<" + std::to_string(e->tab.N) + "," + std::to_string(CC) + "," + std::to_string(r) +
-                             "," + std::to_string(x) + ">";
-            return WF_OK;
-        }
-        const int R = pick_wide_r(e, kp, display);
-        if(R > 1)
-        {
-            WF_CHECK(e, wide_launch(e->tab.N, CC, R, kp, st, display, e->device));
-            e->launches++;
-            e->last_kernel = "stft_wide_kernel<" + std::to_string(e->tab.N) + "," + std::to_string(CC) + "," + std::to_string(R) + ">";
-            return WF_OK;
-        }
-    }
-    switch(e->tab.N)
-    {
-    case 128: return launch_fused<128, CC>(e, kp, st, extra);
-    case 256: return launch_fused<256, CC>(e, kp, st, extra);
-    case 512: return launch_fused<512, CC>(e, kp, st, extra);
-    case 1024: return launch_fused<1024, CC>(e, kp, st, extra);
-    case 2048: return launch_fused<2048, CC>(e, kp, st, extra);
-    case 4096: return launch_fused<4096, CC>(e, kp, st, extra);
-    case 8192: return launch_fused<8192, CC>(e, kp, st, extra);
-    case 16384: return launch_fused<16384, CC>(e, kp, st, extra);
-    case 32768: return launch_fused<32768, CC>(e, kp, st, extra);
-    default: break;
-    }
-    // any other multiple of 16: run-time mixed-radix kernel
-    AnyPlan plan;
-    if(!make_any_plan(e->tab.N, &plan))
-        return fail(e, WF_ERR_UNSUPPORTED_FFT_SIZE, "fft_size %d has no kernel", e->tab.N);
-    const bool in_smem = (size_t)plan.M * 16 + extra <= 200 * 1024;
-    int grid = std::min(kp.n_streams, e->sm_count * (in_smem ? 8 : 2));
-    size_t smem = in_smem ? (size_t)plan.M * 16 + extra : extra;
-    plan.scratch = nullptr;
-    if(!in_smem)
-    {
-        if(int rc = e->s_scratch.reserve(e, (size_t)grid * 2 * plan.M * 2))
-            return rc;
-        plan.scratch = reinterpret_cast<float2 *>(e->s_scratch.p);
-    }
-    static thread_local size_t configured[64] = {0};
-    const int dev = e->device & 63;
-    if(smem > 48 * 1024 && configured[dev] < smem)
-    {
-        WF_CHECK(e, cudaFuncSetAttribute(stft_anyn_kernel<CC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured[dev] = smem;
-    }
-    stft_anyn_kernel<CC><<<grid, kAnyThreads, smem, st>>>(kp, plan);
-    WF_CHECK(e, cudaGetLastError());
-    e->launches++;
-    e->last_kernel = "stft_anyn_kernel<" + std::to_string(CC) + "> N=" + std::to_string(e->tab.N);
-    return WF_OK;
-}
-
 // One CTA per SM; the kernel deals streams round-robin to CTAs first, so each SM gets n_streams/grid (+-1) whole
 // streams (the unit of work: EMA state stays on-chip across a stream's frames) and runs min(max_wpc, that) warps.
-static void fast2048_geometry(int n_streams, int sm_count, int max_wpc, int *warps_per_cta, int *grid)
+void fast2048_geometry(int n_streams, int sm_count, int max_wpc, int *warps_per_cta, int *grid)
 {
     *grid = std::min(n_streams, sm_count);
     const int per_cta = (n_streams + *grid - 1) / *grid;
@@ -314,59 +277,152 @@ static void fast2048_geometry(int n_streams, int sm_count, int max_wpc, int *war
     *warps_per_cta = std::max(std::min(8, max_wpc), std::min(max_wpc, per_cta));
 }
 
-template<int MAXW, bool TSM, bool GATE, bool EXTRA>
-int launch_fast2048(wf_engine *e, const KParams &kp, cudaStream_t st)
+// Warps per stream of the N=2048 team kernel (wf_team2048.cuh), 1 = the warp-per-stream kernel.  Fewer streams than SMs x 16
+// warps: a team of W warps per stream works on W ticks at once.  Up to 8 streams per SM: 16 / W = 1, 2 or 4 teams per SM (a
+// team takes its streams one after the other); measured (profiles/r02_layouts.txt) 256 x 256: 142 -> 272 M spectra/s,
+// 512 x 128: 200 -> 310 M, 1024 x 64: 289 -> 332 M.
+int pick_team_w(const wf_engine *e, const KParams &kp)
 {
-    static thread_local bool configured[64] = {false};
-    const int dev = e->device & 63;
-    if(!configured[dev])
-    {
-        WF_CHECK(e, cudaFuncSetAttribute(stft2048_fast_kernel<MAXW, TSM, GATE, EXTRA>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, fast::smem_bytes(MAXW)));
-        configured[dev] = true;
-    }
-    int wpc = MAXW, grid = 1;
-    fast2048_geometry(kp.n_streams, e->sm_count, MAXW, &wpc, &grid);
-    if(e->fast_wpc_override > 0 && e->fast_wpc_override <= MAXW)
-    {
-        wpc = e->fast_wpc_override;
-        grid = std::min(kp.n_streams, e->sm_count);
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3((unsigned)(wpc * 32));
-    cfg.dynamicSmemBytes = fast::smem_bytes(wpc);
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; // PDL: prologue overlaps the previous launch's tail
-    attr[0].val.programmaticStreamSerializationAllowed = e->use_pdl ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    WF_CHECK(e, cudaLaunchKernelEx(&cfg, stft2048_fast_kernel<MAXW, TSM, GATE, EXTRA>, kp));
-    e->launches++;
-    e->last_kernel = "stft2048_fast_kernel<" + std::to_string(MAXW) + "," + std::to_string((int)TSM) + "," + std::to_string((int)GATE) +
-                     "," + std::to_string((int)EXTRA) + "> grid " + std::to_string(grid) + " x " + std::to_string(wpc) + " warps";
-    return WF_OK;
+    const int team_w = e->knobs.team_w;
+    if(team_w == 1)
+        return 1;
+    int W = 1;
+    const int per_sm = (kp.n_streams + e->sm_count - 1) / e->sm_count;
+    if(per_sm <= 8)
+        W = (per_sm <= 1) ? 16 : (per_sm == 2) ? 8 : 4;
+    if(team_w == 4 || team_w == 8 || team_w == 16)
+        W = team_w;
+    while(W > 1 && W > kp.n_frames)
+        W /= 2;
+    return (W == 2) ? 1 : W;
 }
 
-
-// Hand-specialised path for the headline shape (see wf_fast2048.cuh); everything else takes the generic kernel.
-int dispatch_fast2048(wf_engine *e, const KParams &kp, cudaStream_t st, bool extra)
+// Warps per CTA of the warp-per-stream kernel for N = 2*L*P (wf_warp2.cuh) and its shared memory, into `r`; false when not
+// even one warp's display rows fit (the call then goes to the next family).
+bool fit_warp2(const wf_engine *e, const KParams &kp, bool display, Route &r)
 {
-    const bool tsm = kp.tsmooth != 0, gate = kp.gate != 0;
-#define WF_FAST_CASE(T, G, X)                  \
-    if(tsm == T && gate == G && extra == X) \
-        return launch_fast2048<fast::kMaxWarpsPerCta, T, G, X>(e, kp, st);
-    WF_FAST_CASE(true, true, false)
-    WF_FAST_CASE(true, true, true)
-    WF_FAST_CASE(true, false, false)
-    WF_FAST_CASE(true, false, true)
-    WF_FAST_CASE(false, true, false)
-    WF_FAST_CASE(false, true, true)
-    WF_FAST_CASE(false, false, false)
-    WF_FAST_CASE(false, false, true)
-#undef WF_FAST_CASE
-    return fail(e, WF_ERR_INVALID_ARG, "fast2048 dispatch fell through");
+    constexpr size_t kMaxSmem = 227 * 1024; // opt-in shared memory per CTA on sm_90
+    fast2048_geometry(kp.n_streams, e->sm_count, 16, &r.w, &r.grid);
+    if(display)
+    {
+        // shared memory of the display variant (layout in wf_warp2.cuh): per CTA the setup tables, per warp the tick's dB
+        // row, the bar sample points and — only for the Gaussian / pixel / minimum outputs — two rows of points + scratch
+        const size_t tab = display_table_floats(kp);
+        const bool need_pts = kp.filter || kp.out_pixels || kp.out_min;
+        const size_t per_warp = (size_t)e->tab.B + (size_t)kp.n_sample + (need_pts ? 2 * (size_t)kp.n_points + 64 : 0);
+        r.disp_tab_bytes = (int)((tab * sizeof(float) + 127) / 128 * 128);
+        r.disp_bytes = (int)((per_warp * sizeof(float) + 127) / 128 * 128);
+    }
+    // the display rows cost warps per SM at the largest sizes; the streams simply take more rounds
+    while(r.w > 1 && e->warp2.smem_bytes(r.w, r.disp_tab_bytes, r.disp_bytes) > kMaxSmem)
+        --r.w;
+    r.smem = e->warp2.smem_bytes(r.w, r.disp_tab_bytes, r.disp_bytes);
+    return r.smem <= kMaxSmem;
+}
+
+// The kernel a call runs, in order of precedence: the N=2048 team and warp-per-stream kernels, the N=16384 parity
+// clusters, the warp-per-stream kernel of the other sizes (and of display outputs), the CTA-per-tick clusters, the wide
+// clusters, the fused kernel of the power-of-two sizes and the any-N kernel.
+Route choose_route(const wf_engine *e, const KParams &kp, const CallFacts &f)
+{
+    const Tables &t = e->tab;
+    const SpectrumKnobs &k = e->knobs;
+    const int N = t.N, cc = t.cfg.capture_channels;
+    const bool mono = (cc == 1) && !t.cfg.stereo, x = f.opts;
+    if(N == 2048 && mono && kp.out_db && !f.display && f.aligned16 && f.db16 && !k.force_generic)
+    {
+        if(const int W = pick_team_w(e, kp); W > 1)
+            return {.family = Family::team, .x = x, .w = W, .grid = std::min(e->sm_count, kp.n_streams)};
+        Route r{.family = Family::fast, .x = x, .tsm = kp.tsmooth != 0, .gate = kp.gate != 0};
+        fast2048_geometry(kp.n_streams, e->sm_count, fast::kMaxWarpsPerCta, &r.w, &r.grid);
+        return r;
+    }
+    // N = 16384 (config 5): a cluster of two CTAs per stream splits the bins by parity, each on the spill-free N=8192 plan
+    if(N == 16384 && k.par16384 && k.v3 && e->d_tw0 && mono && kp.out_db && !f.display && !k.force_generic)
+        return {.family = Family::parity, .x = x};
+    // Non-power-of-two sizes with a compiled two-pass plan (wf_warp2.cuh): same launch shape as the N=2048 kernel.  With
+    // display outputs (curve points / bars / pixels / minimum) the same kernel runs the render-time stages per warp; that
+    // variant also takes the power-of-two sizes 512 / 1024 / 2048 (config 1: N=1024, 26 bars).
+    const bool pow2 = is_pow2_kernel_size(N);
+    if(k.warp2 && mono && f.aligned16 && e->warp2.L &&
+       (f.display ? (k.warp2_display && !k.force_generic) : (!pow2 && kp.out_db)))
+    {
+        Route r{.family = Family::warp2, .x = x, .display = f.display};
+        if(fit_warp2(e, kp, f.display, r))
+            return r;
+    }
+    if(k.v3 && e->d_tw1 != nullptr && v3_smem_bytes(N, kp.dch, kp.scratch_q, f.display, cc, 8) <= 227 * 1024)
+        return {.family = Family::v3, .x = f.v3_x, .r = pick_v3_r(e, kp)};
+    if(const int R = pick_wide_r(e, kp, f.display); R > 1)
+        return {.family = Family::wide, .r = R};
+    if(pow2)
+        return {.family = Family::fused};
+    // any other multiple of 16: the run-time mixed-radix kernel, its work buffers in shared memory or in an L2 scratch
+    const size_t extra = display_smem(kp, f, 1), work = (size_t)e->any.M * 16;
+    const bool in_smem = work + extra <= 200 * 1024;
+    return {.family = Family::anyn, .grid = std::min(kp.n_streams, e->sm_count * (in_smem ? 8 : 2)),
+            .smem = in_smem ? work + extra : extra, .scratch = !in_smem};
+}
+
+// last_kernel_name() of a route
+std::string route_name(const wf_engine *e, const Route &r, int n_streams)
+{
+    const int N = e->tab.N, cc = e->tab.cfg.capture_channels;
+    char buf[128];
+    switch(r.family)
+    {
+    case Family::fast:
+        snprintf(buf, sizeof buf, "stft2048_fast_kernel<%d,%d,%d,%d> grid %d x %d warps", fast::kMaxWarpsPerCta, (int)r.tsm,
+                 (int)r.gate, r.x, r.grid, r.w);
+        break;
+    case Family::team:
+        snprintf(buf, sizeof buf, "stft2048_team_kernel<%d,%d> grid %d x %d teams", r.w, r.x, r.grid, 16 / r.w);
+        break;
+    case Family::parity: snprintf(buf, sizeof buf, "stft16384_parity_kernel<%d> %d clusters of 2", r.x, n_streams); break;
+    case Family::warp2:
+        snprintf(buf, sizeof buf, "stft_warp2_kernel<%d,%d%s> N=%d grid %d x %d warps", e->warp2.L, e->warp2.P,
+                 r.display ? ",display" : "", N, r.grid, r.w);
+        break;
+    case Family::v3: snprintf(buf, sizeof buf, "stft_v3_kernel<%d,%d,%d,%d>", N, cc, r.r, r.x); break;
+    case Family::wide: snprintf(buf, sizeof buf, "stft_wide_kernel<%d,%d,%d>", N, cc, r.r); break;
+    case Family::fused: snprintf(buf, sizeof buf, "stft_fused_kernel<%d,%d>", N, cc); break;
+    case Family::anyn: snprintf(buf, sizeof buf, "stft_anyn_kernel<%d> N=%d", cc, N); break;
+    }
+    return buf;
+}
+
+template<int N, int CC>
+cudaError_t launch_fused(const wf_engine *e, const KParams &kp, const CallFacts &f, cudaStream_t st)
+{
+    using G = Geo<N>;
+    const size_t smem = (size_t)G::GROUPS * G::BUF * sizeof(float2) + display_smem(kp, f, G::GROUPS);
+    return launch_kernel(stft_fused_kernel<N, CC>, e->device, (kp.n_streams + G::GROUPS - 1) / G::GROUPS, G::CTA, smem, st,
+                         {}, kp);
+}
+
+template<int CC>
+cudaError_t launch_fused_n(const wf_engine *e, const KParams &kp, const CallFacts &f, cudaStream_t st)
+{
+    switch(e->tab.N)
+    {
+    case 128: return launch_fused<128, CC>(e, kp, f, st);
+    case 256: return launch_fused<256, CC>(e, kp, f, st);
+    case 512: return launch_fused<512, CC>(e, kp, f, st);
+    case 1024: return launch_fused<1024, CC>(e, kp, f, st);
+    case 2048: return launch_fused<2048, CC>(e, kp, f, st);
+    case 4096: return launch_fused<4096, CC>(e, kp, f, st);
+    case 8192: return launch_fused<8192, CC>(e, kp, f, st);
+    case 16384: return launch_fused<16384, CC>(e, kp, f, st);
+    case 32768: return launch_fused<32768, CC>(e, kp, f, st);
+    default: return cudaErrorInvalidValue;
+    }
+}
+
+// stft2048_fast_kernel<kMaxWarpsPerCta, TSM, GATE, EXTRA>, indexed by TSM * 4 + GATE * 2 + EXTRA
+template<int... I>
+std::array<void (*)(KParams), sizeof...(I)> fast_kernels(std::integer_sequence<int, I...>)
+{
+    return {stft2048_fast_kernel<fast::kMaxWarpsPerCta, (I & 4) != 0, (I & 2) != 0, (I & 1) != 0>...};
 }
 
 // Write out every implicit m_decibels mirror (see materialize_hold_kernel) before something other than the N=2048
@@ -482,18 +538,9 @@ int wf_create(const wf_config *cfg, wf_engine **out)
             return fail(e, WF_ERR_UNSUPPORTED_FFT_SIZE, "fft_size %d unsupported", e->tab.N);
         if((rc = open_device(e, cfg->device)))
             return rc;
-        e->force_generic = env_flag("WF_FORCE_GENERIC", false);
-        e->use_pdl = !env_flag("WF_NO_PDL", false);
-        e->wide_r = env_int("WF_WIDE_R", 0);
-        e->use_v3 = env_flag("WF_V3", true);
-        e->team_w = env_int("WF_TEAM_W", 0);
-        e->zero_copy = env_flag("WF_ZERO_COPY", true);
-        e->use_par16384 = env_flag("WF_PAR16384", true);
-        e->use_warp2 = env_flag("WF_WARP2", true);
-        e->use_warp2_display = env_flag("WF_WARP2_DISPLAY", true);
-        e->lazy_hold = env_flag("WF_LAZY_HOLD", true);
-        e->split_runs = env_flag("WF_SPLIT", true);
-        e->fast_wpc_override = env_int("WF_FAST_WPC", 0);
+        e->warp2 = warp2_plan(e->tab.N);
+        if(!is_pow2_kernel_size(e->tab.N))
+            make_any_plan(e->tab.N, &e->any);
 
         const Tables &t = e->tab;
         std::vector<float> tw1, tw2, tw0; // stay empty (and d_tw1 null) for sizes without the CTA-per-tick kernel
@@ -629,14 +676,72 @@ int64_t wf_preview_table(const wf_config *cfg, int which, float *out, int64_t ca
     return copy_table(t, which, out, capacity);
 }
 
-// Launch the fused kernel for streams [s0, s0+count) of the batch; all pointers are DEVICE pointers already
-// offset to stream 0 of the batch.
+// Runs a route: writes out the implicit m_decibels mirrors first unless the route is one of the N=2048 kernels (the other
+// kernels read hold_db as it is), sets the route's own KParams fields, launches, and names the kernel.
+static int launch_route(wf_engine *e, const Route &r, const CallFacts &f, KParams kp, cudaStream_t st)
+{
+    const Tables &t = e->tab;
+    const int N = t.N, cc = t.cfg.capture_channels, dev = e->device;
+    if(r.family != Family::fast && r.family != Family::team)
+    {
+        if(int rc = materialize_hold(e, st))
+            return rc;
+    }
+    cudaError_t err = cudaSuccess;
+    switch(r.family)
+    {
+    case Family::fast:
+    case Family::team:
+        kp.split = e->knobs.split ? 1 : 0;
+        kp.lazy_hold = 1;
+        e->hold_implicit = true;
+        if(r.family == Family::team)
+            err = team2048_launch(r.w, r.x, kp, r.grid, st, dev);
+        else
+        {
+            static const auto kernels = fast_kernels(std::make_integer_sequence<int, 8>{});
+            err = launch_kernel(kernels[r.tsm * 4 + r.gate * 2 + r.x], dev, r.grid, r.w * 32, fast::smem_bytes(r.w), st,
+                                {.pdl = true}, kp);
+        }
+        break;
+    case Family::parity: err = par16384_launch(r.x, kp, e->d_tw1, e->d_tw2, e->d_tw0, st, dev); break;
+    case Family::warp2:
+        kp.split = e->knobs.split ? 1 : 0;
+        kp.disp_tab_bytes = r.disp_tab_bytes;
+        kp.disp_bytes = r.disp_bytes;
+        err = e->warp2.launch[r.x][r.display](kp, r.grid, r.w, r.smem, st, dev);
+        break;
+    case Family::v3: err = v3_launch(N, cc, r.r, r.x, kp, e->d_tw1, e->d_tw2, e->d_tw0, st, f.display, dev); break;
+    case Family::wide: err = wide_launch(N, cc, r.r, kp, st, f.display, dev); break;
+    case Family::fused: err = (cc == 2) ? launch_fused_n<2>(e, kp, f, st) : launch_fused_n<1>(e, kp, f, st); break;
+    case Family::anyn:
+    {
+        AnyPlan plan = e->any;
+        plan.scratch = nullptr;
+        if(r.scratch)
+        {
+            if(int rc = e->s_scratch.reserve(e, (size_t)r.grid * 2 * plan.M * 2))
+                return rc;
+            plan.scratch = reinterpret_cast<float2 *>(e->s_scratch.p);
+        }
+        err = (cc == 2) ? launch_kernel(stft_anyn_kernel<2>, dev, r.grid, kAnyThreads, r.smem, st, {}, kp, plan)
+                        : launch_kernel(stft_anyn_kernel<1>, dev, r.grid, kAnyThreads, r.smem, st, {}, kp, plan);
+        break;
+    }
+    }
+    WF_CHECK(e, err);
+    e->launches++;
+    e->last_kernel = route_name(e, r, kp.n_streams);
+    return WF_OK;
+}
+
+// Runs streams [s0, s0+count) of the batch; all pointers are DEVICE pointers already offset to stream 0 of the batch.
 static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0, int count, const float *pcm,
                         const float *rms, const unsigned char *skip, float *out_db, float *out_points,
                         unsigned char *silent, float *out_peak, float *px_dev, float *min_dev, const float *g_tab_dev)
 {
     const Tables &t = e->tab;
-    const int cc = t.cfg.capture_channels, dch = t.display_channels, och = t.output_channels, B = t.B, N = t.N;
+    const int cc = t.cfg.capture_channels, dch = t.display_channels, och = t.output_channels, B = t.B;
     const size_t T = (size_t)b->n_frames;
     KParams kp{};
     kp.pcm = pcm + (size_t)s0 * (size_t)b->stream_stride;
@@ -704,112 +809,11 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
     kp.dbrange_f = (float)(t.cfg.ceiling_db - t.cfg.floor_db);
     kp.mirror = t.cfg.mirror_freq_axis;
 
-    // shared memory for the display stage: [groups][2][dch <= 2][num_points] floats
-    size_t extra = 0;
-    if(kp.out_points || kp.out_pixels || kp.out_min)
-    {
-        int groups = 1;
-        switch(N)
-        {
-        case 128: groups = Geo<128>::GROUPS; break;
-        case 256: groups = Geo<256>::GROUPS; break;
-        case 512: groups = Geo<512>::GROUPS; break;
-        case 1024: groups = Geo<1024>::GROUPS; break;
-        case 2048: groups = Geo<2048>::GROUPS; break;
-        default: groups = 1; break;
-        }
-        extra = (size_t)groups * 4 * (size_t)kp.scratch_q * sizeof(float);
-    }
-    const bool aligned16 = (((uintptr_t)kp.pcm & 15u) == 0) && ((b->stream_stride & 3) == 0) && ((b->hop & 3) == 0);
-    // (the fast kernel writes each dB row with one bulk copy, which needs a 16-byte aligned destination)
-    const bool fast_ok = (N == 2048) && (cc == 1) && !t.cfg.stereo && kp.out_db && !kp.out_points && !kp.out_pixels &&
-                         !kp.out_min && aligned16 && (((uintptr_t)kp.out_db & 15u) == 0) && !e->force_generic;
-    if(fast_ok)
-    {
-        const bool x = kp.slope || kp.rolloff || kp.normalize || kp.fast_peaks || kp.skip_mask || kp.out_peak || kp.g_tab;
-        kp.lazy_hold = e->lazy_hold ? 1 : 0;
-        kp.split = e->split_runs ? 1 : 0;
-        if(kp.lazy_hold)
-            e->hold_implicit = true;
-        // Fewer streams than SMs x 16 warps: a team of W warps per stream works on W ticks at once (wf_team2048.cuh).
-        // Up to 8 streams per SM: 16 / W = 1, 2 or 4 teams per SM (a team takes its streams one after the other); measured
-        // (profiles/r02_layouts.txt) 256 x 256: 142 -> 272 M spectra/s, 512 x 128: 200 -> 310 M, 1024 x 64: 289 -> 332 M.
-        int W = 1;
-        if(e->team_w != 1)
-        {
-            const int per_sm = (kp.n_streams + e->sm_count - 1) / e->sm_count;
-            if(per_sm <= 8)
-                W = (per_sm <= 1) ? 16 : (per_sm == 2) ? 8 : 4;
-            if(e->team_w == 4 || e->team_w == 8 || e->team_w == 16)
-                W = e->team_w;
-            while(W > 1 && W > kp.n_frames)
-                W /= 2;
-            if(W == 2)
-                W = 1;
-        }
-        if(W > 1)
-        {
-            const int tpc = 16 / W;
-            const int grid = std::min(e->sm_count, kp.n_streams); // streams are dealt to SMs first, then to an SM's teams
-            WF_CHECK(e, team2048_launch(W, x, kp, grid, st, e->use_pdl, e->device));
-            e->launches++;
-            e->last_kernel = "stft2048_team_kernel<" + std::to_string(W) + "," + std::to_string((int)x) + "> grid " + std::to_string(grid) +
-                             " x " + std::to_string(tpc) + " teams";
-            return WF_OK;
-        }
-        return dispatch_fast2048(e, kp, st, x);
-    }
-    {
-        const int rc = materialize_hold(e, st); // the other kernels read hold_db as it is
-        if(rc)
-            return rc;
-    }
-    // N = 16384 (config 5): a cluster of two CTAs per stream splits the bins by parity, each on the spill-free N=8192 plan
-    const bool par_ok = (N == 16384) && e->use_par16384 && e->use_v3 && e->d_tw0 && (cc == 1) && !t.cfg.stereo && kp.out_db &&
-                        !kp.out_points && !kp.out_pixels && !kp.out_min && !e->force_generic;
-    if(par_ok)
-    {
-        const bool x = kp.slope || kp.rolloff || kp.normalize || kp.fast_peaks || kp.skip_mask || kp.out_peak || kp.g_tab;
-        WF_CHECK(e, par16384_launch(x, kp, e->d_tw1, e->d_tw2, e->d_tw0, st, e->device));
-        e->launches++;
-        e->last_kernel = "stft16384_parity_kernel<" + std::to_string((int)x) + "> " + std::to_string(kp.n_streams) + " clusters of 2";
-        return WF_OK;
-    }
-    // Non-power-of-two sizes with a compiled two-pass plan (wf_warp2.cuh): same launch shape as the N=2048 kernel.  With
-    // display outputs (curve points / bars / pixels / minimum) the same kernel runs the render-time stages per warp; that
-    // variant also takes the power-of-two sizes 512 / 1024 / 2048 (config 1: N=1024, 26 bars).
-    const bool disp = kp.out_points || kp.out_pixels || kp.out_min;
-    const bool warp2_ok = e->use_warp2 && (cc == 1) && !t.cfg.stereo && aligned16 &&
-                          (disp ? (e->use_warp2_display && !e->force_generic && (warp2_supported(N) || warp2_pow2_supported(N)))
-                                : (warp2_supported(N) && kp.out_db));
-    if(warp2_ok)
-    {
-        const bool x = kp.slope || kp.rolloff || kp.normalize || kp.fast_peaks || kp.skip_mask || kp.out_peak || kp.g_tab;
-        int wpc = 16, grid = 1;
-        fast2048_geometry(kp.n_streams, e->sm_count, 16, &wpc, &grid);
-        kp.split = e->split_runs ? 1 : 0;
-        if(disp)
-        {
-            // shared memory of the display variant (layout in wf_warp2.cuh): per CTA the setup tables, per warp the tick's dB
-            // row, the bar sample points and — only for the Gaussian / pixel / minimum outputs — two rows of points + scratch
-            const size_t tab = display_table_floats(kp);
-            const bool need_pts = kp.filter || kp.out_pixels || kp.out_min;
-            const size_t per_warp = (size_t)B + (size_t)kp.n_sample + (need_pts ? 2 * (size_t)kp.n_points + 64 : 0);
-            kp.disp_tab_bytes = (int)((tab * sizeof(float) + 127) / 128 * 128);
-            kp.disp_bytes = (int)((per_warp * sizeof(float) + 127) / 128 * 128);
-        }
-        const char *name = "";
-        const cudaError_t rc = warp2_launch(N, x, disp, kp, grid, &wpc, st, e->use_pdl, e->device, &name);
-        if(rc != cudaErrorInvalidConfiguration) // (a curve too long for one warp's share of shared memory falls through)
-        {
-            WF_CHECK(e, rc);
-            e->launches++;
-            e->last_kernel = std::string(name) + " N=" + std::to_string(N) + " grid " + std::to_string(grid) + " x " + std::to_string(wpc) + " warps";
-            return WF_OK;
-        }
-    }
-    return (cc == 2) ? dispatch_n<2>(e, kp, st, extra) : dispatch_n<1>(e, kp, st, extra);
+    const CallFacts f = call_facts(kp);
+    return launch_route(e, choose_route(e, kp, f), f, kp, st);
 }
+
+
 
 int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
 {
@@ -865,7 +869,7 @@ int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
                                b->out_min};
         const bool small = S * T * (size_t)cc * (size_t)N * sizeof(float) <= (1u << 20);
         if(e->zc_valid && memcmp(ptrs, e->zc_ptrs, sizeof(ptrs)) == 0)
-            dev_ptrs = e->zc_dev || (e->zc_ok && small && e->zero_copy); // same buffers as the last call, already classified
+            dev_ptrs = e->zc_dev || (e->zc_ok && small && e->knobs.zero_copy); // same buffers as the last call, already classified
         else
         {
             const int kpcm = ptr_kind(b->pcm);
@@ -876,7 +880,7 @@ int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
             e->zc_dev = (kpcm == 1);
             e->zc_ok = zc;
             e->zc_valid = true;
-            dev_ptrs = e->zc_dev || (zc && small && e->zero_copy);
+            dev_ptrs = e->zc_dev || (zc && small && e->knobs.zero_copy);
         }
     }
 

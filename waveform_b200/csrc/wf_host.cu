@@ -5,6 +5,7 @@
 #include <algorithm>
 #include <cstdarg>
 #include <cstdio>
+#include <map>
 
 namespace wf {
 
@@ -89,6 +90,20 @@ int fill_device(HostCore *c, float *p, long long n, float v, cudaStream_t st)
     WF_CHECK(c, cudaGetLastError());
     c->launches++;
     return WF_OK;
+}
+
+cudaError_t opt_in_smem(const void *kernel, int device, size_t bytes)
+{
+    if(bytes <= 48 * 1024)
+        return cudaSuccess;
+    thread_local std::map<std::pair<const void *, int>, size_t> granted; // (kernel, device) -> bytes
+    size_t &have = granted[{kernel, device}];
+    if(bytes <= have)
+        return cudaSuccess;
+    const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if(err == cudaSuccess)
+        have = bytes;
+    return err;
 }
 
 float last_kernel_ms(HostCore *c)

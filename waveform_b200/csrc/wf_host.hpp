@@ -147,6 +147,46 @@ bool accept_struct(const T *in, size_t prev_size, T &out, bool *is_current = nul
     return true;
 }
 
+// Lets `kernel` use `bytes` of dynamic shared memory on `device` (the opt-in above the default 48 KB).  Asks CUDA once per
+// kernel, device and size: a size at or below one already granted returns at once.
+cudaError_t opt_in_smem(const void *kernel, int device, size_t bytes);
+
+// How cudaLaunchKernelEx launches: with programmatic dependent launch (the kernel's prologue overlaps the tail of the
+// previous launch on the stream) and / or as clusters of `cluster` consecutive CTAs.
+struct LaunchMode {
+    bool pdl = false;
+    unsigned cluster = 1;
+};
+
+// kernel<<<grid, block, smem, st>>>(args...) on `device` (the current one), opted in to `smem` first.
+template<class... P, class... A>
+cudaError_t launch_kernel(void (*kernel)(P...), int device, unsigned grid, unsigned block, size_t smem, cudaStream_t st,
+                          LaunchMode mode, A &&...args)
+{
+    if(cudaError_t err = opt_in_smem((const void *)kernel, device, smem))
+        return err;
+    cudaLaunchAttribute attr[2] = {};
+    unsigned n = 0;
+    if(mode.pdl)
+    {
+        attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[n++].val.programmaticStreamSerializationAllowed = 1;
+    }
+    if(mode.cluster > 1)
+    {
+        attr[n].id = cudaLaunchAttributeClusterDimension;
+        attr[n++].val.clusterDim = {mode.cluster, 1, 1};
+    }
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(block);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cfg.attrs = attr;
+    cfg.numAttrs = n;
+    return cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...);
+}
+
 // Environment knobs (A/B switches for tests and tools).  A flag that is on by default is switched off by a value starting
 // with '0'; one that is off by default is switched on by a value starting with '1'.
 inline bool env_flag(const char *name, bool dflt)

@@ -1,4 +1,5 @@
 // wf_par16384.cu — instantiations + launcher of stft16384_parity_kernel (its own translation unit)
+#include "wf_host.hpp"
 #include "wf_par16384.cuh"
 #include "wf_par16384.hpp"
 
@@ -7,18 +8,8 @@ namespace wf {
 template<bool EXTRA>
 static cudaError_t launch(const KParams &kp, const v3::Tw3 &tw, cudaStream_t st, int device)
 {
-    static thread_local bool configured[64] = {false};
-    const int dev = device & 63;
-    if(!configured[dev])
-    {
-        cudaError_t err = cudaFuncSetAttribute(stft16384_parity_kernel<EXTRA>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               (int)par16384::smem_bytes());
-        if(err != cudaSuccess)
-            return err;
-        configured[dev] = true;
-    }
-    stft16384_parity_kernel<EXTRA><<<dim3((unsigned)(2 * kp.n_streams)), par16384::kTN, par16384::smem_bytes(), st>>>(kp, tw);
-    return cudaGetLastError();
+    return launch_kernel(stft16384_parity_kernel<EXTRA>, device, 2 * kp.n_streams, par16384::kTN, par16384::smem_bytes(),
+                         st, {}, kp, tw);
 }
 
 cudaError_t par16384_launch(bool extra, const KParams &kp, const float *d_tw1, const float *d_tw2, const float *d_tw0,

@@ -1,45 +1,26 @@
 // wf_team2048.cu — instantiations + launcher of stft2048_team_kernel (its own translation unit: compiles in parallel)
+#include "wf_host.hpp"
 #include "wf_team2048.cuh"
 #include "wf_team2048.hpp"
 
 namespace wf {
 
 template<int W, bool EXTRA>
-static cudaError_t launch(const KParams &kp, int grid, cudaStream_t st, bool pdl, int device)
+static cudaError_t launch(const KParams &kp, int grid, cudaStream_t st, int device)
 {
-    static thread_local bool configured[64] = {false};
-    const int dev = device & 63;
-    if(!configured[dev])
-    {
-        cudaError_t err = cudaFuncSetAttribute(stft2048_team_kernel<W, EXTRA>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               team::smem_bytes());
-        if(err != cudaSuccess)
-            return err;
-        configured[dev] = true;
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(team::kWarps * 32);
-    cfg.dynamicSmemBytes = team::smem_bytes();
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, stft2048_team_kernel<W, EXTRA>, kp);
+    return launch_kernel(stft2048_team_kernel<W, EXTRA>, device, grid, team::kWarps * 32, team::smem_bytes(), st,
+                         {.pdl = true}, kp);
 }
 
-cudaError_t team2048_launch(int W, bool extra, const KParams &kp, int grid, cudaStream_t st, bool pdl, int device)
+cudaError_t team2048_launch(int W, bool extra, const KParams &kp, int grid, cudaStream_t st, int device)
 {
-#define WF_TEAM_CASE(WW)                                                                   \
-    if(W == WW)                                                                            \
-        return extra ? launch<WW, true>(kp, grid, st, pdl, device) : launch<WW, false>(kp, grid, st, pdl, device);
-    WF_TEAM_CASE(4)
-    WF_TEAM_CASE(8)
-    WF_TEAM_CASE(16)
-#undef WF_TEAM_CASE
-    return cudaErrorInvalidValue;
+    switch(W)
+    {
+    case 4: return extra ? launch<4, true>(kp, grid, st, device) : launch<4, false>(kp, grid, st, device);
+    case 8: return extra ? launch<8, true>(kp, grid, st, device) : launch<8, false>(kp, grid, st, device);
+    case 16: return extra ? launch<16, true>(kp, grid, st, device) : launch<16, false>(kp, grid, st, device);
+    default: return cudaErrorInvalidValue;
+    }
 }
 
 } // namespace wf

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "wf_host.hpp"
 #include "wf_v3.cuh"
 #include "wf_v3.hpp"
 
@@ -11,30 +12,8 @@ namespace v3impl {
 template<int N, int CC, int R, int EXTRA>
 cudaError_t launch_one(const KParams &kp, const v3::Tw3 &tw, cudaStream_t st, bool display, int device)
 {
-    const size_t smem = v3::smem_bytes<N>(kp.dch, kp.scratch_q, display, CC, R);
-    static thread_local size_t configured[64] = {0};
-    const int dev = device & 63;
-    if(smem > 48 * 1024 && configured[dev] < smem)
-    {
-        cudaError_t err = cudaFuncSetAttribute(stft_v3_kernel<N, CC, R, EXTRA>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               (int)smem);
-        if(err != cudaSuccess)
-            return err;
-        configured[dev] = smem;
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(kp.n_streams * R));
-    cfg.blockDim = dim3((unsigned)v3::Geo3<N>::TN);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = R;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = (R > 1) ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, stft_v3_kernel<N, CC, R, EXTRA>, kp, tw);
+    return launch_kernel(stft_v3_kernel<N, CC, R, EXTRA>, device, kp.n_streams * R, v3::Geo3<N>::TN,
+                         v3::smem_bytes<N>(kp.dch, kp.scratch_q, display, CC, R), st, {.cluster = R}, kp, tw);
 }
 
 template<int N, int CC, int EXTRA>

@@ -3,24 +3,12 @@
 
 namespace wf {
 
-cudaError_t warp2_launch_b(int N, bool extra, bool disp, const KParams &kp, int grid, int *warps, cudaStream_t st, bool pdl, int device,
-                           const char **name);
+Warp2Plan warp2_plan_b(int N);
+Warp2Plan warp2_plan_c(int N);
+Warp2Plan warp2_plan_d(int N);
+Warp2Plan warp2_plan_e(int N);
 
-bool warp2_supported(int N)
-{
-    switch(N)
-    {
-    case 400: case 720: case 800: case 960: case 1456: case 1600: // part A
-    case 1920: case 640: case 1280: case 1536: case 1152: case 1792: // part B
-    case 192: case 320: case 384: case 448: case 576: case 704: case 768: case 832: case 896: // part C
-    case 1344: case 1408: case 1664: case 1728: case 880: case 480: case 528: case 352: case 288: // part D
-        return true;
-    default: return false;
-    }
-}
-
-cudaError_t warp2_launch(int N, bool extra, bool disp, const KParams &kp, int grid, int *warps, cudaStream_t st, bool pdl, int device,
-                         const char **name)
+Warp2Plan warp2_plan(int N)
 {
     using namespace warp2;
     switch(N)
@@ -31,8 +19,12 @@ cudaError_t warp2_launch(int N, bool extra, bool disp, const KParams &kp, int gr
         WF_WARP2_CASE(960, 20, 24)   // 48 kHz / 50 fps
         WF_WARP2_CASE(1456, 26, 28)  // 44.1 kHz / 30 fps (1470 & -16): 2^4 7 13
         WF_WARP2_CASE(1600, 25, 32)  // 48 kHz / 30 fps
-    default: return warp2_launch_b(N, extra, disp, kp, grid, warps, st, pdl, device, name);
+    default: break;
     }
+    for(auto part : {warp2_plan_b, warp2_plan_c, warp2_plan_d, warp2_plan_e})
+        if(const Warp2Plan p = part(N); p.L)
+            return p;
+    return {};
 }
 
 } // namespace wf

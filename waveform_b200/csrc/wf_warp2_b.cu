@@ -3,15 +3,7 @@
 
 namespace wf {
 
-cudaError_t warp2_launch_c(int N, bool extra, bool disp, const KParams &kp, int grid, int *warps, cudaStream_t st, bool pdl, int device,
-                           const char **name);
-cudaError_t warp2_launch_e(int N, bool extra, bool disp, const KParams &kp, int grid, int *warps, cudaStream_t st, bool pdl, int device,
-                           const char **name);
-cudaError_t warp2_launch_d(int N, bool extra, bool disp, const KParams &kp, int grid, int *warps, cudaStream_t st, bool pdl, int device,
-                           const char **name);
-
-cudaError_t warp2_launch_b(int N, bool extra, bool disp, const KParams &kp, int grid, int *warps, cudaStream_t st, bool pdl, int device,
-                           const char **name)
+Warp2Plan warp2_plan_b(int N)
 {
     using namespace warp2;
     switch(N)
@@ -22,12 +14,8 @@ cudaError_t warp2_launch_b(int N, bool extra, bool disp, const KParams &kp, int 
         WF_WARP2_CASE(1536, 24, 32)
         WF_WARP2_CASE(1792, 28, 32)
         WF_WARP2_CASE(1920, 30, 32)
-    default: break;
+    default: return {};
     }
-    cudaError_t rc = warp2_launch_c(N, extra, disp, kp, grid, warps, st, pdl, device, name);
-    if(rc == cudaErrorInvalidValue)
-        rc = warp2_launch_d(N, extra, disp, kp, grid, warps, st, pdl, device, name);
-    return (rc == cudaErrorInvalidValue) ? warp2_launch_e(N, extra, disp, kp, grid, warps, st, pdl, device, name) : rc;
 }
 
 } // namespace wf

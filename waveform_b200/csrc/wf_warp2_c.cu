@@ -3,8 +3,7 @@
 
 namespace wf {
 
-cudaError_t warp2_launch_c(int N, bool extra, bool disp, const KParams &kp, int grid, int *warps, cudaStream_t st, bool pdl, int device,
-                           const char **name)
+Warp2Plan warp2_plan_c(int N)
 {
     using namespace warp2;
     switch(N)
@@ -18,7 +17,7 @@ cudaError_t warp2_launch_c(int N, bool extra, bool disp, const KParams &kp, int 
         WF_WARP2_CASE(768, 16, 24)
         WF_WARP2_CASE(832, 16, 26)
         WF_WARP2_CASE(896, 16, 28)
-    default: return cudaErrorInvalidValue;
+    default: return {};
     }
 }
 

@@ -3,8 +3,7 @@
 
 namespace wf {
 
-cudaError_t warp2_launch_d(int N, bool extra, bool disp, const KParams &kp, int grid, int *warps, cudaStream_t st, bool pdl, int device,
-                           const char **name)
+Warp2Plan warp2_plan_d(int N)
 {
     using namespace warp2;
     switch(N)
@@ -18,7 +17,7 @@ cudaError_t warp2_launch_d(int N, bool extra, bool disp, const KParams &kp, int 
         WF_WARP2_CASE(528, 12, 22)   // 48 kHz / 90 fps (533 & -16)
         WF_WARP2_CASE(352, 11, 16)   // 44.1 kHz / 120 fps (367 & -16)
         WF_WARP2_CASE(288, 12, 12)   // 48 kHz / 165 fps (290 & -16)
-    default: return cudaErrorInvalidValue;
+    default: return {};
     }
 }
 

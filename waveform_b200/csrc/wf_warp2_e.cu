@@ -5,10 +5,7 @@
 
 namespace wf {
 
-bool warp2_pow2_supported(int N) { return N == 512 || N == 1024 || N == 2048; }
-
-cudaError_t warp2_launch_e(int N, bool extra, bool disp, const KParams &kp, int grid, int *warps, cudaStream_t st, bool pdl, int device,
-                           const char **name)
+Warp2Plan warp2_plan_e(int N)
 {
     using namespace warp2;
     switch(N)
@@ -16,7 +13,7 @@ cudaError_t warp2_launch_e(int N, bool extra, bool disp, const KParams &kp, int 
         WF_WARP2_CASE(512, 16, 16)
         WF_WARP2_CASE(1024, 16, 32)  // 32 lanes in pass B and in the epilogue (8 bin pairs per lane)
         WF_WARP2_CASE(2048, 32, 32)
-    default: return cudaErrorInvalidValue;
+    default: return {};
     }
 }
 

@@ -2,6 +2,7 @@
 // compiles in parallel with wf_engine.cu.
 #include <cuda_runtime.h>
 
+#include "wf_host.hpp"
 #include "wf_wide.cuh"
 #include "wf_wide.hpp"
 
@@ -12,30 +13,8 @@ namespace {
 template<int N, int CC, int R>
 cudaError_t launch_one(const KParams &kp, cudaStream_t st, bool display, int device)
 {
-    const size_t smem = wide::smem_bytes<N>(kp.dch, kp.scratch_q, display);
-    static thread_local size_t configured[64] = {0};
-    const int dev = device & 63;
-    if(smem > 48 * 1024 && configured[dev] < smem)
-    {
-        cudaError_t err =
-            cudaFuncSetAttribute(stft_wide_kernel<N, CC, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if(err != cudaSuccess)
-            return err;
-        configured[dev] = smem;
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(kp.n_streams * R));
-    cfg.blockDim = dim3((unsigned)Geo<N>::TN);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = R;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, stft_wide_kernel<N, CC, R>, kp);
+    return launch_kernel(stft_wide_kernel<N, CC, R>, device, kp.n_streams * R, Geo<N>::TN,
+                         wide::smem_bytes<N>(kp.dch, kp.scratch_q, display), st, {.cluster = R}, kp);
 }
 
 template<int N, int CC>
