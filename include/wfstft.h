@@ -207,9 +207,36 @@ int wf_set_state(wf_engine *e, int32_t first_stream, int32_t count, const float 
  * src/source_generic.cpp:161-167 to a peak shared by all channels on all GPUs):
  *   gain[t] = min(target_db - peak[t], max_gain);  out[s][t][ch][k] += gain[t]  for k >= 1
  * `peak` is the (all-reduced) wf_batch.out_peak array; `data` is an out_db-shaped ([..][bins]) or
- * out_points-shaped ([..][num_points]) buffer, `row_len` its innermost length.  Device or host pointers. */
+ * out_points-shaped ([..][num_points]) buffer, `row_len` its innermost length.  Device or host pointers.
+ * On out_points-shaped buffers the result is NOT what render() would draw from normalised m_decibels: point 0 is left alone
+ * (it is not bin 0), Lanczos / Catmull-Rom taps that fall off the row are dropped without renormalising, and low-frequency
+ * taps reach bin 0, which the gain skips.  To get display outputs of normalised rows, use wf_render with `peak`. */
 int wf_peak_normalize(wf_engine *e, float *data, int32_t n_streams, int32_t n_frames, int32_t row_len,
                       const float *peak, float target_db, float max_gain, void *cuda_stream);
+
+/* The render-time display stage on dB rows the caller passes in: the out_points / out_pixels / out_min a wf_process call
+ * computes from its own m_decibels rows (src/source.cpp:1381-1424, 1473-1565), for rows held elsewhere — out_db of an
+ * earlier call, rows made on another GPU, or rows normalised by the cross-channel peak gain (BASELINE config 5).  Rendering
+ * a call's own out_db without `peak` gives that call's display outputs bit for bit.  With `peak`, the gain of
+ * wf_peak_normalize (same arithmetic, bins k >= 1) is added to each row before it is rendered, in the same pass; with
+ * write_db the normalised rows are also stored back into db, which then equals what wf_peak_normalize leaves.
+ * The call is stateless: it never reads or writes EMA state, m_decibels mirrors or flags.  Pointers are all host or all
+ * device (a host `peak` with a device `db` is copied); device pointers are enqueued on `cuda_stream` (NULL = the engine's
+ * own stream) without synchronising, host pointers are staged and the call returns when the results are home.
+ * WF_ERR_INVALID_ARG: a negative count, display outputs on an engine without display points, write_db without peak, or
+ * nothing requested (no display output and no write_db).  wf_last_kernel_name / wf_last_kernel_ms / wf_launch_count report
+ * the render launch. */
+typedef struct wf_render_batch {
+    uint32_t struct_size;      /* = sizeof(wf_render_batch) */
+    int32_t n_streams, n_frames;
+    float *db;                 /* [n_streams][n_frames][display_channels][bins]: out_db of earlier calls (host or device) */
+    const float *peak;         /* optional [n_frames]: the (all-reduced) out_peak; gain[t] = min(target_db - peak[t], max_gain)
+                                  is added to bins k >= 1 before rendering, with wf_peak_normalize's exact arithmetic */
+    float target_db, max_gain;
+    int32_t write_db;          /* 1: store the normalised rows back into db (wf_peak_normalize's result, in the same pass) */
+    float *out_points, *out_pixels, *out_min; /* optional; shapes and meaning as in wf_batch */
+} wf_render_batch;
+int wf_render(wf_engine *e, const wf_render_batch *rb, void *cuda_stream);
 
 /* Page-locked, device-mapped host memory for the live path (≙ the plugin's AlignedBuffer for m_fft_input / m_decibels,
  * src/aligned_buffer.hpp:30-80, but visible to the GPU).  When EVERY buffer of a small batch (at most 1 MiB of PCM) lives in
@@ -221,12 +248,12 @@ void wf_host_free(void *p);
 
 /* Number of kernel launches this engine has issued (bench.py reports it as gpu_launches). */
 int64_t wf_launch_count(const wf_engine *e);
-/* Name (template arguments and launch geometry included) of the spectrum kernel the most recent wf_process* call
+/* Name (template arguments and launch geometry included) of the kernel the most recent wf_process* or wf_render call
  * dispatched to, e.g. "stft2048_fast_kernel<12,1,1,0> grid 132 x 12 warps"; "" before the first call.  Valid until the
  * next call on this engine.  bench.py reports it as roofline.kernel, the tests assert the routing with it. */
 const char *wf_last_kernel_name(const wf_engine *e);
-/* Device time (ms) of the kernel section of the most recent wf_process / wf_process_async / wf_peak_normalize call,
- * measured with CUDA events on the launching stream; < 0 if none. Synchronises on the recorded events. */
+/* Device time (ms) of the kernel section of the most recent wf_process / wf_process_async / wf_peak_normalize / wf_render
+ * call, measured with CUDA events on the launching stream; < 0 if none. Synchronises on the recorded events. */
 float wf_last_kernel_ms(wf_engine *e);
 
 

@@ -25,6 +25,7 @@
 #include "wf_team2048.hpp"
 #include "wf_warp2.hpp"
 #include "wf_par16384.hpp"
+#include "wf_render.hpp"
 #include "wf_nvtx.hpp"
 #include "wf_tables.hpp"
 #include "wfstft.h"
@@ -67,6 +68,7 @@ struct wf_engine : HostCore {
     DevBuf<float> s_gtab; // [n_frames][2] per-tick (g, 1-g) of a TV-exponential batch with frame_seconds
     std::vector<float> h_gtab;
     DevBuf<float> s_scratch; // any-N kernel work buffers when N/2 complex points x 2 exceed shared memory
+    DevBuf<float> s_render;  // wf_render: one dB row per group when a row does not fit in shared memory
     // zero-copy verdict of the last host-pointer batch (live ticks reuse the same buffers every call)
     const void *zc_ptrs[9] = {};
     bool zc_ok = false, zc_dev = false, zc_valid = false;
@@ -228,6 +230,35 @@ CallFacts call_facts(const KParams &kp)
             .v3_x = opts_but_peak ? 3 : (kp.out_peak ? 1 : 0),
             .aligned16 = (((uintptr_t)kp.pcm & 15u) == 0) && ((kp.stream_stride & 3) == 0) && ((kp.hop & 3) == 0),
             .db16 = ((uintptr_t)kp.out_db & 15u) == 0};
+}
+
+// The display stage's settings (src/source.cpp:1381-1424, 1473-1565) in KParams: set here for the spectrum kernels and for
+// wf_render alike, so that both render the same way.  kp.dch must be set; the output pointers are the caller's.
+void set_display_params(const wf_engine *e, KParams &kp)
+{
+    const Tables &t = e->tab;
+    kp.interp_idx = e->d_interp_idx;
+    kp.interp_w = e->d_interp_w;
+    kp.band_widths = e->d_band_widths;
+    kp.band_offsets = e->d_band_offsets;
+    kp.n_points = t.num_points;
+    kp.n_sample = (t.cfg.display_mode == WF_DISPLAY_BAR && t.cfg.interp_mode != WF_INTERP_POINT) ? (int)t.interp_indices.size() : 0;
+    kp.scratch_q = t.num_points + (kp.dch * kp.n_sample + 3) / 4;
+    kp.taps = t.interp_taps;
+    kp.radius = t.interp_radius;
+    kp.display_bar = (t.cfg.display_mode == WF_DISPLAY_BAR);
+    kp.interp_mode = t.cfg.interp_mode;
+    kp.gauss_w = e->d_gauss;
+    kp.gauss_radius = t.gauss_radius;
+    kp.gauss_size = (int)t.gauss.size();
+    kp.gauss_sum = t.gauss_sum;
+    kp.filter = (t.cfg.filter_mode == WF_FILTER_GAUSS);
+    kp.px_lo = t.px_lo;
+    kp.px_hi = t.px_hi;
+    kp.px_cpos = t.px_cpos;
+    kp.ceiling_f = (float)t.cfg.ceiling_db;
+    kp.dbrange_f = (float)(t.cfg.ceiling_db - t.cfg.floor_db);
+    kp.mirror = t.cfg.mirror_freq_axis;
 }
 
 // Shared memory of the display stage in the fused and any-N kernels: [groups][2][dch <= 2][num_points] floats
@@ -784,30 +815,9 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
     kp.vol_target = t.cfg.volume_target;
     kp.max_gain = t.cfg.max_gain;
     kp.write_hold = 1;
-    kp.interp_idx = e->d_interp_idx;
-    kp.interp_w = e->d_interp_w;
-    kp.band_widths = e->d_band_widths;
-    kp.band_offsets = e->d_band_offsets;
-    kp.n_points = t.num_points;
-    kp.n_sample = (t.cfg.display_mode == WF_DISPLAY_BAR && t.cfg.interp_mode != WF_INTERP_POINT) ? (int)t.interp_indices.size() : 0;
-    kp.scratch_q = t.num_points + (dch * kp.n_sample + 3) / 4;
-    kp.taps = t.interp_taps;
-    kp.radius = t.interp_radius;
-    kp.display_bar = (t.cfg.display_mode == WF_DISPLAY_BAR);
-    kp.interp_mode = t.cfg.interp_mode;
-    kp.gauss_w = e->d_gauss;
-    kp.gauss_radius = t.gauss_radius;
-    kp.gauss_size = (int)t.gauss.size();
-    kp.gauss_sum = t.gauss_sum;
-    kp.filter = (t.cfg.filter_mode == WF_FILTER_GAUSS);
+    set_display_params(e, kp);
     kp.out_pixels = b->out_pixels ? px_dev + (size_t)s0 * T * dch * t.num_points : nullptr;
     kp.out_min = b->out_min ? min_dev + (size_t)s0 * T * 2 : nullptr;
-    kp.px_lo = t.px_lo;
-    kp.px_hi = t.px_hi;
-    kp.px_cpos = t.px_cpos;
-    kp.ceiling_f = (float)t.cfg.ceiling_db;
-    kp.dbrange_f = (float)(t.cfg.ceiling_db - t.cfg.floor_db);
-    kp.mirror = t.cfg.mirror_freq_axis;
 
     const CallFacts f = call_facts(kp);
     return launch_route(e, choose_route(e, kp, f), f, kp, st);
@@ -1168,6 +1178,90 @@ int wf_peak_normalize(wf_engine *e, float *data, int32_t n_streams, int32_t n_fr
         WF_CHECK(e, cudaMemcpyAsync(data, d_data, total * sizeof(float), cudaMemcpyDeviceToHost, st));
         WF_CHECK(e, cudaStreamSynchronize(st));
     }
+    return WF_OK;
+}
+
+int wf_render(wf_engine *e, const wf_render_batch *rb, void *cuda_stream)
+{
+    if(!e || !rb)
+        return WF_ERR_INVALID_ARG;
+    NvtxRange nvtx("wf_render");
+    if(rb->struct_size != sizeof(wf_render_batch))
+        return fail(e, WF_ERR_ABI, "wf_render_batch.struct_size %u != %zu", rb->struct_size, sizeof(wf_render_batch));
+    const Tables &t = e->tab;
+    const int dch = t.display_channels, B = t.B, np = t.num_points;
+    if(rb->n_streams < 0 || rb->n_frames < 0)
+        return fail(e, WF_ERR_INVALID_ARG, "n_streams/n_frames must be >= 0");
+    const bool display = rb->out_points || rb->out_pixels || rb->out_min;
+    if(display && np <= 0)
+        return fail(e, WF_ERR_INVALID_ARG, "display outputs requested but the engine has no display points");
+    if(rb->write_db && !rb->peak)
+        return fail(e, WF_ERR_INVALID_ARG, "write_db is set but the call carries no peak");
+    if(!display && !rb->write_db)
+        return fail(e, WF_ERR_INVALID_ARG, "nothing requested: no display output and no write_db");
+    if(rb->n_streams == 0 || rb->n_frames == 0)
+        return WF_OK;
+    if(!rb->db)
+        return fail(e, WF_ERR_INVALID_ARG, "db is null");
+
+    WF_CHECK(e, cudaSetDevice(e->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : e->stream;
+    const size_t T = (size_t)rb->n_frames, rows = (size_t)rb->n_streams * T, n_db = rows * dch * B, n_pts = rows * dch * np;
+    const bool dev = is_device_ptr(rb->db);
+    KParams kp{};
+    kp.n_streams = rb->n_streams;
+    kp.n_frames = rb->n_frames;
+    kp.dch = dch;
+    set_display_params(e, kp);
+    RenderArgs ra{.db = rb->db, .peak = rb->peak, .target_db = rb->target_db, .max_gain = rb->max_gain,
+                  .write_db = rb->write_db ? 1 : 0, .display = display ? 1 : 0, .rows = (long long)rows, .n_frames = rb->n_frames, .B = B,
+                  .len = dch * B};
+    // host buffers go through the engine's staging buffers, in and out on `st`
+    Staging sg(e, st, !dev);
+    ra.db = const_cast<float *>(sg.in(e->s_out_db, static_cast<const float *>(rb->db), n_db));
+    Staging sp(e, st, rb->peak && (!dev || !is_device_ptr(rb->peak))); // a host peak is copied even with device rows
+    ra.peak = sp.in(e->s_peak, rb->peak, T);
+    if(sp.rc)
+        return sp.rc;
+    if(rb->write_db && !dev)
+        sg.out(e->s_out_db, rb->db, n_db);
+    kp.out_points = sg.out(e->s_out_points, rb->out_points, n_pts);
+    kp.out_pixels = sg.out(e->s_px, rb->out_pixels, n_pts);
+    kp.out_min = sg.out(e->s_min, rb->out_min, rows * 2);
+    if(sg.rc)
+        return sg.rc;
+    ra.vec4 = ((uintptr_t)ra.db & 15u) == 0;
+
+    RenderPlan pl;
+    WF_CHECK(e, render_plan(kp, B, (long long)rows, e->sm_count, e->device, &pl));
+    if(pl.grid == 0)
+        return fail(e, WF_ERR_INVALID_ARG, "the display stage's scratch (%d points x %d channels) exceeds shared memory", np, dch);
+    ra.tab_smem = pl.tab_smem;
+    ra.row_smem = pl.row_smem;
+    ra.tab_floats = pl.tab_floats;
+    ra.group_floats = pl.group_floats;
+    if(!pl.row_smem)
+    {
+        if(int rc = e->s_render.reserve(e, (size_t)pl.grid * pl.groups * ra.len))
+            return rc;
+        ra.scratch = e->s_render;
+    }
+    WF_CHECK(e, cudaEventRecord(e->ev0, st));
+    WF_CHECK(e, render_launch(pl, kp, ra, st, e->device));
+    e->launches++;
+    WF_CHECK(e, cudaEventRecord(e->ev1, st));
+    e->ev_valid = true;
+    char name[128];
+    if(pl.tn == 32)
+        snprintf(name, sizeof name, "render_kernel<32> grid %d x %d warps", pl.grid, pl.groups);
+    else
+        snprintf(name, sizeof name, "render_kernel<%d> grid %d", pl.tn, pl.grid);
+    e->last_kernel = name;
+    if(dev)
+        return WF_OK;
+    if(int rc = sg.finish())
+        return rc;
+    WF_CHECK(e, cudaStreamSynchronize(st));
     return WF_OK;
 }
 

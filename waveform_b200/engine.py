@@ -43,7 +43,7 @@ EXPORTS = [
     "wf_abi_version", "wf_strerror", "wf_last_error", "wf_config_init", "wf_create", "wf_destroy", "wf_get_info",
     "wf_get_table", "wf_gravity", "wf_process", "wf_process_async", "wf_synchronize", "wf_reset_state",
     "wf_get_state", "wf_set_state", "wf_peak_normalize", "wf_launch_count", "wf_last_kernel_ms", "wf_last_kernel_name",
-    "wf_host_alloc", "wf_host_free", "wf_preview_table",
+    "wf_host_alloc", "wf_host_free", "wf_preview_table", "wf_render",
     "wf_meter_config_init", "wf_meter_create", "wf_meter_destroy", "wf_meter_last_error", "wf_meter_window",
     "wf_meter_process", "wf_meter_process_async", "wf_meter_reset", "wf_meter_launch_count", "wf_meter_last_kernel_ms",
     "wf_wave_config_init", "wf_wave_create", "wf_wave_destroy", "wf_wave_last_error", "wf_wave_process",
@@ -131,6 +131,14 @@ class WfBatch(C.Structure):
     ]
 
 
+class WfRenderBatch(C.Structure):
+    _fields_ = [
+        ("struct_size", C.c_uint32), ("n_streams", C.c_int32), ("n_frames", C.c_int32),
+        ("db", C.c_void_p), ("peak", C.c_void_p), ("target_db", C.c_float), ("max_gain", C.c_float),
+        ("write_db", C.c_int32), ("out_points", C.c_void_p), ("out_pixels", C.c_void_p), ("out_min", C.c_void_p),
+    ]
+
+
 class WfError(RuntimeError):
     def __init__(self, status: int, msg: str):
         super().__init__(f"libwfstft status {status}: {msg}")
@@ -173,6 +181,7 @@ def load_library():
     L.wf_get_state.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp]
     L.wf_set_state.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp]
     L.wf_peak_normalize.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, C.c_float, C.c_float, vp]
+    L.wf_render.argtypes = [vp, C.POINTER(WfRenderBatch), vp]
     L.wf_launch_count.restype = C.c_int64
     L.wf_launch_count.argtypes = [vp]
     L.wf_last_kernel_ms.restype = C.c_float
@@ -518,6 +527,50 @@ class Engine(_Handle):
         if stream == 0:
             stream = 1  # cudaStreamLegacy; NULL would select the engine's private stream
         self._check(self.L.wf_peak_normalize(self.h, _ptr(data), S, T, row, _ptr(peak), target_db, max_gain, stream))
+
+    def render(self, db, peak=None, target_db: float = -3.0, max_gain: float = 30.0, write_db: bool = False,
+               want_points: bool = False, want_pixels: bool = False, stream=None):
+        """The display stage (wf_render) on dB rows db[S, T, display_channels, bins] — out_db of earlier calls, a numpy array
+        (host path, synchronous) or a contiguous float32 CUDA tensor (device path, on torch's current stream unless `stream`
+        is given).  With `peak` ([T], numpy or tensor) the cross-channel peak gain min(target_db - peak[t], max_gain) is
+        added to bins k >= 1 before rendering; write_db=True also stores the normalised rows back into `db`, in place.
+        Returns dict(points=[S, T, dch, P]) for want_points and pixels=[S, T, dch, P], min=[S, T, 2] for want_pixels."""
+        S, T, dch, B = db.shape
+        if dch != self.display_channels or B != self.bins:
+            raise ValueError(f"db rows are [{dch}][{B}], the engine's are [{self.display_channels}][{self.bins}]")
+        if hasattr(db, "data_ptr"):
+            import torch
+            assert db.is_cuda and db.dtype == torch.float32 and db.is_contiguous()
+            mk = lambda shape: torch.empty(shape, dtype=torch.float32, device=db.device)  # noqa: E731
+            if stream is None:
+                stream = torch.cuda.current_stream(db.device).cuda_stream
+            if peak is not None and hasattr(peak, "data_ptr"):
+                assert peak.dtype == torch.float32 and peak.is_contiguous()
+        else:
+            if not (isinstance(db, np.ndarray) and db.dtype == np.float32 and db.flags.c_contiguous):
+                if write_db:
+                    raise ValueError("write_db needs db as a C-contiguous float32 array (it is updated in place)")
+                db = np.ascontiguousarray(db, dtype=np.float32)
+            mk = lambda shape: np.empty(shape, dtype=np.float32)  # noqa: E731
+        if peak is not None and not hasattr(peak, "data_ptr"):
+            peak = np.ascontiguousarray(peak, dtype=np.float32)
+        if peak is not None:
+            assert tuple(peak.shape) == (T,), peak.shape
+        out = {}
+        if want_points:
+            out["points"] = mk((S, T, dch, self.num_points))
+        if want_pixels:
+            out["pixels"], out["min"] = mk((S, T, dch, self.num_points)), mk((S, T, 2))
+        rb = WfRenderBatch()
+        rb.struct_size = C.sizeof(WfRenderBatch)
+        rb.n_streams, rb.n_frames = S, T
+        rb.db, rb.peak = _ptr(db), _ptr(peak)
+        rb.target_db, rb.max_gain, rb.write_db = target_db, max_gain, int(bool(write_db))
+        rb.out_points, rb.out_pixels, rb.out_min = _ptr(out.get("points")), _ptr(out.get("pixels")), _ptr(out.get("min"))
+        if stream == 0:
+            stream = 1  # cudaStreamLegacy; NULL would select the engine's private stream
+        self._check(self.L.wf_render(self.h, C.byref(rb), stream))
+        return out
 
 
 def make_meter_config(settings: dict | None = None, sample_rate: int = 48000, channels: int = 2, max_streams: int = 1,

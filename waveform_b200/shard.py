@@ -1,7 +1,7 @@
 """Multi-GPU plumbing for the spectrum path: one process per GPU, streams sharded contiguously, no data-path
 collective (SURVEY.md §8e).  The only exchange is the optional cross-channel peak normalisation
 (BASELINE.json configs[4]): a MAX all-reduce of n_frames floats over torch.distributed (NCCL on GPUs, gloo in the
-CPU tests), followed by the local wf_peak_normalize pass.
+CPU tests), followed by the local wf_peak_normalize pass, or by one wf_render pass when display outputs are wanted.
 
 Nothing here computes spectra; it only decides which rank owns which streams and moves the peak vector.
 """
@@ -47,4 +47,15 @@ class ShardedEngine:
         allreduce_peak(out["peak"], self.group)
         key = "db" if "db" in out else "points"
         self.engine.peak_normalize(out[key], out["peak"], target_db, max_gain)
+        return out
+
+    def process_normalized_display(self, pcm, n_frames, hop, target_db=-3.0, max_gain=30.0, want_points=False,
+                                   want_pixels=False, **kw):
+        """Config 5 with display outputs: the spectrum call (dB rows and peak, no display outputs), the all-reduce, then
+        one wf_render pass that normalises the rows in place and renders points / pixels / min from the normalised rows —
+        what render() draws from normalised m_decibels."""
+        out = self.engine.process(pcm, n_frames, hop, want_peak=True, **kw)
+        allreduce_peak(out["peak"], self.group)
+        out.update(self.engine.render(out["db"], out["peak"], target_db, max_gain, write_db=True, want_points=want_points,
+                                      want_pixels=want_pixels))
         return out
