@@ -125,6 +125,12 @@ typedef enum wf_table {
     WF_TABLE_GAUSS = 6          /* float[2*ceil(3 sigma)-1] m_kernel.weights */
 } wf_table;
 
+/* Sample format of wf_batch.pcm. */
+typedef enum wf_pcm_format {
+    WF_PCM_F32 = 0, /* float samples */
+    WF_PCM_S16 = 1  /* int16_t samples; sample v stands for v * 2^-15 exactly ((float)v * 0x1p-15f) */
+} wf_pcm_format;
+
 /* One call = n_streams independent sources x n_frames consecutive ticks.
  *   frame t of capture channel c of stream s = pcm[s*stream_stride + c*channel_stride + t*hop ... + fft_size)
  * i.e. what CircularBuffer::peek_front hands tick_spectrum on successive ticks (src/source_generic.cpp:55-59)
@@ -137,9 +143,14 @@ typedef struct wf_batch {
     int32_t hop;               /* samples between consecutive frames (>= 1) */
     int32_t first_stream;      /* state slot of stream 0 of this batch (0 <= first_stream, first+n <= max_streams) */
     float seconds;             /* tick delta for TVEXPONENTIAL gravity (src/source.hpp:301-312); ignored otherwise */
-    const float *pcm;          /* planar float PCM, host or device */
-    int64_t stream_stride;     /* in floats */
-    int64_t channel_stride;    /* in floats */
+    const float *pcm;          /* planar PCM, host or device: float samples, or int16_t samples (cast to const float *) when
+                                  pcm_format is WF_PCM_S16, in which case pcm must be 2-byte aligned.  Strides and hop count
+                                  SAMPLES in either format.  An S16 call gives bit for bit the results of the F32 call on
+                                  (float)v * 0x1p-15f, whenever both take the same kernel (wf_last_kernel_name() of an S16 call is
+                                  the F32 name + " s16"); frames are 16-byte aligned for the N=2048 / warp-per-stream kernels when
+                                  pcm is 16-byte aligned and stream_stride and hop are multiples of 8 samples (F32: of 4). */
+    int64_t stream_stride;     /* in samples */
+    int64_t channel_stride;    /* in samples */
     const float *input_rms;    /* [n_streams][n_frames] m_input_rms per tick; REQUIRED when normalize_volume is set (else
                                   WF_ERR_INVALID_ARG: never a silent max_gain), ignored otherwise */
     const uint8_t *skip_mask;  /* optional [n_streams][n_frames]: nonzero = "not enough audio" for that tick */
@@ -155,6 +166,8 @@ typedef struct wf_batch {
                                   Only TVEXPONENTIAL smoothing looks at it: gravity = exp(-seconds / (gravity * 0.1934...))
                                   is then evaluated per tick as get_gravity() does (src/source.hpp:301-312), so a batch
                                   recorded with jittering frame times replays exactly.  NULL: `seconds` for every tick. */
+    int32_t pcm_format;        /* wf_pcm_format of pcm (0 = WF_PCM_F32).  A caller built against the previous header
+                                  (struct_size = offsetof(wf_batch, pcm_format)) passes float PCM. */
 } wf_batch;
 
 typedef struct wf_engine wf_engine;

@@ -23,7 +23,7 @@ struct AnyPlan {
 
 constexpr int kAnyThreads = 256;
 
-template<int CC>
+template<int CC, typename TS>
 __global__ void __launch_bounds__(kAnyThreads) stft_anyn_kernel(const __grid_constant__ KParams p,
                                                                   const __grid_constant__ AnyPlan plan)
 {
@@ -48,7 +48,7 @@ __global__ void __launch_bounds__(kAnyThreads) stft_anyn_kernel(const __grid_con
     bool last_silent = (fl & 1u) != 0;
     bool prev_out_silent0 = (fl & 2u) != 0;
     bool prev_out_silent1 = (fl & 4u) != 0;
-    const float *pcm_s = p.pcm + (size_t)s * p.stream_stride;
+    const TS *pcm_s = Pcm<TS>::base(p.pcm) + (size_t)s * p.stream_stride;
 
     for(int t = 0; t < T; ++t)
     {
@@ -61,12 +61,12 @@ __global__ void __launch_bounds__(kAnyThreads) stft_anyn_kernel(const __grid_con
         for(int c = 0; c < CC; ++c)
         {
             // ---- frame + window -> bufA (packed as N/2 complex points) ----
-            const float *frame = pcm_s + (size_t)c * p.channel_stride + (size_t)t * p.hop;
+            const TS *frame = pcm_s + (size_t)c * p.channel_stride + (size_t)t * p.hop;
             bool nzl = false;
             __syncthreads(); // previous users of the buffers are done
             for(int n = tid; n < M; n += kAnyThreads)
             {
-                float2 z = make_float2(ldg_stream_f1(frame + 2 * n), ldg_stream_f1(frame + 2 * n + 1));
+                float2 z = make_float2(Pcm<TS>::load1(frame + 2 * n), Pcm<TS>::load1(frame + 2 * n + 1));
                 nzl |= (z.x != 0.0f) | (z.y != 0.0f);
                 if(p.window != nullptr)
                 {

@@ -210,6 +210,7 @@ struct Route {
     size_t smem = 0;                // warp2, any-N: dynamic shared memory bytes
     bool scratch = false;           // any-N: work buffers in an L2 scratch instead of shared memory
     bool display = false;           // warp2: the display variant
+    bool s16 = false;               // int16 samples (every family: the Pcm<int16_t> instantiation, wf_pcm.cuh)
     int disp_tab_bytes = 0, disp_bytes = 0; // warp2 with display outputs: per-CTA tables, per-warp rows
 };
 
@@ -222,13 +223,16 @@ struct CallFacts {
     bool db16;      // out_db is 16-byte aligned (the N=2048 kernels write each dB row with one bulk copy)
 };
 
-CallFacts call_facts(const KParams &kp)
+// Frames start at 16-byte boundaries (TMA) when pcm does and the stream stride and hop are whole multiples of 16 bytes:
+// 4 float samples, 8 int16 samples.  `aligned8` of KParams is the same fact at 8 bytes (launch_range).
+CallFacts call_facts(const KParams &kp, bool s16)
 {
     const bool opts_but_peak = kp.slope || kp.rolloff || kp.normalize || kp.fast_peaks || kp.skip_mask || kp.g_tab;
+    const long long q = s16 ? 7 : 3; // samples per 16 bytes, minus one
     return {.display = kp.out_points || kp.out_pixels || kp.out_min,
             .opts = opts_but_peak || kp.out_peak,
             .v3_x = opts_but_peak ? 3 : (kp.out_peak ? 1 : 0),
-            .aligned16 = (((uintptr_t)kp.pcm & 15u) == 0) && ((kp.stream_stride & 3) == 0) && ((kp.hop & 3) == 0),
+            .aligned16 = (((uintptr_t)kp.pcm & 15u) == 0) && ((kp.stream_stride & q) == 0) && ((kp.hop & q) == 0),
             .db16 = ((uintptr_t)kp.out_db & 15u) == 0};
 }
 
@@ -419,41 +423,41 @@ std::string route_name(const wf_engine *e, const Route &r, int n_streams)
     case Family::fused: snprintf(buf, sizeof buf, "stft_fused_kernel<%d,%d>", N, cc); break;
     case Family::anyn: snprintf(buf, sizeof buf, "stft_anyn_kernel<%d> N=%d", cc, N); break;
     }
-    return buf;
+    return r.s16 ? std::string(buf) + " s16" : std::string(buf);
 }
 
-template<int N, int CC>
+template<int N, int CC, typename TS>
 cudaError_t launch_fused(const wf_engine *e, const KParams &kp, const CallFacts &f, cudaStream_t st)
 {
     using G = Geo<N>;
     const size_t smem = (size_t)G::GROUPS * G::BUF * sizeof(float2) + display_smem(kp, f, G::GROUPS);
-    return launch_kernel(stft_fused_kernel<N, CC>, e->device, (kp.n_streams + G::GROUPS - 1) / G::GROUPS, G::CTA, smem, st,
+    return launch_kernel(stft_fused_kernel<N, CC, TS>, e->device, (kp.n_streams + G::GROUPS - 1) / G::GROUPS, G::CTA, smem, st,
                          {}, kp);
 }
 
-template<int CC>
+template<int CC, typename TS>
 cudaError_t launch_fused_n(const wf_engine *e, const KParams &kp, const CallFacts &f, cudaStream_t st)
 {
     switch(e->tab.N)
     {
-    case 128: return launch_fused<128, CC>(e, kp, f, st);
-    case 256: return launch_fused<256, CC>(e, kp, f, st);
-    case 512: return launch_fused<512, CC>(e, kp, f, st);
-    case 1024: return launch_fused<1024, CC>(e, kp, f, st);
-    case 2048: return launch_fused<2048, CC>(e, kp, f, st);
-    case 4096: return launch_fused<4096, CC>(e, kp, f, st);
-    case 8192: return launch_fused<8192, CC>(e, kp, f, st);
-    case 16384: return launch_fused<16384, CC>(e, kp, f, st);
-    case 32768: return launch_fused<32768, CC>(e, kp, f, st);
+    case 128: return launch_fused<128, CC, TS>(e, kp, f, st);
+    case 256: return launch_fused<256, CC, TS>(e, kp, f, st);
+    case 512: return launch_fused<512, CC, TS>(e, kp, f, st);
+    case 1024: return launch_fused<1024, CC, TS>(e, kp, f, st);
+    case 2048: return launch_fused<2048, CC, TS>(e, kp, f, st);
+    case 4096: return launch_fused<4096, CC, TS>(e, kp, f, st);
+    case 8192: return launch_fused<8192, CC, TS>(e, kp, f, st);
+    case 16384: return launch_fused<16384, CC, TS>(e, kp, f, st);
+    case 32768: return launch_fused<32768, CC, TS>(e, kp, f, st);
     default: return cudaErrorInvalidValue;
     }
 }
 
-// stft2048_fast_kernel<kMaxWarpsPerCta, TSM, GATE, EXTRA>, indexed by TSM * 4 + GATE * 2 + EXTRA
-template<int... I>
+// stft2048_fast_kernel<kMaxWarpsPerCta, TSM, GATE, EXTRA, TS>, indexed by TSM * 4 + GATE * 2 + EXTRA
+template<typename TS, int... I>
 std::array<void (*)(KParams), sizeof...(I)> fast_kernels(std::integer_sequence<int, I...>)
 {
-    return {stft2048_fast_kernel<fast::kMaxWarpsPerCta, (I & 4) != 0, (I & 2) != 0, (I & 1) != 0>...};
+    return {stft2048_fast_kernel<fast::kMaxWarpsPerCta, (I & 4) != 0, (I & 2) != 0, (I & 1) != 0, TS>...};
 }
 
 // Write out every implicit m_decibels mirror (see materialize_hold_kernel) before something other than the N=2048
@@ -727,24 +731,30 @@ static int launch_route(wf_engine *e, const Route &r, const CallFacts &f, KParam
         kp.lazy_hold = 1;
         e->hold_implicit = true;
         if(r.family == Family::team)
-            err = team2048_launch(r.w, r.x, kp, r.grid, st, dev);
+            err = team2048_launch(r.w, r.x, r.s16, kp, r.grid, st, dev);
         else
         {
-            static const auto kernels = fast_kernels(std::make_integer_sequence<int, 8>{});
-            err = launch_kernel(kernels[r.tsm * 4 + r.gate * 2 + r.x], dev, r.grid, r.w * 32, fast::smem_bytes(r.w), st,
-                                {.pdl = true}, kp);
+            static const auto kernels = fast_kernels<float>(std::make_integer_sequence<int, 8>{});
+            static const auto kernels_s16 = fast_kernels<int16_t>(std::make_integer_sequence<int, 8>{});
+            err = launch_kernel((r.s16 ? kernels_s16 : kernels)[r.tsm * 4 + r.gate * 2 + r.x], dev, r.grid, r.w * 32,
+                                fast::smem_bytes(r.w), st, {.pdl = true}, kp);
         }
         break;
-    case Family::parity: err = par16384_launch(r.x, kp, e->d_tw1, e->d_tw2, e->d_tw0, st, dev); break;
+    case Family::parity: err = par16384_launch(r.x, r.s16, kp, e->d_tw1, e->d_tw2, e->d_tw0, st, dev); break;
     case Family::warp2:
         kp.split = e->knobs.split ? 1 : 0;
         kp.disp_tab_bytes = r.disp_tab_bytes;
         kp.disp_bytes = r.disp_bytes;
-        err = e->warp2.launch[r.x][r.display](kp, r.grid, r.w, r.smem, st, dev);
+        err = e->warp2.launch[r.s16][r.x][r.display](kp, r.grid, r.w, r.smem, st, dev);
         break;
-    case Family::v3: err = v3_launch(N, cc, r.r, r.x, kp, e->d_tw1, e->d_tw2, e->d_tw0, st, f.display, dev); break;
-    case Family::wide: err = wide_launch(N, cc, r.r, kp, st, f.display, dev); break;
-    case Family::fused: err = (cc == 2) ? launch_fused_n<2>(e, kp, f, st) : launch_fused_n<1>(e, kp, f, st); break;
+    case Family::v3: err = v3_launch(N, cc, r.r, r.x, r.s16, kp, e->d_tw1, e->d_tw2, e->d_tw0, st, f.display, dev); break;
+    case Family::wide: err = wide_launch(N, cc, r.r, r.s16, kp, st, f.display, dev); break;
+    case Family::fused:
+        if(r.s16)
+            err = (cc == 2) ? launch_fused_n<2, int16_t>(e, kp, f, st) : launch_fused_n<1, int16_t>(e, kp, f, st);
+        else
+            err = (cc == 2) ? launch_fused_n<2, float>(e, kp, f, st) : launch_fused_n<1, float>(e, kp, f, st);
+        break;
     case Family::anyn:
     {
         AnyPlan plan = e->any;
@@ -755,8 +765,12 @@ static int launch_route(wf_engine *e, const Route &r, const CallFacts &f, KParam
                 return rc;
             plan.scratch = reinterpret_cast<float2 *>(e->s_scratch.p);
         }
-        err = (cc == 2) ? launch_kernel(stft_anyn_kernel<2>, dev, r.grid, kAnyThreads, r.smem, st, {}, kp, plan)
-                        : launch_kernel(stft_anyn_kernel<1>, dev, r.grid, kAnyThreads, r.smem, st, {}, kp, plan);
+        if(r.s16)
+            err = (cc == 2) ? launch_kernel(stft_anyn_kernel<2, int16_t>, dev, r.grid, kAnyThreads, r.smem, st, {}, kp, plan)
+                            : launch_kernel(stft_anyn_kernel<1, int16_t>, dev, r.grid, kAnyThreads, r.smem, st, {}, kp, plan);
+        else
+            err = (cc == 2) ? launch_kernel(stft_anyn_kernel<2, float>, dev, r.grid, kAnyThreads, r.smem, st, {}, kp, plan)
+                            : launch_kernel(stft_anyn_kernel<1, float>, dev, r.grid, kAnyThreads, r.smem, st, {}, kp, plan);
         break;
     }
     }
@@ -764,6 +778,12 @@ static int launch_route(wf_engine *e, const Route &r, const CallFacts &f, KParam
     e->launches++;
     e->last_kernel = route_name(e, r, kp.n_streams);
     return WF_OK;
+}
+
+// pcm + `samples` samples of the batch's format (the pointer stays `const float *`, as in wf_batch and KParams)
+static const float *pcm_offset(const float *pcm, size_t samples, bool s16)
+{
+    return reinterpret_cast<const float *>(reinterpret_cast<const char *>(pcm) + samples * (s16 ? 2 : 4));
 }
 
 // Runs streams [s0, s0+count) of the batch; all pointers are DEVICE pointers already offset to stream 0 of the batch.
@@ -774,15 +794,18 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
     const Tables &t = e->tab;
     const int cc = t.cfg.capture_channels, dch = t.display_channels, och = t.output_channels, B = t.B;
     const size_t T = (size_t)b->n_frames;
+    const bool s16 = b->pcm_format == WF_PCM_S16;
     KParams kp{};
-    kp.pcm = pcm + (size_t)s0 * (size_t)b->stream_stride;
+    kp.pcm = pcm_offset(pcm, (size_t)s0 * (size_t)b->stream_stride, s16);
     kp.stream_stride = b->stream_stride;
     kp.channel_stride = b->channel_stride;
     kp.n_streams = count;
     kp.n_frames = b->n_frames;
     kp.hop = b->hop;
-    kp.aligned8 = (((uintptr_t)kp.pcm & 7u) == 0) && ((b->stream_stride & 1) == 0) && ((b->channel_stride & 1) == 0) &&
-                  ((b->hop & 1) == 0);
+    // every frame starts at an 8-byte boundary: 2 float samples, 4 int16 samples
+    const long long q = s16 ? 3 : 1;
+    kp.aligned8 = (((uintptr_t)kp.pcm & 7u) == 0) && ((b->stream_stride & q) == 0) && ((b->channel_stride & q) == 0) &&
+                  ((b->hop & q) == 0);
     kp.input_rms = rms ? rms + (size_t)s0 * T : nullptr;
     kp.skip_mask = skip ? skip + (size_t)s0 * T : nullptr;
     kp.window = e->d_window;
@@ -819,19 +842,24 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
     kp.out_pixels = b->out_pixels ? px_dev + (size_t)s0 * T * dch * t.num_points : nullptr;
     kp.out_min = b->out_min ? min_dev + (size_t)s0 * T * 2 : nullptr;
 
-    const CallFacts f = call_facts(kp);
-    return launch_route(e, choose_route(e, kp, f), f, kp, st);
+    const CallFacts f = call_facts(kp, s16);
+    Route r = choose_route(e, kp, f);
+    r.s16 = s16;
+    return launch_route(e, r, f, kp, st);
 }
 
 
 
-int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
+int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
 {
-    if(!e || !b)
+    if(!e || !b_in)
         return WF_ERR_INVALID_ARG;
     NvtxRange nvtx("wf_process");
-    if(b->struct_size != sizeof(wf_batch))
-        return fail(e, WF_ERR_ABI, "wf_batch.struct_size %u != %zu", b->struct_size, sizeof(wf_batch));
+    // the current struct or the previous one (which ends before pcm_format: float PCM)
+    wf_batch bv;
+    if(!accept_struct(b_in, offsetof(wf_batch, pcm_format), bv))
+        return fail(e, WF_ERR_ABI, "wf_batch.struct_size %u != %zu", b_in->struct_size, sizeof(wf_batch));
+    const wf_batch *b = &bv;
     const Tables &t = e->tab;
     const int cc = t.cfg.capture_channels, dch = t.display_channels, B = t.B, N = t.N;
     if(b->n_streams < 0 || b->n_frames < 0 || b->hop < 1)
@@ -845,6 +873,12 @@ int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
         return fail(e, WF_ERR_INVALID_ARG, "pcm is null");
     if(b->stream_stride < 0 || b->channel_stride < 0)
         return fail(e, WF_ERR_INVALID_ARG, "negative strides are not supported");
+    if(b->pcm_format != WF_PCM_F32 && b->pcm_format != WF_PCM_S16)
+        return fail(e, WF_ERR_INVALID_ARG, "pcm_format %d is not a wf_pcm_format", b->pcm_format);
+    const bool s16 = b->pcm_format == WF_PCM_S16;
+    const size_t sample_bytes = s16 ? sizeof(int16_t) : sizeof(float);
+    if(s16 && ((uintptr_t)b->pcm & 1u) != 0)
+        return fail(e, WF_ERR_INVALID_ARG, "int16 pcm must be 2-byte aligned");
     if(t.cfg.normalize_volume && !b->input_rms)
         return fail(e, WF_ERR_INVALID_ARG, "normalize_volume is set but the batch carries no input_rms (m_input_rms per tick: "
                                               "wf_meter in WF_METER_INPUT_RMS mode, or the host's own update_input_rms)");
@@ -877,7 +911,7 @@ int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
         // launch + one synchronisation.  Every buffer of the batch must be device-addressable for that.
         const void *ptrs[9] = {b->pcm, b->input_rms, b->skip_mask, b->out_db, b->out_points, b->out_silent, b->out_peak, b->out_pixels,
                                b->out_min};
-        const bool small = S * T * (size_t)cc * (size_t)N * sizeof(float) <= (1u << 20);
+        const bool small = S * T * (size_t)cc * (size_t)N * sample_bytes <= (1u << 20);
         if(e->zc_valid && memcmp(ptrs, e->zc_ptrs, sizeof(ptrs)) == 0)
             dev_ptrs = e->zc_dev || (e->zc_ok && small && e->knobs.zero_copy); // same buffers as the last call, already classified
         else
@@ -925,7 +959,7 @@ int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
         rc = buf.reserve(e, n);
         return buf.p;
     };
-    rc = e->s_pcm.reserve(e, span);
+    rc = e->s_pcm.reserve(e, (span * sample_bytes + sizeof(float) - 1) / sizeof(float)); // s_pcm counts floats
     float *d_out_db = stage(e->s_out_db, b->out_db, S * T * dch * B);
     float *d_out_points = stage(e->s_out_points, b->out_points, S * T * dch * t.num_points);
     float *d_rms = stage(e->s_rms, b->input_rms, S * T);
@@ -947,7 +981,7 @@ int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
         WF_CHECK(e, cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
         WF_CHECK(e, cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming));
     }
-    const size_t in_bytes = span * sizeof(float);
+    const size_t in_bytes = span * sample_bytes;
     int nchunks = (int)std::min<size_t>(std::min<size_t>(wf_engine::kMaxChunks, S), std::max<size_t>(1, in_bytes >> 25));
     const int per = (int)((S + nchunks - 1) / nchunks);
     nchunks = (int)((S + per - 1) / per);
@@ -967,7 +1001,8 @@ int wf_process_async(wf_engine *e, const wf_batch *b, void *cuda_stream)
         const int cnt = std::min<int>(per, (int)S - s0);
         const size_t off = (size_t)s0 * (size_t)b->stream_stride;
         const size_t cspan = (size_t)(cnt - 1) * (size_t)b->stream_stride + per_stream_span;
-        WF_CHECK(e, cudaMemcpyAsync(e->s_pcm + off, b->pcm + off, cspan * sizeof(float), cudaMemcpyHostToDevice, e->s_h2d));
+        WF_CHECK(e, cudaMemcpyAsync(const_cast<float *>(pcm_offset(e->s_pcm, off, s16)), pcm_offset(b->pcm, off, s16),
+                                   cspan * sample_bytes, cudaMemcpyHostToDevice, e->s_h2d));
         if(d_rms)
             WF_CHECK(e, cudaMemcpyAsync(d_rms + (size_t)s0 * T, b->input_rms + (size_t)s0 * T, (size_t)cnt * T * sizeof(float),
                                        cudaMemcpyHostToDevice, e->s_h2d));

@@ -126,10 +126,12 @@ __device__ __forceinline__ pk::c64 dbfs2(float m1, float m2, float db_min)
 // store wrote — the hold / quirk path reads the previous row, the next warp reads it after a split-mode hand-over —
 // comes after cp.async.bulk.wait_group 0 and a proxy fence.  The mirror write-back reads the last row from the staging
 // buffer, which still holds it.
-template<int MAXW, bool TSM, bool GATE, bool EXTRA>
+template<int MAXW, bool TSM, bool GATE, bool EXTRA, typename TS>
 __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __grid_constant__ KParams p)
 {
     using namespace fast;
+    using PS = Pcm<TS>;
+    constexpr uint32_t kFrameBytes = PS::frame_bytes(kN); // TMA transfer of one frame (the landing buffer holds a float frame)
     static_assert(MAXW <= kMaxWarpsPerCta, "shared memory holds at most kMaxWarpsPerCta warps");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float2 *s_win = reinterpret_cast<float2 *>(smem_raw);
@@ -241,8 +243,9 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
     {
         int li, t0, t1;
         segment(0, li, t0, t1);
-        mbar_expect_tx(mbar, kN * 4);
-        tma_load_1d(land, p.pcm + (size_t)(blockIdx.x + li * G) * p.stream_stride + (size_t)t0 * p.hop, kN * 4, mbar);
+        mbar_expect_tx(mbar, kFrameBytes);
+        tma_load_1d(land, PS::base(p.pcm) + (size_t)(blockIdx.x + li * G) * p.stream_stride + (size_t)t0 * p.hop, kFrameBytes,
+                    mbar);
     }
 
     for(int j = 0; j < nseg; ++j)
@@ -283,7 +286,7 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
         // dbfs(state) (see the end of this loop); it is rebuilt from the state wherever it is needed
         const bool hold_lazy = (fl & 8u) != 0;
         bool last_from_state = false; // the last tick's outputs are dbfs(state) (normal tick), not a hold / quirk
-        const float *pcm_s = p.pcm + (size_t)s * p.stream_stride;
+        const TS *pcm_s = PS::base(p.pcm) + (size_t)s * p.stream_stride;
         float *hold_s = p.hold_db + (size_t)s * B;
 
 #pragma unroll 1
@@ -294,13 +297,12 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
             phase ^= 1u;
             pk::c64 v[32];
             unsigned long long nzbits = 0;
-            const pk::c64 *land64 = reinterpret_cast<const pk::c64 *>(land);
             const pk::c64 *buf64 = reinterpret_cast<const pk::c64 *>(buf);
             const pk::c64 *win64 = reinterpret_cast<const pk::c64 *>(s_win);
 #pragma unroll
             for(int pidx = 0; pidx < 32; ++pidx)
             {
-                v[pidx] = land64[lane + 32 * pidx];
+                v[pidx] = PS::smem_pair(land, lane + 32 * pidx);
                 nzbits |= v[pidx];
             }
             // every lane has the frame in registers: the landing buffer takes the next frame (or the next segment's
@@ -308,16 +310,16 @@ __global__ void __launch_bounds__(MAXW * 32, 1) stft2048_fast_kernel(const __gri
             __syncwarp();
             if(lane == 0)
             {
-                const float *next = nullptr;
+                const TS *next = nullptr;
                 if(t + 1 < t1)
                     next = pcm_s + (size_t)(t + 1) * p.hop;
                 else if(s_next >= 0)
-                    next = p.pcm + (size_t)s_next * p.stream_stride + (size_t)t0_next * p.hop;
+                    next = PS::base(p.pcm) + (size_t)s_next * p.stream_stride + (size_t)t0_next * p.hop;
                 if(next != nullptr)
                 {
                     fence_proxy_async();
-                    mbar_expect_tx(mbar, kN * 4);
-                    tma_load_1d(land, next, kN * 4, mbar);
+                    mbar_expect_tx(mbar, kFrameBytes);
+                    tma_load_1d(land, next, kFrameBytes, mbar);
                 }
             }
 #pragma unroll

@@ -18,15 +18,16 @@
 #include <stdint.h>
 
 #include "wf_fft.cuh"
+#include "wf_pcm.cuh"
 
 namespace wf {
 
 struct KParams {
     // input
-    const float *pcm;
+    const float *pcm;                // float or int16_t samples (the kernel's sample type, see wf_pcm.cuh)
     long long stream_stride, channel_stride;
     int n_streams, n_frames, hop;
-    int aligned8; // every frame start is 8-byte aligned -> float2 loads
+    int aligned8; // every frame start is 8-byte aligned -> sample-pair loads
     const float *input_rms;          // [n_streams][n_frames] or null
     const unsigned char *skip_mask;  // [n_streams][n_frames] or null
     // tables
@@ -182,18 +183,6 @@ __device__ __forceinline__ float group_max(float x, float *scratch)
     }
 }
 
-__device__ __forceinline__ float2 ldg_stream_f2(const float2 *p)
-{
-    float2 r;
-    asm volatile("ld.global.nc.L1::no_allocate.v2.f32 {%0, %1}, [%2];" : "=f"(r.x), "=f"(r.y) : "l"(p));
-    return r;
-}
-__device__ __forceinline__ float ldg_stream_f1(const float *p)
-{
-    float r;
-    asm volatile("ld.global.nc.L1::no_allocate.f32 %0, [%1];" : "=f"(r) : "l"(p));
-    return r;
-}
 __device__ __forceinline__ void stg_stream(float *p, float v)
 {
     asm volatile("st.global.cs.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
@@ -307,16 +296,18 @@ struct Fft<N, PlanT<TN_, R0, Rest...>> {
 
     // Issues the loads of one frame (as M complex points) into registers; no use of the values yet, so the loads
     // stay in flight across whatever the caller does next (software prefetch of the next tick).
-    static __device__ __forceinline__ void load_raw(float2 (&v)[P], const float *frame, const KParams &p, int tid)
+    template<typename TS>
+    static __device__ __forceinline__ void load_raw(float2 (&v)[P], const TS *frame, const KParams &p, int tid)
     {
+        using PS = Pcm<TS>;
         if(p.aligned8)
         {
-            const float2 *f2 = reinterpret_cast<const float2 *>(frame);
+            const typename PS::Pair *f2 = reinterpret_cast<const typename PS::Pair *>(frame);
 #pragma unroll
             for(int b = 0; b < P0::BPT; ++b)
 #pragma unroll
                 for(int t = 0; t < R0; ++t)
-                    v[b * R0 + t] = ldg_stream_f2(f2 + (tid + b * TN + t * P0::BF));
+                    v[b * R0 + t] = PS::load2(f2 + (tid + b * TN + t * P0::BF));
         }
         else
         {
@@ -326,7 +317,7 @@ struct Fft<N, PlanT<TN_, R0, Rest...>> {
                 for(int t = 0; t < R0; ++t)
                 {
                     const int n = tid + b * TN + t * P0::BF;
-                    v[b * R0 + t] = make_float2(ldg_stream_f1(frame + 2 * n), ldg_stream_f1(frame + 2 * n + 1));
+                    v[b * R0 + t] = make_float2(PS::load1(frame + 2 * n), PS::load1(frame + 2 * n + 1));
                 }
         }
     }
@@ -352,14 +343,16 @@ struct Fft<N, PlanT<TN_, R0, Rest...>> {
         return nz;
     }
     // Pulls a frame's cache lines into L2 (for plans whose register budget has no room for a register prefetch).
-    static __device__ __forceinline__ void prefetch_l2(const float *frame, int tid)
+    template<typename TS>
+    static __device__ __forceinline__ void prefetch_l2(const TS *frame, int tid)
     {
-        constexpr int LINES = (N * 4) / 128;
+        constexpr int LINES = (N * Pcm<TS>::kBytes) / 128;
         for(int l = tid; l < LINES; l += TN)
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(frame + l * 32));
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(frame + l * (128 / Pcm<TS>::kBytes)));
     }
     // Loads the frame (as M complex points), applies the window, reports whether any sample is nonzero.
-    static __device__ __forceinline__ bool load_frame(float2 (&v)[P], const float *frame, const KParams &p, int tid)
+    template<typename TS>
+    static __device__ __forceinline__ bool load_frame(float2 (&v)[P], const TS *frame, const KParams &p, int tid)
     {
         load_raw(v, frame, p, tid);
         return finish_load(v, p, tid);
@@ -729,7 +722,7 @@ __device__ __forceinline__ void display_stage_tab(const KParams &p, const DispTa
 }
 
 // ---- the fused kernel ------------------------------------------------------------------------------
-template<int N, int CC>
+template<int N, int CC, typename TS>
 __global__ void __launch_bounds__(Geo<N>::CTA, Geo<N>::MINB) stft_fused_kernel(const __grid_constant__ KParams p)
 {
     using G = Geo<N>;
@@ -767,7 +760,7 @@ __global__ void __launch_bounds__(Geo<N>::CTA, Geo<N>::MINB) stft_fused_kernel(c
     bool prev_out_silent0 = (fl & 2u) != 0;
     bool prev_out_silent1 = (fl & 4u) != 0;
 
-    const float *pcm_s = p.pcm + (size_t)s * p.stream_stride;
+    const TS *pcm_s = Pcm<TS>::base(p.pcm) + (size_t)s * p.stream_stride;
     float *hold_s = p.hold_db + (size_t)s * och * B;
 
     // Software pipelining of the PCM loads: plans with <= 16 points per thread keep the NEXT frame's samples in
@@ -792,14 +785,14 @@ __global__ void __launch_bounds__(Geo<N>::CTA, Geo<N>::MINB) stft_fused_kernel(c
 #pragma unroll
         for(int c = 0; c < CC; ++c)
         {
-            const float *frame = pcm_s + (size_t)c * p.channel_stride + (size_t)t * p.hop;
+            const TS *frame = pcm_s + (size_t)c * p.channel_stride + (size_t)t * p.hop;
             if(!REGPF)
                 F::load_raw(v, frame, p, tid);
             const bool nz = group_any<TN>(F::finish_load(v, p, tid));
             F::run(v, buf, p.tw, tid);
             {
                 // next frame of this stream: the other channel of this tick, or channel 0 of the next tick
-                const float *next = (c + 1 < CC) ? frame + p.channel_stride
+                const TS *next = (c + 1 < CC) ? frame + p.channel_stride
                                                  : pcm_s + (size_t)(t + 1) * p.hop;
                 if(c + 1 < CC || t + 1 < p.n_frames)
                 {

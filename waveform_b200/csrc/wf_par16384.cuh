@@ -28,21 +28,23 @@ constexpr int kTN = G::TN;       // 256 threads
 constexpr int kP = G::P;         // 16 points (= bins) per thread
 constexpr int kHP = kP / 2;      // bin pairs per thread
 constexpr size_t kBufBytes = (((size_t)G::BUF * sizeof(float2)) + 127) / 128 * 128;
-constexpr size_t kStageBytes = (size_t)kN * sizeof(float); // the whole frame, TMA-staged one tick ahead
+constexpr size_t kStageBytes = (size_t)kN * sizeof(float); // the whole frame, TMA-staged one tick ahead (int16: first half)
 constexpr size_t smem_bytes() { return kBufBytes + kStageBytes + 16; }
 } // namespace par16384
 
 // The body is instantiated once per cluster rank (r = 0: even bins, r = 1: odd bins) so that every bin index, twiddle index and
 // output address is a per-thread base + a compile-time offset: with a run-time rank ncu showed 31 % of the 23 062
 // warp-instructions per frame in IMAD / MOV / LEA / IADD3 / LOP3 / ISETP (profiles/r02_par16384.txt).
-template<bool EXTRA, int r>
+template<bool EXTRA, int r, typename TS>
 __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &tw, unsigned char *smem_raw, unsigned (*redf)[2])
 {
     using namespace wide;
     using namespace par16384;
     constexpr int B = kBins, TN = kTN, P = kP, HP = kHP, MS = kSub;
     float2 *buf = reinterpret_cast<float2 *>(smem_raw);
-    const pk::c64 *stage = reinterpret_cast<const pk::c64 *>(smem_raw + kBufBytes); // frame t: pairs z[n], n < 8192
+    using PS = Pcm<TS>;
+    const unsigned char *stage = smem_raw + kBufBytes; // frame t: pairs z[n], n < 8192 (float or int16 samples)
+    constexpr uint32_t kFrameBytes = PS::frame_bytes(kN);
     uint64_t *mbar = reinterpret_cast<uint64_t *>(smem_raw + kBufBytes + kStageBytes);
     const int tid = threadIdx.x;
     const int s = blockIdx.x >> 1;
@@ -72,7 +74,7 @@ __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &t
     bool pos = (fl & 2u) != 0, pos_valid = true; // prev_out_silent over ALL bins of the stream, evaluated lazily
     bool part = true;                            // this thread's share of the last producing tick
     unsigned red_par = 0;
-    const float *pcm_s = p.pcm + (size_t)s * p.stream_stride;
+    const TS *pcm_s = PS::base(p.pcm) + (size_t)s * p.stream_stride;
     float *hold_s = p.hold_db + (size_t)s * B;
 
     // cluster-wide AND of the per-thread flags (rare: a silent tick that needs the answer, and once at the end)
@@ -90,7 +92,7 @@ __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &t
     };
 
     // TMA staging (cp.async.bulk + mbarrier) needs 16-byte aligned frames; otherwise the frame is loaded straight from global
-    const bool use_tma = (((uintptr_t)pcm_s & 15u) == 0) && ((p.hop & 3) == 0);
+    const bool use_tma = (((uintptr_t)pcm_s & 15u) == 0) && ((p.hop & (16 / PS::kBytes - 1)) == 0);
     uint32_t phase = 0;
     if(tid == 0)
     {
@@ -103,8 +105,8 @@ __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &t
     cluster_wait();
     if(use_tma && T > 0 && tid == 0)
     {
-        fast::mbar_expect_tx(mbar, (uint32_t)kStageBytes);
-        fast::tma_load_1d(const_cast<pk::c64 *>(stage), pcm_s, (uint32_t)kStageBytes, mbar);
+        fast::mbar_expect_tx(mbar, kFrameBytes);
+        fast::tma_load_1d(const_cast<unsigned char *>(stage), pcm_s, kFrameBytes, mbar);
     }
     const pk::c64 *win = reinterpret_cast<const pk::c64 *>(p.window2) + tid; // pairs (w[2n], w[2n+1]), n = a*TN + tid
     const pk::c64 *tw0 = reinterpret_cast<const pk::c64 *>(tw.tw0) + tid;    // W_8192^(a*TN + tid)
@@ -115,7 +117,7 @@ __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &t
 #pragma unroll 1
     for(int t = 0; t < T; ++t)
     {
-        const float *frame = pcm_s + (size_t)t * p.hop;
+        const TS *frame = pcm_s + (size_t)t * p.hop;
         // ---- both halves of the frame, window, radix-2 first stage for MY parity ----
         pk::c64 x[P];
         unsigned long long nzbits = 0;
@@ -129,7 +131,7 @@ __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &t
 #pragma unroll
                 for(int a = 0; a < P; ++a)
                 {
-                    pk::c64 za = stage[a * TN + tid], zb = stage[MS + a * TN + tid];
+                    pk::c64 za = PS::smem_pair(stage, a * TN + tid), zb = PS::smem_pair(stage, MS + a * TN + tid);
                     nzbits |= za | zb;
                     if(p.window2 != nullptr)
                     {
@@ -144,7 +146,7 @@ __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &t
 #pragma unroll
                 for(int a = 0; a < P; ++a)
                 {
-                    pk::c64 za = stage[a * TN + tid], zb = stage[MS + a * TN + tid];
+                    pk::c64 za = PS::smem_pair(stage, a * TN + tid), zb = PS::smem_pair(stage, MS + a * TN + tid);
                     nzbits |= za | zb;
                     if(p.window2 != nullptr)
                     {
@@ -158,28 +160,28 @@ __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &t
             if(tid == 0 && t + 1 < T)
             {
                 fast::fence_proxy_async();
-                fast::mbar_expect_tx(mbar, (uint32_t)kStageBytes);
-                fast::tma_load_1d(const_cast<pk::c64 *>(stage), frame + p.hop, (uint32_t)kStageBytes, mbar);
+                fast::mbar_expect_tx(mbar, kFrameBytes);
+                fast::tma_load_1d(const_cast<unsigned char *>(stage), frame + p.hop, kFrameBytes, mbar);
             }
         }
         else
         {
-            const float2 *lo = reinterpret_cast<const float2 *>(frame) + tid;
-            const float2 *hi = lo + MS;
+            const typename PS::Pair *lo = reinterpret_cast<const typename PS::Pair *>(frame) + tid;
+            const typename PS::Pair *hi = lo + MS;
 #pragma unroll
             for(int a = 0; a < P; ++a)
             {
                 pk::c64 za, zb;
                 if(p.aligned8)
                 {
-                    za = pk::from(ldg_stream_f2(lo + a * TN));
-                    zb = pk::from(ldg_stream_f2(hi + a * TN));
+                    za = pk::from(PS::load2(lo + a * TN));
+                    zb = pk::from(PS::load2(hi + a * TN));
                 }
                 else
                 {
-                    const float *f = frame + 2 * (a * TN + tid);
-                    za = pk::make(ldg_stream_f1(f), ldg_stream_f1(f + 1));
-                    zb = pk::make(ldg_stream_f1(f + 2 * MS), ldg_stream_f1(f + 2 * MS + 1));
+                    const TS *f = frame + 2 * (a * TN + tid);
+                    za = pk::make(PS::load1(f), PS::load1(f + 1));
+                    zb = pk::make(PS::load1(f + 2 * MS), PS::load1(f + 2 * MS + 1));
                 }
                 nzbits |= za | zb;
                 if(p.window2 != nullptr)
@@ -364,16 +366,16 @@ __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &t
     cluster_wait();
 }
 
-template<bool EXTRA>
+template<bool EXTRA, typename TS>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(par16384::kTN, 2)
     stft16384_parity_kernel(const __grid_constant__ KParams p, const __grid_constant__ v3::Tw3 tw)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ unsigned redf[2][2]; // [parity of the exchange][rank]: this rank's "all my outputs <= floor-10 dB"
     if(wide::cluster_ctarank() == 0)
-        par16384_body<EXTRA, 0>(p, tw, smem_raw, redf);
+        par16384_body<EXTRA, 0, TS>(p, tw, smem_raw, redf);
     else
-        par16384_body<EXTRA, 1>(p, tw, smem_raw, redf);
+        par16384_body<EXTRA, 1, TS>(p, tw, smem_raw, redf);
 }
 
 } // namespace wf

@@ -36,10 +36,12 @@ __device__ __forceinline__ void bar_sync(int id, int nthreads)
 }
 } // namespace team
 
-template<int W, bool EXTRA>
+template<int W, bool EXTRA, typename TS>
 __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(const __grid_constant__ KParams p)
 {
     using namespace fast;
+    using PS = Pcm<TS>;
+    constexpr uint32_t kFrameBytes = PS::frame_bytes(kN); // TMA transfer of one frame
     constexpr int TPC = team::kWarps / W; // teams per CTA
     constexpr int BW = kM / W;            // bins per warp in phase 2
     constexpr int BPL = BW / 32;          // bins per lane: 2, 4, 8, 16
@@ -97,15 +99,16 @@ __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(con
     // first frame of this warp: tick wi of the team's first stream
     if(tm < n_local && wi < T && lane == 0)
     {
-        mbar_expect_tx(mbar, kN * 4);
-        tma_load_1d(buf, p.pcm + (size_t)(blockIdx.x + tm * G) * p.stream_stride + (size_t)wi * p.hop, kN * 4, mbar);
+        mbar_expect_tx(mbar, kFrameBytes);
+        tma_load_1d(buf, PS::base(p.pcm) + (size_t)(blockIdx.x + tm * G) * p.stream_stride + (size_t)wi * p.hop, kFrameBytes,
+                    mbar);
     }
 
     for(int li = tm; li < n_local; li += TPC)
     {
         const int s = (int)blockIdx.x + li * G;
         const bool have_next_stream = (li + TPC) < n_local;
-        const float *pcm_s = p.pcm + (size_t)s * p.stream_stride;
+        const TS *pcm_s = PS::base(p.pcm) + (size_t)s * p.stream_stride;
         float *hold_s = p.hold_db + (size_t)s * B;
         float *state_s = p.state + (size_t)s * B;
 
@@ -162,7 +165,7 @@ __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(con
 #pragma unroll
                 for(int pidx = 0; pidx < 32; ++pidx)
                 {
-                    v[pidx] = buf64[lane + 32 * pidx];
+                    v[pidx] = PS::smem_pair(buf, lane + 32 * pidx);
                     nzbits |= v[pidx];
                 }
 #pragma unroll
@@ -190,16 +193,16 @@ __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(con
                             v[n1] = buf64[n1 * 33 + lane];
                         __syncwarp();
                         // next frame of this warp: tick t + W of this stream, else tick wi of the team's next stream
-                        const float *next = nullptr;
+                        const TS *next = nullptr;
                         if(t + W < T)
                             next = pcm_s + (size_t)(t + W) * p.hop;
                         else if(have_next_stream)
-                            next = p.pcm + (size_t)(s + TPC * G) * p.stream_stride + (size_t)wi * p.hop;
+                            next = PS::base(p.pcm) + (size_t)(s + TPC * G) * p.stream_stride + (size_t)wi * p.hop;
                         if(lane == 0 && next != nullptr)
                         {
                             fence_proxy_async();
-                            mbar_expect_tx(mbar, kN * 4);
-                            tma_load_1d(buf, next, kN * 4, mbar);
+                            mbar_expect_tx(mbar, kFrameBytes);
+                            tma_load_1d(buf, next, kFrameBytes, mbar);
                         }
                     }
                 }

@@ -93,28 +93,31 @@ struct Fft3 {
     using G = Geo3<N>;
     static constexpr int M = G::M, A = G::A, B = G::B, C = G::C, TN = G::TN, P = G::P;
 
-    static __device__ __forceinline__ void load_raw(float2 (&v)[P], const float *frame, int aligned8, int tid)
+    template<typename TS>
+    static __device__ __forceinline__ void load_raw(float2 (&v)[P], const TS *frame, int aligned8, int tid)
     {
+        using PS = Pcm<TS>;
         if(aligned8)
         {
-            const float2 *f2 = reinterpret_cast<const float2 *>(frame) + tid;
+            const typename PS::Pair *f2 = reinterpret_cast<const typename PS::Pair *>(frame) + tid;
 #pragma unroll
             for(int a = 0; a < A; ++a)
-                v[a] = ldg_stream_f2(f2 + a * TN);
+                v[a] = PS::load2(f2 + a * TN);
         }
         else
         {
-            const float *f1 = frame + 2 * tid;
+            const TS *f1 = frame + 2 * tid;
 #pragma unroll
             for(int a = 0; a < A; ++a)
-                v[a] = make_float2(ldg_stream_f1(f1 + 2 * a * TN), ldg_stream_f1(f1 + 2 * a * TN + 1));
+                v[a] = make_float2(PS::load1(f1 + 2 * a * TN), PS::load1(f1 + 2 * a * TN + 1));
         }
     }
     // pull a frame's cache lines into L2 (when there is no register room for a register prefetch)
-    static __device__ __forceinline__ void prefetch_l2(const float *frame, int tid)
+    template<typename TS>
+    static __device__ __forceinline__ void prefetch_l2(const TS *frame, int tid)
     {
-        for(int l = tid; l < N / 32; l += TN)
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(frame + l * 32));
+        for(int l = tid; l < N * Pcm<TS>::kBytes / 128; l += TN)
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(frame + l * (128 / Pcm<TS>::kBytes)));
     }
     // non-zero test (src/source_generic.cpp:63-76) + window multiply (:97-103); returns "any sample non-zero" (this thread).
     // Split plan: the radix-2 first stage is fused in, pair by pair, so that window and twiddle values die immediately:
@@ -274,7 +277,7 @@ struct Fft3 {
 // EXTRA: 0 = plain, 1 = + per-tick peak output (BASELINE config 5), 3 = + slope / fast peaks / skip mask / volume
 // normalisation / roll-off as well.  Keeping the peak apart matters: ncu on config 5 (profiles/r01m_v3_c5.txt) showed the
 // all-features epilogue costing 54 warp-instructions per bin although only the peak was in use.
-template<int N, int CC, int R, int EXTRA>
+template<int N, int CC, int R, int EXTRA, typename TS>
 __global__ void __launch_bounds__(v3::Geo3<N>::TN, v3::Geo3<N>::MINB)
     stft_v3_kernel(const __grid_constant__ KParams p, const __grid_constant__ v3::Tw3 tw)
 {
@@ -352,7 +355,7 @@ __global__ void __launch_bounds__(v3::Geo3<N>::TN, v3::Geo3<N>::MINB)
     bool part0 = true, part1 = true;
     unsigned red_par = 0;
 
-    const float *pcm_s = p.pcm + (size_t)s * p.stream_stride;
+    const TS *pcm_s = Pcm<TS>::base(p.pcm) + (size_t)s * p.stream_stride;
     float *hold_s = p.hold_db + (size_t)s * och * B;
 
     // cluster-wide AND of the per-thread partial "outputs <= floor-10" flags of the last tick that produced outputs
@@ -631,7 +634,7 @@ __global__ void __launch_bounds__(v3::Geo3<N>::TN, v3::Geo3<N>::MINB)
         const bool mine = (int)r < nf;
         const int my_t = t0 + (int)r;
         // next frame this CTA will need after (my tick, channel c)
-        auto next_frame = [&](int c) -> const float * {
+        auto next_frame = [&](int c) -> const TS * {
             if(c + 1 < CC)
                 return pcm_s + (size_t)(c + 1) * p.channel_stride + (size_t)my_t * p.hop;
             return (my_t + R < T) ? pcm_s + (size_t)(my_t + R) * p.hop : nullptr;
@@ -650,7 +653,7 @@ __global__ void __launch_bounds__(v3::Geo3<N>::TN, v3::Geo3<N>::MINB)
             {
                 pk::c64 x[P];
                 const bool nzt = F::finish_load(x, v, p.window2, tid, tw);
-                const float *nx = next_frame(c);
+                const TS *nx = next_frame(c);
                 if(nx != nullptr)
                 {
                     if(EARLY_PF)
@@ -705,7 +708,7 @@ __global__ void __launch_bounds__(v3::Geo3<N>::TN, v3::Geo3<N>::MINB)
                     if(!KEEP_V)
                         F::load_raw(v, pcm_s + (size_t)c * p.channel_stride + (size_t)my_t * p.hop, p.aligned8, tid);
                     const bool nzt = F::finish_load(x, v, p.window2, tid, tw);
-                    const float *nx = next_frame(c);
+                    const TS *nx = next_frame(c);
                     if(nx != nullptr)
                     {
                         if(EARLY_PF)

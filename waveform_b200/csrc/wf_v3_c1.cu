@@ -8,6 +8,8 @@ namespace wf {
 
 cudaError_t v3_launch_c2(int N, int R, int extra, const KParams &kp, const v3::Tw3 &tw, cudaStream_t st, bool display,
                          int device);
+cudaError_t v3_launch_s16(int N, int cc, int R, int extra, const KParams &kp, const v3::Tw3 &tw, cudaStream_t st, bool display,
+                          int device);
 
 bool v3_supported(int N) { return N == 1024 || N == 2048 || N == 4096 || N == 8192 || N == 16384; }
 int v3_min_cluster(int N) { return (N <= 8192) ? 1 : 2; }
@@ -75,14 +77,16 @@ void v3_build_twiddles(int N, std::vector<float> &tw1, std::vector<float> &tw2, 
     }
 }
 
-cudaError_t v3_launch(int N, int cc, int R, int extra, const KParams &kp, const float *d_tw1, const float *d_tw2,
+cudaError_t v3_launch(int N, int cc, int R, int extra, bool s16, const KParams &kp, const float *d_tw1, const float *d_tw2,
                       const float *d_tw0, cudaStream_t st, bool display, int device)
 {
     v3::Tw3 tw{reinterpret_cast<const float2 *>(d_tw1), reinterpret_cast<const float2 *>(d_tw2),
                reinterpret_cast<const float2 *>(d_tw0)};
+    if(s16)
+        return v3_launch_s16(N, cc, R, extra, kp, tw, st, display, device);
     if(cc == 2)
         return v3_launch_c2(N, R, extra, kp, tw, st, display, device);
-    return v3impl::launch_cc<1>(N, R, extra, kp, tw, st, display, device);
+    return v3impl::launch_cc<1, float>(N, R, extra, kp, tw, st, display, device);
 }
 
 } // namespace wf

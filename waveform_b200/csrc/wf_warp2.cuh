@@ -58,11 +58,12 @@ struct Geo {
 // wf_kernels.cuh, the one the CTA-per-tick kernels use) run on the warp right after the tick's dB row, which is then kept
 // in a per-warp shared-memory row (it doubles as the "previous row" of the hold paths; out_db may be null).  The extra
 // per-warp area (p.disp_bytes: dB row, display scratch, arg-min scratch) follows the regular per-warp areas.
-template<int L, int P, bool EXTRA, bool DISP = false>
+template<int L, int P, bool EXTRA, bool DISP, typename TS>
 __global__ void __launch_bounds__(warp2::Geo<L, P>::kWarps * 32, 1) stft_warp2_kernel(const __grid_constant__ KParams p)
 {
     using namespace fast;
     using G = warp2::Geo<L, P>;
+    using PS = Pcm<TS>;
     constexpr int M = G::M, N = G::N, R = G::R, PP = G::PP, Q = G::Q, B = M;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float2 *s_win = reinterpret_cast<float2 *>(smem_raw); // window pairs (x[2n], x[2n+1]) * (2/sum(w))/2
@@ -176,8 +177,9 @@ __global__ void __launch_bounds__(warp2::Geo<L, P>::kWarps * 32, 1) stft_warp2_k
     {
         int li, t0, t1;
         segment(0, li, t0, t1);
-        mbar_expect_tx(mbar, N * 4);
-        tma_load_1d(buf, p.pcm + (size_t)(blockIdx.x + li * GR) * p.stream_stride + (size_t)t0 * p.hop, N * 4, mbar);
+        mbar_expect_tx(mbar, PS::frame_bytes(N));
+        tma_load_1d(buf, PS::base(p.pcm) + (size_t)(blockIdx.x + li * GR) * p.stream_stride + (size_t)t0 * p.hop, PS::frame_bytes(N),
+                    mbar);
     }
 
     for(int j = 0; j < nseg; ++j)
@@ -225,7 +227,7 @@ __global__ void __launch_bounds__(warp2::Geo<L, P>::kWarps * 32, 1) stft_warp2_k
         const unsigned char fl = p.flags[s];
         bool last_silent = (fl & 1u) != 0;
         bool prev_out_silent = (fl & 2u) != 0;
-        const float *pcm_s = p.pcm + (size_t)s * p.stream_stride;
+        const TS *pcm_s = PS::base(p.pcm) + (size_t)s * p.stream_stride;
         float *hold_s = p.hold_db + (size_t)s * B;
 
 #pragma unroll 1
@@ -240,7 +242,7 @@ __global__ void __launch_bounds__(warp2::Geo<L, P>::kWarps * 32, 1) stft_warp2_k
 #pragma unroll
             for(int pi = 0; pi < P; ++pi)
             {
-                v[pi] = buf64[la + L * pi];
+                v[pi] = PS::smem_pair(buf, la + L * pi);
                 nzbits |= act_a ? v[pi] : 0ull;
             }
 #pragma unroll
@@ -270,16 +272,16 @@ __global__ void __launch_bounds__(warp2::Geo<L, P>::kWarps * 32, 1) stft_warp2_k
                 asm volatile("prefetch.global.L2 [%0];" ::"l"(p.state + (size_t)s_next * B + (lane * 32) % B));
             if(lane == 0)
             {
-                const float *next = nullptr;
+                const TS *next = nullptr;
                 if(t + 1 < t1)
                     next = pcm_s + (size_t)(t + 1) * p.hop;
                 else if(s_next >= 0)
-                    next = p.pcm + (size_t)s_next * p.stream_stride + (size_t)t0_next * p.hop;
+                    next = PS::base(p.pcm) + (size_t)s_next * p.stream_stride + (size_t)t0_next * p.hop;
                 if(next != nullptr)
                 {
                     fence_proxy_async();
-                    mbar_expect_tx(mbar, N * 4);
-                    tma_load_1d(buf, next, N * 4, mbar);
+                    mbar_expect_tx(mbar, PS::frame_bytes(N));
+                    tma_load_1d(buf, next, PS::frame_bytes(N), mbar);
                 }
             }
             // ---- pass B: radix-L register DFT over n1: X[k2 + P k1] = v[perm(L, k1)] on lane k2 ----

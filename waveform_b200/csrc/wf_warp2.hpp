@@ -14,8 +14,9 @@ using Warp2Launch = cudaError_t (*)(const KParams &kp, int grid, int warps, size
 struct Warp2Plan {
     int L = 0, P = 0;
     int table_bytes = 0, warp_bytes = 0; // shared memory per CTA and per warp of the plain kernel
-    Warp2Launch launch[2][2] = {};       // [extra][disp]: extra = slope / fast peaks / skip mask / volume / roll-off / peak
-                                         // output in use; disp = display outputs (points / pixels / minimum) requested
+    Warp2Launch launch[2][2][2] = {};    // [s16][extra][disp]: s16 = int16 samples (wf_pcm.cuh); extra = slope / fast peaks /
+                                         // skip mask / volume / roll-off / peak output in use; disp = display outputs (points /
+                                         // pixels / minimum) requested
 
     // a CTA of `warps` warps, with the display variant's per-CTA tables and per-warp rows (0 for the plain kernel)
     size_t smem_bytes(int warps, size_t disp_tab_bytes, size_t disp_warp_bytes) const

@@ -59,7 +59,7 @@ constexpr size_t smem_bytes(int dch, int n_points, bool display)
 
 } // namespace wide
 
-template<int N, int CC, int R>
+template<int N, int CC, int R, typename TS>
 __global__ void __launch_bounds__(Geo<N>::TN, Geo<N>::MINB) stft_wide_kernel(const __grid_constant__ KParams p)
 {
     using namespace wide;
@@ -110,7 +110,7 @@ __global__ void __launch_bounds__(Geo<N>::TN, Geo<N>::MINB) stft_wide_kernel(con
     bool part0 = true, part1 = true;
     unsigned red_par = 0;
 
-    const float *pcm_s = p.pcm + (size_t)s * p.stream_stride;
+    const TS *pcm_s = Pcm<TS>::base(p.pcm) + (size_t)s * p.stream_stride;
     float *hold_s = p.hold_db + (size_t)s * och * B;
 
     // cluster-wide AND of the per-thread partial flags of the last tick that produced outputs (rare path)

@@ -128,7 +128,19 @@ class WfBatch(C.Structure):
         ("input_rms", C.c_void_p), ("skip_mask", C.c_void_p),
         ("out_db", C.c_void_p), ("out_points", C.c_void_p), ("out_silent", C.c_void_p), ("out_peak", C.c_void_p),
         ("out_pixels", C.c_void_p), ("out_min", C.c_void_p), ("frame_seconds", C.c_void_p),
+        ("pcm_format", C.c_int32),
     ]
+
+
+# wf_pcm_format: the sample type of wf_batch.pcm
+PCM_F32, PCM_S16 = 0, 1
+_PCM_FORMATS = {"f32": PCM_F32, "s16": PCM_S16}
+
+
+def _pcm_format(name) -> int:
+    if name not in _PCM_FORMATS:
+        raise ValueError(f"pcm_format must be 'f32' or 's16', got {name!r}")
+    return _PCM_FORMATS[name]
 
 
 class WfRenderBatch(C.Structure):
@@ -343,9 +355,10 @@ class _Inputs:
     """The shared prelude of the engines' process(): `pcm` as [S, channels, samples] (a 2-D array is one stream), checked
     against the engine's channel count and the samples the call needs.  A numpy array becomes contiguous float32 (host
     path); a torch tensor must be a contiguous float32 CUDA tensor (device path), and `stream` is then torch's current
-    stream.  new() allocates an output and aux() brings an optional per-tick input to the same side as pcm."""
+    stream.  new() allocates an output and aux() brings an optional per-tick input to the same side as pcm.
+    With s16=True the samples stay int16 as they are: a numpy int16 array or a contiguous int16 CUDA tensor, else ValueError."""
 
-    def __init__(self, pcm, channels: int, need: int, who: str = "engine"):
+    def __init__(self, pcm, channels: int, need: int, who: str = "engine", s16: bool = False):
         self.is_torch = hasattr(pcm, "data_ptr")
         if pcm.ndim == 2:
             pcm = pcm[None]
@@ -355,13 +368,20 @@ class _Inputs:
         if self.ns < need:
             raise ValueError(f"need {need} samples per channel, got {self.ns}")
         self.stream = None
+        if s16:
+            if self.is_torch:
+                import torch
+                if not (pcm.is_cuda and pcm.dtype == torch.int16 and pcm.is_contiguous()):
+                    raise ValueError("pcm_format='s16' needs a contiguous int16 CUDA tensor")
+            elif not (isinstance(pcm, np.ndarray) and pcm.dtype == np.int16):
+                raise ValueError("pcm_format='s16' needs an int16 numpy array")
         if self.is_torch:
             import torch
-            assert pcm.is_cuda and pcm.dtype == torch.float32 and pcm.is_contiguous()
+            assert s16 or (pcm.is_cuda and pcm.dtype == torch.float32 and pcm.is_contiguous())
             self.f32, self.u8 = torch.float32, torch.uint8
             self.stream = torch.cuda.current_stream(pcm.device).cuda_stream
         else:
-            pcm = np.ascontiguousarray(pcm, dtype=np.float32)
+            pcm = np.ascontiguousarray(pcm, dtype=np.int16 if s16 else np.float32)
             self.f32, self.u8 = np.float32, np.uint8
         self.pcm = pcm
 
@@ -440,8 +460,9 @@ class Engine(_Handle):
     def process_raw(self, pcm_ptr, n_streams, n_frames, hop, stream_stride, channel_stride, *, first_stream=0,
                     seconds=1.0 / 60.0, input_rms=None, skip_mask=None, out_db=None, out_points=None,
                     out_silent=None, out_peak=None, out_pixels=None, out_min=None, stream=None, sync=True,
-                    frame_seconds=None):
-        """Thin wrapper over wf_process / wf_process_async with raw pointers (ints)."""
+                    frame_seconds=None, pcm_format="f32"):
+        """Thin wrapper over wf_process / wf_process_async with raw pointers (ints).  pcm_format: "f32" (float samples) or
+        "s16" (int16 samples, v * 2**-15); strides and hop count samples either way."""
         b = WfBatch()
         b.struct_size = C.sizeof(WfBatch)
         b.n_streams, b.n_frames, b.hop, b.first_stream = n_streams, n_frames, hop, first_stream
@@ -452,6 +473,7 @@ class Engine(_Handle):
         b.out_db, b.out_points, b.out_silent, b.out_peak = out_db, out_points, out_silent, out_peak
         b.out_pixels, b.out_min = out_pixels, out_min
         b.frame_seconds = frame_seconds  # host pointer (int) or None
+        b.pcm_format = _pcm_format(pcm_format)
         if sync and stream is None:
             self._check(self.L.wf_process(self.h, C.byref(b)))
         else:
@@ -461,10 +483,13 @@ class Engine(_Handle):
 
     def process(self, pcm, n_frames: int, hop: int, *, first_stream=0, seconds=1.0 / 60.0, input_rms=None,
                 skip_mask=None, want_db=True, want_points=False, want_silent=True, want_peak=False, want_pixels=False,
-                frame_seconds=None):
+                frame_seconds=None, pcm_format="f32"):
         """pcm: [n_streams, capture_channels, samples] float32 — numpy (host path, staged inside the C call)
-        or a CUDA torch tensor (device path, outputs are CUDA tensors)."""
-        x = _Inputs(pcm, self.capture_channels, (n_frames - 1) * hop + self.fft_size)
+        or a CUDA torch tensor (device path, outputs are CUDA tensors).  pcm_format="s16": int16 samples instead (an int16
+        numpy array or contiguous int16 CUDA tensor), read by the kernels as v * 2**-15; the default converts any numpy
+        array to float32 as it is, without scaling."""
+        s16 = _pcm_format(pcm_format) == PCM_S16
+        x = _Inputs(pcm, self.capture_channels, (n_frames - 1) * hop + self.fft_size, s16=s16)
         S, cc, ns, mk, f32, u8 = x.S, x.cc, x.ns, x.new, x.f32, x.u8
         input_rms, skip_mask = x.aux(input_rms, f32), x.aux(skip_mask, u8)
         dch, B, P = self.display_channels, self.bins, self.num_points
@@ -491,7 +516,8 @@ class Engine(_Handle):
                          input_rms=_ptr(input_rms), skip_mask=_ptr(skip_mask), out_db=_ptr(out.get("db")),
                          out_points=_ptr(out.get("points")), out_silent=_ptr(out.get("silent")),
                          out_peak=_ptr(out.get("peak")), out_pixels=_ptr(out.get("pixels")), out_min=_ptr(out.get("min")),
-                         stream=x.stream, sync=not x.is_torch, frame_seconds=None if fs is None else fs.ctypes.data)
+                         stream=x.stream, sync=not x.is_torch, frame_seconds=None if fs is None else fs.ctypes.data,
+                         pcm_format=pcm_format)
         return out
 
     def synchronize(self):
