@@ -125,7 +125,8 @@ typedef enum wf_table {
     WF_TABLE_GAUSS = 6          /* float[2*ceil(3 sigma)-1] m_kernel.weights */
 } wf_table;
 
-/* Sample format of wf_batch.pcm. */
+/* Sample format of the PCM of all three engines: wf_batch.pcm, wf_meter_batch.pcm and wf_wave_batch.pcm (their
+ * pcm_format field).  An unknown value, or int16 pcm at an odd address, is WF_ERR_INVALID_ARG. */
 typedef enum wf_pcm_format {
     WF_PCM_F32 = 0, /* float samples */
     WF_PCM_S16 = 1  /* int16_t samples; sample v stands for v * 2^-15 exactly ((float)v * 0x1p-15f) */
@@ -312,8 +313,13 @@ typedef struct wf_meter_batch {
     int32_t hop;              /* new samples per tick (>= 1) */
     int32_t first_stream;
     float seconds;            /* tick delta for TVEXPONENTIAL gravity */
-    const float *pcm;         /* planar float PCM, host or device: sample i of channel c of stream s at
-                                 pcm[s*stream_stride + c*channel_stride + i], i < n_ticks*hop */
+    const float *pcm;         /* planar PCM, host or device: sample i of channel c of stream s at
+                                 pcm[s*stream_stride + c*channel_stride + i], i < n_ticks*hop.  float samples, or int16_t
+                                 samples (cast to const float *) when pcm_format is WF_PCM_S16, in which case pcm must be 2-byte
+                                 aligned.  Strides and hop count SAMPLES in either format.  The 4-sample loads and the one-pass
+                                 kernel need pcm aligned to 4 samples (16 B float, 8 B int16) and strides that are multiples of
+                                 4 samples; the facts are the same in samples for both formats, so an S16 call takes the F32
+                                 call's path and gives bit for bit the F32 results on (float)v * 0x1p-15f, state included. */
     int64_t stream_stride;
     int64_t channel_stride;
     float *out_db;            /* optional [n_streams][n_ticks][capture_channels] m_meter_val (dBFS); unused for INPUT_RMS */
@@ -325,6 +331,10 @@ typedef struct wf_meter_batch {
      * lerp(border_top, border_bottom, clamp(ceiling - m_meter_val, 0, range) / range) */
     float *out_pixels;        /* [n_streams][n_ticks][capture_channels] */
     float *out_min;           /* [n_streams][n_ticks][2]: (miny, minpos) — first strict minimum, starting from (height, 0) */
+    int32_t pcm_format;       /* wf_pcm_format of pcm (0 = WF_PCM_F32).  The ring and the EMA state hold float either way, so
+                                 calls of both formats may follow each other on one engine.  A caller built against the previous
+                                 header (struct_size = offsetof(wf_meter_batch, pcm_format)) passes float PCM; the size before
+                                 that (offsetof(wf_meter_batch, out_pixels)) is still accepted too. */
 } wf_meter_batch;
 
 typedef struct wf_meter wf_meter;
@@ -382,7 +392,10 @@ typedef struct wf_wave_batch {
     int32_t n_streams;        /* must equal max_streams */
     int32_t n_ticks;
     int32_t hop;              /* samples per capture packet / tick (>= 1) */
-    const float *pcm;         /* planar float PCM, host or device; >= n_ticks*hop samples per channel */
+    const float *pcm;         /* planar PCM, host or device; >= n_ticks*hop samples per channel.  float samples, or int16_t
+                                 samples (cast to const float *) when pcm_format is WF_PCM_S16, in which case pcm must be 2-byte
+                                 aligned.  Strides and hop count SAMPLES in either format; an S16 call gives bit for bit the
+                                 F32 results on (float)v * 0x1p-15f, state included. */
     int64_t stream_stride;
     int64_t channel_stride;
     const float *input_rms;   /* optional [n_streams][n_ticks] m_input_rms per tick (volume normalisation) */
@@ -394,6 +407,9 @@ typedef struct wf_wave_batch {
     float *out_points;        /* [n_streams][n_ticks][display_channels][width] interpolated (+ Gaussian-smoothed) dB */
     float *out_pixels;        /* same shape: m_interp_bufs after the dB -> pixel lerp/clamp (height measured from the top) */
     float *out_min;           /* [n_streams][n_ticks][2]: (miny, minpos), first strict minimum over both channels from (cpos, 0) */
+    int32_t pcm_format;       /* wf_pcm_format of pcm (0 = WF_PCM_F32).  A caller built against the previous header
+                                 (struct_size = offsetof(wf_wave_batch, pcm_format)) passes float PCM; the size before that
+                                 (offsetof(wf_wave_batch, out_points)) is still accepted too. */
 } wf_wave_batch;
 
 typedef struct wf_wave wf_wave;

@@ -857,7 +857,7 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
     NvtxRange nvtx("wf_process");
     // the current struct or the previous one (which ends before pcm_format: float PCM)
     wf_batch bv;
-    if(!accept_struct(b_in, offsetof(wf_batch, pcm_format), bv))
+    if(!accept_struct(b_in, {offsetof(wf_batch, pcm_format)}, bv))
         return fail(e, WF_ERR_ABI, "wf_batch.struct_size %u != %zu", b_in->struct_size, sizeof(wf_batch));
     const wf_batch *b = &bv;
     const Tables &t = e->tab;
@@ -873,12 +873,10 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
         return fail(e, WF_ERR_INVALID_ARG, "pcm is null");
     if(b->stream_stride < 0 || b->channel_stride < 0)
         return fail(e, WF_ERR_INVALID_ARG, "negative strides are not supported");
-    if(b->pcm_format != WF_PCM_F32 && b->pcm_format != WF_PCM_S16)
-        return fail(e, WF_ERR_INVALID_ARG, "pcm_format %d is not a wf_pcm_format", b->pcm_format);
+    size_t sample_bytes = 0;
+    if(int rc = pcm_sample_bytes(e, b->pcm_format, b->pcm, &sample_bytes))
+        return rc;
     const bool s16 = b->pcm_format == WF_PCM_S16;
-    const size_t sample_bytes = s16 ? sizeof(int16_t) : sizeof(float);
-    if(s16 && ((uintptr_t)b->pcm & 1u) != 0)
-        return fail(e, WF_ERR_INVALID_ARG, "int16 pcm must be 2-byte aligned");
     if(t.cfg.normalize_volume && !b->input_rms)
         return fail(e, WF_ERR_INVALID_ARG, "normalize_volume is set but the batch carries no input_rms (m_input_rms per tick: "
                                               "wf_meter in WF_METER_INPUT_RMS mode, or the host's own update_input_rms)");

@@ -106,6 +106,17 @@ cudaError_t opt_in_smem(const void *kernel, int device, size_t bytes)
     return err;
 }
 
+int pcm_sample_bytes(HostCore *c, int32_t format, const void *pcm, size_t *bytes)
+{
+    if(format != WF_PCM_F32 && format != WF_PCM_S16)
+        return fail(c, WF_ERR_INVALID_ARG, "pcm_format %d is not a wf_pcm_format", format);
+    const bool s16 = format == WF_PCM_S16;
+    if(s16 && ((uintptr_t)pcm & 1u) != 0)
+        return fail(c, WF_ERR_INVALID_ARG, "int16 pcm must be 2-byte aligned");
+    *bytes = s16 ? sizeof(int16_t) : sizeof(float);
+    return WF_OK;
+}
+
 float last_kernel_ms(HostCore *c)
 {
     if(!c || !c->ev_valid || cudaEventSynchronize(c->ev1) != cudaSuccess)

@@ -10,6 +10,7 @@
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <new>
 #include <string>
 #include <utility>
@@ -131,21 +132,31 @@ struct DevBuf {
     }
 };
 
-// A caller's struct of the current size, or of the previous ABI's size (`prev_size`: it ends before the fields added
-// since, which then read as zero).  False for any other struct_size.  `out` carries the current struct_size either way.
+// A caller's struct of the current size, or of one of the earlier ABI sizes in `prev_sizes` (each ends before the fields
+// added since, which then read as zero).  False for any other struct_size.  `out` carries the current struct_size either way;
+// `is_current` tells whether the caller passed the current size.
 template<class T>
-bool accept_struct(const T *in, size_t prev_size, T &out, bool *is_current = nullptr)
+bool accept_struct(const T *in, std::initializer_list<size_t> prev_sizes, T &out, bool *is_current = nullptr)
 {
     const bool cur = in->struct_size == sizeof(T);
-    if(!cur && in->struct_size != prev_size)
+    size_t n = cur ? sizeof(T) : 0;
+    for(const size_t prev : prev_sizes)
+        if(!cur && in->struct_size == prev)
+            n = prev;
+    if(n == 0)
         return false;
     out = T{};
-    memcpy(&out, in, cur ? sizeof(T) : prev_size);
+    memcpy(&out, in, n);
     out.struct_size = (uint32_t)sizeof(T);
     if(is_current)
         *is_current = cur;
     return true;
 }
+
+// The sample format of a call's PCM (wf_pcm_format; wf_batch, wf_meter_batch and wf_wave_batch carry the same field):
+// `bytes` := bytes per sample.  WF_ERR_INVALID_ARG for a value that is not a wf_pcm_format, or for int16 PCM at an odd
+// address.
+int pcm_sample_bytes(HostCore *c, int32_t format, const void *pcm, size_t *bytes);
 
 // Lets `kernel` use `bytes` of dynamic shared memory on `device` (the opt-in above the default 48 KB).  Asks CUDA once per
 // kernel, device and size: a size at or below one already granted returns at once.
@@ -213,9 +224,15 @@ class Staging {
     template<class T>
     const T *in(DevBuf<T> &buf, const T *src, size_t n)
     {
-        if(!take(buf, src, n))
+        return in_bytes(buf, src, n * sizeof(T));
+    }
+    // an input of `bytes` bytes held in a buffer of T (int16 PCM behind a `const float *`): exactly those bytes are copied
+    template<class T>
+    const T *in_bytes(DevBuf<T> &buf, const T *src, size_t bytes)
+    {
+        if(!take(buf, src, (bytes + sizeof(T) - 1) / sizeof(T)))
             return src;
-        rc = copy(buf.p, src, n * sizeof(T), cudaMemcpyHostToDevice);
+        rc = copy(buf.p, src, bytes, cudaMemcpyHostToDevice);
         return buf.p;
     }
     template<class T>

@@ -14,6 +14,9 @@
 //                       edges from the samples if any — O(W/block) instead of O(W) per tick, windows overlap W/hop times;
 //   K3 recurrence       one thread per stream walks the ticks: sqrt/mean, EMA (fast-peaks rule), dBFS, m_last_silent;
 //   (history)           K1 also writes the last W samples of the timeline into the (double-buffered) ring for the next call.
+// The kernels that read PCM take its sample type (float or int16_t, wf_meter_batch.pcm_format) as their last template
+// argument and load it only through Pcm<TS> (wf_pcm.cuh).  The ring and the partials hold float whatever the input: an int16
+// call widens its samples as it loads them, sums them in the float call's order, and leaves the state a float call leaves.
 // There is no CPU fallback.
 #include <cuda_runtime.h>
 
@@ -26,6 +29,7 @@
 #include "wf_display.cuh"
 #include "wf_host.hpp"
 #include "wf_nvtx.hpp"
+#include "wf_pcm.cuh"
 #include "wf_tables.hpp"
 #include "wfstft.h"
 
@@ -81,16 +85,21 @@ __device__ __forceinline__ void meter_pixels(const MParams &p, size_t st, float 
 }
 
 // Row pointers of one (stream, channel): history ring first (timeline positions [0, W)), then this call's PCM.
+template<typename TS>
 struct Row {
-    const float *hist, *pcm;
+    const float *hist;
+    const TS *pcm;
 };
-__device__ __forceinline__ Row row_of(const MParams &p, int s, int c)
+template<typename TS>
+__device__ __forceinline__ Row<TS> row_of(const MParams &p, int s, int c)
 {
-    return {p.hist + ((size_t)s * p.cc + c) * p.W, p.pcm + (size_t)s * p.stream_stride + (size_t)c * p.channel_stride};
+    return {p.hist + ((size_t)s * p.cc + c) * p.W,
+            wf::Pcm<TS>::base(p.pcm) + (size_t)s * p.stream_stride + (size_t)c * p.channel_stride};
 }
-__device__ __forceinline__ float vsample(const Row &r, int W, long long u)
+template<typename TS>
+__device__ __forceinline__ float vsample(const Row<TS> &r, int W, long long u)
 {
-    return (u < W) ? r.hist[u] : __ldg(r.pcm + (u - W));
+    return (u < W) ? r.hist[u] : wf::Pcm<TS>::ldg1(r.pcm + (u - W));
 }
 
 template<int MODE>
@@ -118,8 +127,8 @@ __device__ __forceinline__ float warp_combine(float v)
     return v;
 }
 // scalar reduction of timeline positions [lo, hi) by one warp (ragged edges, history, unaligned PCM)
-template<int MODE>
-__device__ __forceinline__ float reduce_range(const Row &r0, const Row &r1, bool two, int W, long long lo, long long hi,
+template<int MODE, typename TS>
+__device__ __forceinline__ float reduce_range(const Row<TS> &r0, const Row<TS> &r1, bool two, int W, long long lo, long long hi,
                                               int lane, float acc)
 {
     for(long long u = lo + lane; u < hi; u += 32)
@@ -132,10 +141,11 @@ __device__ __forceinline__ float reduce_range(const Row &r0, const Row &r1, bool
 }
 
 // K1: one warp per (stream, partial channel, 256-sample chunk): lane l reduces samples [8l, 8l+8) of the chunk, groups of
-// bl/8 lanes combine into one partial per bl-sample block.  Chunks that lie wholly inside 16-byte aligned new PCM (all
-// but the few that touch the history ring or the end) take two 128-bit loads per lane.  The same pass writes the last W
-// samples of the timeline into the ring for the next call (every sample is read exactly once here).
-template<int MODE>
+// bl/8 lanes combine into one partial per bl-sample block.  Chunks that lie wholly inside new PCM aligned to 4 samples (all
+// but the few that touch the history ring or the end) take two 4-sample loads per lane (128-bit for float, 64-bit for
+// int16) and sum them as a pairwise tree; the others load and sum their 8 samples in sequence.  The same pass writes the last
+// W samples of the timeline into the ring for the next call (every sample is read exactly once here).
+template<int MODE, typename TS>
 __global__ void meter_block_kernel(const MParams p, const int vec4)
 {
     const int warps_per_cta = blockDim.x >> 5;
@@ -153,22 +163,23 @@ __global__ void meter_block_kernel(const MParams p, const int vec4)
         const int c = (int)((w / p.nchunk) % p.pc);
         const int s = (int)(w / ((long long)p.nchunk * p.pc));
         const long long u0 = (long long)j * kChunk;
-        const Row r0 = row_of(p, s, c);
-        const Row r1 = two ? row_of(p, s, 1) : r0;
+        const Row<TS> r0 = row_of<TS>(p, s, c);
+        const Row<TS> r1 = two ? row_of<TS>(p, s, 1) : r0;
         float *h0 = p.hist_next + ((size_t)s * p.cc + c) * p.W;
         float *h1 = p.hist_next + ((size_t)s * p.cc + 1) * p.W;
         float acc = 0.0f;
         const long long ul = u0 + 8 * lane; // my 8 samples
         if(vec4 && u0 >= p.W && u0 + kChunk <= L)
         {
-            const float4 *q0 = reinterpret_cast<const float4 *>(r0.pcm + (ul - p.W));
-            const float4 a = __ldg(q0), b = __ldg(q0 + 1);
+            using Quad = typename wf::Pcm<TS>::Quad;
+            const Quad *q0 = reinterpret_cast<const Quad *>(r0.pcm + (ul - p.W));
+            const float4 a = wf::Pcm<TS>::ldg4(q0), b = wf::Pcm<TS>::ldg4(q0 + 1);
             float4 a1 = make_float4(0.f, 0.f, 0.f, 0.f), b1 = a1;
             if(two)
             {
-                const float4 *q1 = reinterpret_cast<const float4 *>(r1.pcm + (ul - p.W));
-                a1 = __ldg(q1);
-                b1 = __ldg(q1 + 1);
+                const Quad *q1 = reinterpret_cast<const Quad *>(r1.pcm + (ul - p.W));
+                a1 = wf::Pcm<TS>::ldg4(q1);
+                b1 = wf::Pcm<TS>::ldg4(q1 + 1);
             }
             acc = combine<MODE>(combine<MODE>(contrib<MODE>(a.x, a1.x), contrib<MODE>(a.y, a1.y)),
                                 combine<MODE>(contrib<MODE>(a.z, a1.z), contrib<MODE>(a.w, a1.w)));
@@ -236,7 +247,7 @@ __global__ void meter_block_kernel(const MParams p, const int vec4)
 }
 
 // K2: one warp per (stream, tick, partial channel): window [lo, hi) of the timeline
-template<int MODE>
+template<int MODE, typename TS>
 __global__ void meter_window_kernel(const MParams p)
 {
     const int warps_per_cta = blockDim.x >> 5;
@@ -251,8 +262,8 @@ __global__ void meter_window_kernel(const MParams p)
         const int s = (int)(w / ((long long)p.pc * p.n_ticks));
         const long long lo = (long long)(t + 1) * p.hop, hi = lo + p.W;
         const long long jb = (lo + p.bl - 1) / p.bl, je = hi / p.bl;
-        const Row r0 = row_of(p, s, c);
-        const Row r1 = two ? row_of(p, s, 1) : r0;
+        const Row<TS> r0 = row_of<TS>(p, s, c);
+        const Row<TS> r1 = two ? row_of<TS>(p, s, 1) : r0;
         float acc = 0.0f;
         if(jb <= je)
         {
@@ -324,11 +335,12 @@ __global__ void meter_scan_kernel(const MParams p)
 
 // ---- one-pass path: hop divides the window (the plugin's usual case: 150 ms at 48 kHz = 7200 = 9 x 800 samples at 60 fps) ----
 // One CTA per stream.  Every hop-sized block of the stream's timeline (W/hop blocks of history ring, then one block per
-// tick) is reduced ONCE by one warp with 128-bit loads — the same pass copies the last W samples into the next call's ring —
+// tick) is reduced ONCE by one warp with 4-sample loads — the same pass copies the last W samples into the next call's ring —
 // and its partial lands in shared memory; a tick's window is then exactly W/hop consecutive partials, combined by one
 // thread per (tick, channel); finally the per-stream recurrence (EMA, dBFS, m_last_silent) runs on one lane per channel.
 // Samples cross HBM once, nothing else does: the three-kernel path above wrote and re-read per-32-sample partials W/hop times.
-template<int MODE>
+// A lane's groups of 4 samples are i0 + 32u whatever the sample type: int16 blocks take 64-bit loads in the same grouping.
+template<int MODE, typename TS>
 __global__ void __launch_bounds__(256) meter_fused_kernel(const MParams p)
 {
     extern __shared__ float sm[];
@@ -351,15 +363,21 @@ __global__ void __launch_bounds__(256) meter_fused_kernel(const MParams p)
         const int c = w / NB, b = w - c * NB;
         if(have_part && b < nb && b < T)
             continue;
-        const Row r0 = row_of(p, s, c);
-        const Row r1 = two ? row_of(p, s, 1) : r0;
-        const float4 *src0 = reinterpret_cast<const float4 *>((b < nb) ? r0.hist + (size_t)b * hop : r0.pcm + (size_t)(b - nb) * hop);
-        const float4 *src1 = reinterpret_cast<const float4 *>((b < nb) ? r1.hist + (size_t)b * hop : r1.pcm + (size_t)(b - nb) * hop);
+        const Row<TS> r0 = row_of<TS>(p, s, c);
+        const Row<TS> r1 = two ? row_of<TS>(p, s, 1) : r0;
+        // block b: the ring (float, read as float4) for b < nb, else this call's PCM (read as Pcm<TS>::Quad); group i is
+        // samples [4i, 4i+4) of the block either way
+        using Quad = typename wf::Pcm<TS>::Quad;
+        const Quad *src0 = reinterpret_cast<const Quad *>((b < nb) ? reinterpret_cast<const TS *>(r0.hist + (size_t)b * hop)
+                                                                   : r0.pcm + (size_t)(b - nb) * hop);
+        const Quad *src1 = reinterpret_cast<const Quad *>((b < nb) ? reinterpret_cast<const TS *>(r1.hist + (size_t)b * hop)
+                                                                   : r1.pcm + (size_t)(b - nb) * hop);
         const bool keep = b >= T; // one of the last W/hop blocks: belongs to the next call's ring
         float4 *h0 = reinterpret_cast<float4 *>(p.hist_next + ((size_t)s * cc + c) * W + (size_t)(b - T) * hop);
         float4 *h1 = reinterpret_cast<float4 *>(p.hist_next + ((size_t)s * cc + 1) * W + (size_t)(b - T) * hop);
         float acc = 0.0f;
-        // four 128-bit loads in flight per lane and channel (a hop of 800 samples is 6.25 loads per lane)
+        // four loads in flight per lane and channel, 128-bit for float and 64-bit for int16 (a hop of 800 samples is 6.25 loads
+        // per lane; eight int16 loads in flight cost registers and occupancy and were slower)
         for(int i0 = lane; i0 < q4; i0 += 128)
         {
             float4 a[4], a1[4];
@@ -371,9 +389,9 @@ __global__ void __launch_bounds__(256) meter_fused_kernel(const MParams p)
                 a1[u] = a[u];
                 if(i < q4)
                 {
-                    a[u] = (b < nb) ? src0[i] : __ldg(src0 + i);
+                    a[u] = (b < nb) ? reinterpret_cast<const float4 *>(src0)[i] : wf::Pcm<TS>::ldg4(src0 + i);
                     if(two)
-                        a1[u] = (b < nb) ? src1[i] : __ldg(src1 + i);
+                        a1[u] = (b < nb) ? reinterpret_cast<const float4 *>(src1)[i] : wf::Pcm<TS>::ldg4(src1 + i);
                 }
             }
 #pragma unroll
@@ -556,7 +574,7 @@ int wf_meter_create(const wf_meter_config *cfg_in, wf_meter **out)
     return wf::create_engine(out, g_meter_create_error, wf_meter_destroy, [&](wf_meter *m) -> int {
         // the current struct or the previous one, which ends before height: its display settings are absent
         bool display_settings = false;
-        if(!wf::accept_struct(cfg_in, offsetof(wf_meter_config, height), m->cfg, &display_settings))
+        if(!wf::accept_struct(cfg_in, {offsetof(wf_meter_config, height)}, m->cfg, &display_settings))
             return wf::fail(m, WF_ERR_ABI, "wf_meter_config.struct_size mismatch");
         const wf_meter_config *cfg = &m->cfg;
         if(cfg->capture_channels < 1 || cfg->capture_channels > 2 || cfg->max_streams < 1 || cfg->sample_rate < 16 ||
@@ -637,9 +655,10 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b_in, void *cuda_s
     if(!m || !b_in)
         return WF_ERR_INVALID_ARG;
     wf::NvtxRange nvtx("wf_meter_process");
-    // the current struct or the previous one (which ends before out_pixels: no display outputs)
+    // the current struct, the previous one (which ends before pcm_format: float PCM) or the one before (which ends before
+    // out_pixels: no display outputs either)
     wf_meter_batch bv;
-    if(!wf::accept_struct(b_in, offsetof(wf_meter_batch, out_pixels), bv))
+    if(!wf::accept_struct(b_in, {offsetof(wf_meter_batch, pcm_format), offsetof(wf_meter_batch, out_pixels)}, bv))
         return wf::fail(m, WF_ERR_ABI, "wf_meter_batch.struct_size %u != %zu", b_in->struct_size, sizeof(wf_meter_batch));
     const wf_meter_batch *b = &bv;
     if((b->out_pixels || b->out_min) && !m->display)
@@ -657,6 +676,10 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b_in, void *cuda_s
         return wf::fail(m, WF_ERR_INVALID_ARG, "pcm is null");
     if(b->stream_stride < 0 || b->channel_stride < 0)
         return wf::fail(m, WF_ERR_INVALID_ARG, "negative strides are not supported");
+    size_t sample_bytes = 0;
+    if(int rc = wf::pcm_sample_bytes(m, b->pcm_format, b->pcm, &sample_bytes))
+        return rc;
+    const bool s16 = b->pcm_format == WF_PCM_S16;
     if((long long)b->n_ticks * b->hop > 0x7fffffffLL - m->W)
         return wf::fail(m, WF_ERR_INVALID_ARG, "n_ticks * hop too large for one call");
 
@@ -686,7 +709,7 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b_in, void *cuda_s
     // a call with host buffers (told by pcm alone) is staged through device memory; the RMS feed has no dB / silent outputs
     const size_t span = (S - 1) * (size_t)b->stream_stride + (size_t)(cc - 1) * (size_t)b->channel_stride + T * (size_t)b->hop;
     wf::Staging io(m, st, !wf::is_device_ptr(b->pcm));
-    const float *d_pcm = io.in(m->s_pcm, b->pcm, span);
+    const float *d_pcm = io.in_bytes(m->s_pcm, b->pcm, span * sample_bytes);
     float *d_db = io.out(m->s_db, is_feed ? nullptr : b->out_db, out_n);
     float *d_lin = io.out(m->s_lin, b->out_lin, out_n);
     unsigned char *d_silent = io.out(m->s_silent, is_feed ? nullptr : b->out_silent, S * T);
@@ -740,8 +763,10 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b_in, void *cuda_s
 
     WF_CHECK(m, cudaEventRecord(m->ev0, st));
     constexpr int kWarps = 8;
-    // 128-bit loads need 16-byte aligned rows (W is a multiple of 16 samples already)
-    const int vec4 = (((uintptr_t)d_pcm & 15u) == 0) && ((b->stream_stride & 3) == 0) && ((b->channel_stride & 3) == 0);
+    // 4-sample group loads (128-bit for float, 64-bit for int16) need rows aligned to 4 samples (W is a multiple of 16
+    // samples already).  The facts are stated in samples, so an int16 call takes the float call's path and summation order.
+    const int vec4 = (((uintptr_t)d_pcm & (4 * sample_bytes - 1)) == 0) && ((b->stream_stride & 3) == 0) &&
+                     ((b->channel_stride & 3) == 0);
     // one-pass path: the window is a whole number of hops (meter_fused_kernel)
     const size_t fused_smem = ((size_t)pc * ((size_t)(W / b->hop) + T) + T * pc) * sizeof(float);
     const bool fused = m->use_fused && vec4 && (W % b->hop) == 0 && (b->hop % 4) == 0 && fused_smem <= 96 * 1024;
@@ -772,33 +797,44 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b_in, void *cuda_s
             kernel<<<(int)S, 256, fused_smem, st>>>(p);
             return cudaGetLastError();
         };
-        switch(m->cfg.mode)
-        {
-        case WF_METER_PEAK: WF_CHECK(m, launch(meter_fused_kernel<WF_METER_PEAK>)); break;
-        case WF_METER_RMS: WF_CHECK(m, launch(meter_fused_kernel<WF_METER_RMS>)); break;
-        default: WF_CHECK(m, launch(meter_fused_kernel<WF_METER_INPUT_RMS>)); break;
-        }
+        auto launch_mode = [&](auto ts) -> cudaError_t {
+            using TS = decltype(ts);
+            switch(m->cfg.mode)
+            {
+            case WF_METER_PEAK: return launch(meter_fused_kernel<WF_METER_PEAK, TS>);
+            case WF_METER_RMS: return launch(meter_fused_kernel<WF_METER_RMS, TS>);
+            default: return launch(meter_fused_kernel<WF_METER_INPUT_RMS, TS>);
+            }
+        };
+        WF_CHECK(m, s16 ? launch_mode(int16_t{}) : launch_mode(float{}));
         m->launches += 1;
     }
     else
     {
     m->part_hop = 0; // the general path does not maintain the block partials
     const int g1 = grid_for((long long)S * pc * nchunk, kWarps, m->sm_count), g2 = grid_for((long long)S * T * pc, kWarps, m->sm_count);
-    switch(m->cfg.mode)
-    {
-    case WF_METER_PEAK:
-        meter_block_kernel<WF_METER_PEAK><<<g1, kWarps * 32, 0, st>>>(p, vec4);
-        meter_window_kernel<WF_METER_PEAK><<<g2, kWarps * 32, 0, st>>>(p);
-        break;
-    case WF_METER_RMS:
-        meter_block_kernel<WF_METER_RMS><<<g1, kWarps * 32, 0, st>>>(p, vec4);
-        meter_window_kernel<WF_METER_RMS><<<g2, kWarps * 32, 0, st>>>(p);
-        break;
-    default:
-        meter_block_kernel<WF_METER_INPUT_RMS><<<g1, kWarps * 32, 0, st>>>(p, vec4);
-        meter_window_kernel<WF_METER_INPUT_RMS><<<g2, kWarps * 32, 0, st>>>(p);
-        break;
-    }
+    auto launch_k12 = [&](auto ts) {
+        using TS = decltype(ts);
+        switch(m->cfg.mode)
+        {
+        case WF_METER_PEAK:
+            meter_block_kernel<WF_METER_PEAK, TS><<<g1, kWarps * 32, 0, st>>>(p, vec4);
+            meter_window_kernel<WF_METER_PEAK, TS><<<g2, kWarps * 32, 0, st>>>(p);
+            break;
+        case WF_METER_RMS:
+            meter_block_kernel<WF_METER_RMS, TS><<<g1, kWarps * 32, 0, st>>>(p, vec4);
+            meter_window_kernel<WF_METER_RMS, TS><<<g2, kWarps * 32, 0, st>>>(p);
+            break;
+        default:
+            meter_block_kernel<WF_METER_INPUT_RMS, TS><<<g1, kWarps * 32, 0, st>>>(p, vec4);
+            meter_window_kernel<WF_METER_INPUT_RMS, TS><<<g2, kWarps * 32, 0, st>>>(p);
+            break;
+        }
+    };
+    if(s16)
+        launch_k12(int16_t{});
+    else
+        launch_k12(float{});
     WF_CHECK(m, cudaGetLastError());
     meter_scan_kernel<<<(int)((S + 127) / 128), 128, 0, st>>>(p);
     WF_CHECK(m, cudaGetLastError());

@@ -1,10 +1,14 @@
-// wf_pcm.cuh — the PCM sample formats of wf_batch.pcm_format, as the spectrum kernels' frame loads see them.
+// wf_pcm.cuh — the PCM sample formats (wf_pcm_format) of wf_batch, wf_meter_batch and wf_wave_batch, as the kernels of all
+// three engines load them.
 //
-// Every family loads its frames through Pcm<TS> (TS = float or int16_t): the streamed global loads of one or two samples,
-// the read of a sample pair out of a TMA landing buffer, and the byte counts (frame size, TMA transfer, L2 lines).  The
-// samples come out as float; an int16 sample v is v * 2^-15, which is exact in float32, so an int16 frame and the float
-// frame holding the same values go through the rest of the pipeline (window, FFT, EMA, dB, display) identically.
-// Pointers into the PCM stay `const float *` in KParams; Pcm<TS>::base reinterprets them, and offsets count samples.
+// Every kernel that reads PCM does so through Pcm<TS> (TS = float or int16_t).  The spectrum families use the streamed
+// global loads of one or two samples, the read of a sample pair out of a TMA landing buffer, and the byte counts (frame size,
+// TMA transfer, L2 lines).  The level meter uses the read-only-path loads of one sample and of a group of four (16 bytes of
+// float, 8 bytes of int16), and the waveform gathers single samples.  The samples come out as float; an int16 sample v is
+// v * 2^-15, which is exact in float32, so int16 input and the float input holding the same values go through the rest of
+// each pipeline (window, FFT, EMA, dB, display; the meter's sums and ring; the waveform's buffers) identically.
+// Pointers into the PCM stay `const float *` in the kernels' parameters; Pcm<TS>::base reinterprets them, and offsets
+// count samples.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -32,11 +36,15 @@ struct Pcm;
 template<>
 struct Pcm<float> {
     using Pair = float2;           // two consecutive samples, loaded as one (8-byte aligned)
+    using Quad = float4;           // four consecutive samples, loaded as one (16-byte aligned)
     static constexpr int kBytes = 4;
     static __host__ __device__ constexpr uint32_t frame_bytes(int n) { return (uint32_t)n * 4u; }
     static __device__ __forceinline__ const float *base(const float *pcm) { return pcm; }
     static __device__ __forceinline__ float load1(const float *q) { return ldg_stream_f1(q); }
     static __device__ __forceinline__ float2 load2(const Pair *q) { return ldg_stream_f2(q); }
+    // read-only-path loads (ld.global.nc) of one sample and of four
+    static __device__ __forceinline__ float ldg1(const float *q) { return __ldg(q); }
+    static __device__ __forceinline__ float4 ldg4(const Quad *q) { return __ldg(q); }
     // sample pair n (samples 2n, 2n+1) of a frame staged in shared memory, as a packed complex value
     static __device__ __forceinline__ pk::c64 smem_pair(const void *land, int n)
     {
@@ -47,6 +55,7 @@ struct Pcm<float> {
 template<>
 struct Pcm<int16_t> {
     using Pair = uint32_t;         // two consecutive samples, loaded as one (4-byte aligned)
+    using Quad = uint2;            // four consecutive samples, loaded as one (8-byte aligned)
     static constexpr int kBytes = 2;
     static __host__ __device__ constexpr uint32_t frame_bytes(int n) { return (uint32_t)n * 2u; }
     static __device__ __forceinline__ const int16_t *base(const float *pcm) { return reinterpret_cast<const int16_t *>(pcm); }
@@ -66,6 +75,19 @@ struct Pcm<int16_t> {
         uint32_t w;
         asm volatile("ld.global.nc.L1::no_allocate.b32 %0, [%1];" : "=r"(w) : "l"(q));
         return widen2(w);
+    }
+    // The same value as widen(): the bits 0x4b400000 + v are the float 1.5 * 2^23 + v (its ulp is 1), and
+    // (1.5 * 2^23 + v) * 2^-15 - 384 = v * 2^-15 is exact in one FMA (v = 0 gives +0.0f).  An integer add and an FMA in
+    // place of I2F keep the waveform display kernels within their 64 registers without spills.
+    static __device__ __forceinline__ float ldg1(const int16_t *q)
+    {
+        return __fmaf_rn(__int_as_float(0x4b400000 + (int)__ldg(q)), 0x1p-15f, -384.0f);
+    }
+    static __device__ __forceinline__ float4 ldg4(const Quad *q) // widened in sample order
+    {
+        const uint2 w = __ldg(q);
+        const float2 lo = widen2(w.x), hi = widen2(w.y);
+        return make_float4(lo.x, lo.y, hi.x, hi.y);
     }
     static __device__ __forceinline__ pk::c64 smem_pair(const void *land, int n)
     {

@@ -10,7 +10,10 @@
 // each, which sample of the packet it takes — integer arithmetic, bit-exact) and the device does what is left per stream:
 // gather the samples, keep the scrolling buffer (a ring in shared memory), evaluate the all-zero "silent" rule, convert
 // the new points to dBFS (|x|, stereo / mono mix), add the volume compensation, and write the buffer row of every tick.
-// HBM traffic: the packet's sectors once in, width floats per display channel and tick out.  There is no CPU fallback.
+// HBM traffic: the packet's sectors once in, width floats per display channel and tick out.  The kernels take the sample
+// type of the PCM (float or int16_t, wf_wave_batch.pcm_format) as their last template argument and gather it only through
+// Pcm<TS> (wf_pcm.cuh); everything after the gather (buffers, silent rule, dBFS, display) sees the widened floats, so an
+// int16 call and the float call on the same values agree bit for bit.  There is no CPU fallback.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -25,6 +28,7 @@
 #include "wf_display.cuh"
 #include "wf_host.hpp"
 #include "wf_nvtx.hpp"
+#include "wf_pcm.cuh"
 #include "wf_tables.hpp"
 #include "wfstft.h"
 
@@ -287,7 +291,7 @@ __device__ __forceinline__ void wave_display(const WDisp &p, const Seg &seg, int
 
 // One CTA per stream; the scrolling buffers live in shared memory as rings (head = oldest point).  DISP: with the display
 // stage after every tick (out may then be null).
-template<class P>
+template<class P, typename TS>
 __global__ void __launch_bounds__(256, std::is_same_v<P, WDisp> ? 4 : 0) wave_kernel(const P p)
 {
     constexpr bool DISP = std::is_same_v<P, WDisp>;
@@ -300,8 +304,8 @@ __global__ void __launch_bounds__(256, std::is_same_v<P, WDisp> ? 4 : 0) wave_ke
             ring[i] = p.state[(size_t)s * 2 * W + i];
         int head = 0;
         bool last_silent = p.flags[s] != 0;
-        const float *pcm0 = p.pcm + (size_t)s * p.stream_stride;
-        const float *pcm1 = pcm0 + p.channel_stride;
+        const TS *pcm0 = wf::Pcm<TS>::base(p.pcm) + (size_t)s * p.stream_stride;
+        const TS *pcm1 = pcm0 + p.channel_stride;
         __syncthreads();
         for(int t = 0; t < p.n_ticks; ++t)
         {
@@ -312,9 +316,9 @@ __global__ void __launch_bounds__(256, std::is_same_v<P, WDisp> ? 4 : 0) wave_ke
                 const int q = __ldg(p.src + o0 + i);
                 int pos = head + i;
                 pos -= (pos >= W) ? W : 0;
-                r0[pos] = (q >= 0) ? __ldg(pcm0 + q) : 0.0f;
+                r0[pos] = (q >= 0) ? wf::Pcm<TS>::ldg1(pcm0 + q) : 0.0f;
                 if(p.cc > 1)
-                    r1[pos] = (q >= 0) ? __ldg(pcm1 + q) : 0.0f;
+                    r1[pos] = (q >= 0) ? wf::Pcm<TS>::ldg1(pcm1 + q) : 0.0f;
             }
             head += cnt;
             head -= (head >= W) ? W : 0;
@@ -452,7 +456,7 @@ __device__ __forceinline__ int wrap2(int x, int cap) { return x - ((x >= cap) ? 
 
 // DISP: the display stage runs over the rows of every chunk after they are stored (out may then be null).  Its instantiations
 // get 64 registers (4 CTAs per SM) instead of 48: the plain ones keep their budget.
-template<int MODE, class P>
+template<int MODE, class P, typename TS>
 __global__ void __launch_bounds__(256, std::is_same_v<P, WDisp> ? 4 : 5) wave_chunk_kernel(const P p)
 {
     constexpr bool DISP = std::is_same_v<P, WDisp>;
@@ -470,8 +474,8 @@ __global__ void __launch_bounds__(256, std::is_same_v<P, WDisp> ? 4 : 5) wave_ch
     const bool vec = ((W & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 15) == 0);
     for(int s = blockIdx.x; s < p.n_streams; s += gridDim.x)
     {
-        const float *pcm0 = p.pcm + (size_t)s * p.stream_stride;
-        const float *pcm1 = pcm0 + p.channel_stride;
+        const TS *pcm0 = wf::Pcm<TS>::base(p.pcm) + (size_t)s * p.stream_stride;
+        const TS *pcm1 = pcm0 + p.channel_stride;
         float *st0 = p.state + (size_t)s * 2 * W, *st1 = st0 + W;
         int wc0 = 0, wc1 = 0; // non-zero entries in the current window of E0 / E1
         {
@@ -570,8 +574,8 @@ __global__ void __launch_bounds__(256, std::is_same_v<P, WDisp> ? 4 : 5) wave_ch
 #pragma unroll
                     for(int u = 0; u < WCH_U; ++u)
                     {
-                        ra[u] = (q[u] >= 0) ? __ldg(pcm0 + q[u]) : 0.0f;
-                        rb[u] = (TWO && q[u] >= 0) ? __ldg(pcm1 + q[u]) : 0.0f;
+                        ra[u] = (q[u] >= 0) ? wf::Pcm<TS>::ldg1(pcm0 + q[u]) : 0.0f;
+                        rb[u] = (TWO && q[u] >= 0) ? wf::Pcm<TS>::ldg1(pcm1 + q[u]) : 0.0f;
                     }
 #pragma unroll
                     for(int u = 0; u < WCH_U; ++u)
@@ -910,14 +914,19 @@ bool wave_clock_ok(const wf_wave_config &c)
            ((uint64_t)c.meter_ms * 1000000ull) / (uint64_t)c.width != 0;
 }
 
-const void *chunk_kernel(int mode, bool disp)
+template<typename TS>
+const void *chunk_kernel_of(int mode, bool disp)
 {
     static const void *const k[2][4] = {
-        {(const void *)wave_chunk_kernel<0, WParams>, (const void *)wave_chunk_kernel<1, WParams>,
-         (const void *)wave_chunk_kernel<2, WParams>, (const void *)wave_chunk_kernel<3, WParams>},
-        {(const void *)wave_chunk_kernel<0, WDisp>, (const void *)wave_chunk_kernel<1, WDisp>,
-         (const void *)wave_chunk_kernel<2, WDisp>, (const void *)wave_chunk_kernel<3, WDisp>}};
+        {(const void *)wave_chunk_kernel<0, WParams, TS>, (const void *)wave_chunk_kernel<1, WParams, TS>,
+         (const void *)wave_chunk_kernel<2, WParams, TS>, (const void *)wave_chunk_kernel<3, WParams, TS>},
+        {(const void *)wave_chunk_kernel<0, WDisp, TS>, (const void *)wave_chunk_kernel<1, WDisp, TS>,
+         (const void *)wave_chunk_kernel<2, WDisp, TS>, (const void *)wave_chunk_kernel<3, WDisp, TS>}};
     return k[disp ? 1 : 0][mode];
+}
+const void *chunk_kernel(int mode, bool disp, bool s16)
+{
+    return s16 ? chunk_kernel_of<int16_t>(mode, disp) : chunk_kernel_of<float>(mode, disp);
 }
 
 // The tick-by-tick timestamp walk of tick_waveform (src/source_generic.cpp:303-339,358) for packets of `hop` samples that
@@ -1001,7 +1010,7 @@ int wf_wave_create(const wf_wave_config *cfg_in, wf_wave **out)
     *out = nullptr;
     return wf::create_engine(out, g_wave_create_error, wf_wave_destroy, [&](wf_wave *w) -> int {
         bool display_settings = false;
-        if(!wf::accept_struct(cfg_in, kPrevWaveConfig, w->cfg, &display_settings))
+        if(!wf::accept_struct(cfg_in, {kPrevWaveConfig}, w->cfg, &display_settings))
             return wf::fail(w, WF_ERR_ABI, "wf_wave_config.struct_size mismatch");
         const wf_wave_config *cfg = &w->cfg;
         if(cfg->capture_channels < 1 || cfg->capture_channels > 2 || cfg->max_streams < 1 || !wave_clock_ok(*cfg))
@@ -1028,9 +1037,13 @@ int wf_wave_create(const wf_wave_config *cfg_in, wf_wave **out)
             const int ring_bytes = (int)((2 * (size_t)cfg->width + w->disp_scratch) * sizeof(float));
             if(ring_bytes > 48 * 1024) // widths above 6144: both scrolling rings exceed the default 48 KB
             {
-                WF_CHECK(w, cudaFuncSetAttribute(wave_kernel<WParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * (size_t)cfg->width * sizeof(float))));
+                WF_CHECK(w, cudaFuncSetAttribute(wave_kernel<WParams, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * (size_t)cfg->width * sizeof(float))));
+                WF_CHECK(w, cudaFuncSetAttribute(wave_kernel<WParams, int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * (size_t)cfg->width * sizeof(float))));
                 if(display)
-                    WF_CHECK(w, cudaFuncSetAttribute(wave_kernel<WDisp>, cudaFuncAttributeMaxDynamicSharedMemorySize, ring_bytes));
+                {
+                    WF_CHECK(w, cudaFuncSetAttribute(wave_kernel<WDisp, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, ring_bytes));
+                    WF_CHECK(w, cudaFuncSetAttribute(wave_kernel<WDisp, int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, ring_bytes));
+                }
             }
         }
         {
@@ -1041,13 +1054,17 @@ int wf_wave_create(const wf_wave_config *cfg_in, wf_wave **out)
             w->chunk_floats = mult[w->chunk_mode] * cfg->width;
             for(int disp = 0; disp < (display ? 2 : 1); ++disp)
             {
-                const void *k = chunk_kernel(w->chunk_mode, disp != 0);
                 const int bytes = (w->chunk_floats + (disp ? w->disp_scratch : 0)) * (int)sizeof(float);
-                if(bytes > 48 * 1024)
-                    WF_CHECK(w, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
                 int per_sm = 0;
-                WF_CHECK(w, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, 256, (size_t)bytes));
-                // one resident wave: streams are equal work, a partial second wave is a tail
+                for(const bool s16 : {false, true})
+                {
+                    const void *k = chunk_kernel(w->chunk_mode, disp != 0, s16);
+                    if(bytes > 48 * 1024)
+                        WF_CHECK(w, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+                    if(!s16) // the float kernel's occupancy sizes the grid of both (one resident wave: streams are equal
+                             // work, a partial second wave is a tail)
+                        WF_CHECK(w, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, 256, (size_t)bytes));
+                }
                 (disp ? w->disp_per_sm : w->chunk_per_sm) = std::max(1, per_sm);
             }
         }
@@ -1097,9 +1114,10 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b_in, void *cuda_stre
     if(!w || !b_in)
         return WF_ERR_INVALID_ARG;
     wf::NvtxRange nvtx("wf_wave_process");
-    // the current struct or the previous one (which ends before out_points: no display outputs)
+    // the current struct, the previous one (which ends before pcm_format: float PCM) or the one before (which ends before
+    // out_points: no display outputs either)
     wf_wave_batch bv;
-    if(!wf::accept_struct(b_in, offsetof(wf_wave_batch, out_points), bv))
+    if(!wf::accept_struct(b_in, {offsetof(wf_wave_batch, pcm_format), offsetof(wf_wave_batch, out_points)}, bv))
         return wf::fail(w, WF_ERR_ABI, "wf_wave_batch.struct_size %u != %zu", b_in->struct_size, sizeof(wf_wave_batch));
     const wf_wave_batch *b = &bv;
     if(b->n_ticks < 0 || b->hop < 1)
@@ -1116,6 +1134,10 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b_in, void *cuda_stre
         return wf::fail(w, WF_ERR_INVALID_ARG, "pcm is null, or none of out / out_points / out_pixels is set");
     if(b->stream_stride < 0 || b->channel_stride < 0)
         return wf::fail(w, WF_ERR_INVALID_ARG, "negative strides are not supported");
+    size_t sample_bytes = 0;
+    if(int rc = wf::pcm_sample_bytes(w, b->pcm_format, b->pcm, &sample_bytes))
+        return rc;
+    const bool s16 = b->pcm_format == WF_PCM_S16;
     if((long long)b->n_ticks * b->hop > 0x7fffffffLL)
         return wf::fail(w, WF_ERR_INVALID_ARG, "n_ticks * hop too large for one call");
 
@@ -1166,7 +1188,7 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b_in, void *cuda_stre
     const size_t out_n = S * T * w->dch * (size_t)W;
     const size_t span = (S - 1) * (size_t)b->stream_stride + (size_t)(cc - 1) * (size_t)b->channel_stride + T * (size_t)b->hop;
     wf::Staging io(w, st, !wf::is_device_ptr(b->pcm));
-    const float *d_pcm = io.in(w->s_pcm, b->pcm, span);
+    const float *d_pcm = io.in_bytes(w->s_pcm, b->pcm, span * sample_bytes);
     const float *d_rms = io.in(w->s_rms, b->input_rms, S * T);
     float *d_out = io.out(w->s_out, b->out, out_n);
     float *d_points = io.out(w->s_points, b->out_points, out_n);
@@ -1226,12 +1248,16 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b_in, void *cuda_stre
     const size_t scratch = disp ? (size_t)w->disp_scratch * sizeof(float) : 0;
     void *args[] = {disp ? (void *)&pd : (void *)&p};
     if(w->chunked)
-        WF_CHECK(w, cudaLaunchKernel(chunk_kernel(w->chunk_mode, disp), dim3(grid), dim3(256), args,
+        WF_CHECK(w, cudaLaunchKernel(chunk_kernel(w->chunk_mode, disp, s16), dim3(grid), dim3(256), args,
                                      (size_t)w->chunk_floats * sizeof(float) + scratch, st));
+    else if(disp && s16)
+        wave_kernel<WDisp, int16_t><<<grid, 256, 2 * (size_t)W * sizeof(float) + scratch, st>>>(pd);
     else if(disp)
-        wave_kernel<WDisp><<<grid, 256, 2 * (size_t)W * sizeof(float) + scratch, st>>>(pd);
+        wave_kernel<WDisp, float><<<grid, 256, 2 * (size_t)W * sizeof(float) + scratch, st>>>(pd);
+    else if(s16)
+        wave_kernel<WParams, int16_t><<<grid, 256, 2 * (size_t)W * sizeof(float), st>>>(p);
     else
-        wave_kernel<WParams><<<grid, 256, 2 * (size_t)W * sizeof(float), st>>>(p);
+        wave_kernel<WParams, float><<<grid, 256, 2 * (size_t)W * sizeof(float), st>>>(p);
     WF_CHECK(w, cudaGetLastError());
     w->launches++;
     WF_CHECK(w, cudaEventRecord(w->ev1, st));
@@ -1268,7 +1294,7 @@ int64_t wf_wave_preview_plan(const wf_wave_config *cfg_in, int32_t n_ticks, int3
     if(!cfg_in || n_ticks < 0 || hop < 1)
         return WF_ERR_INVALID_ARG;
     wf_wave_config cfg_v;
-    if(!wf::accept_struct(cfg_in, kPrevWaveConfig, cfg_v))
+    if(!wf::accept_struct(cfg_in, {kPrevWaveConfig}, cfg_v))
         return WF_ERR_ABI;
     const wf_wave_config *cfg = &cfg_v;
     if(!wave_clock_ok(*cfg))
@@ -1297,7 +1323,7 @@ int64_t wf_wave_preview_table(const wf_wave_config *cfg_in, int which, float *ou
         return WF_ERR_INVALID_ARG;
     wf_wave_config cfg;
     bool display_settings;
-    if(!wf::accept_struct(cfg_in, kPrevWaveConfig, cfg, &display_settings))
+    if(!wf::accept_struct(cfg_in, {kPrevWaveConfig}, cfg, &display_settings))
         return WF_ERR_ABI;
     if(which != WF_TABLE_INTERP_INDICES && which != WF_TABLE_INTERP_WEIGHTS && which != WF_TABLE_GAUSS)
         return WF_ERR_INVALID_ARG;

@@ -80,6 +80,7 @@ class WfWaveBatch(C.Structure):
         ("pcm", C.c_void_p), ("stream_stride", C.c_int64), ("channel_stride", C.c_int64),
         ("input_rms", C.c_void_p), ("out", C.c_void_p), ("out_silent", C.c_void_p),
         ("out_points", C.c_void_p), ("out_pixels", C.c_void_p), ("out_min", C.c_void_p),
+        ("pcm_format", C.c_int32),
     ]
 
 
@@ -90,6 +91,7 @@ class WfMeterBatch(C.Structure):
         ("pcm", C.c_void_p), ("stream_stride", C.c_int64), ("channel_stride", C.c_int64),
         ("out_db", C.c_void_p), ("out_lin", C.c_void_p), ("out_silent", C.c_void_p),
         ("out_pixels", C.c_void_p), ("out_min", C.c_void_p),
+        ("pcm_format", C.c_int32),
     ]
 
 
@@ -132,7 +134,7 @@ class WfBatch(C.Structure):
     ]
 
 
-# wf_pcm_format: the sample type of wf_batch.pcm
+# wf_pcm_format: the sample type of wf_batch.pcm, wf_meter_batch.pcm and wf_wave_batch.pcm
 PCM_F32, PCM_S16 = 0, 1
 _PCM_FORMATS = {"f32": PCM_F32, "s16": PCM_S16}
 
@@ -642,12 +644,16 @@ class MeterEngine(_Handle):
         count = self.cfg.max_streams - first_stream if count is None else count
         self._check(self.L.wf_meter_reset(self.h, first_stream, count))
 
-    def process(self, pcm, n_ticks: int, hop: int, *, first_stream=0, seconds=1.0 / 60.0, stream=None, want_pixels=False):
+    def process(self, pcm, n_ticks: int, hop: int, *, first_stream=0, seconds=1.0 / 60.0, stream=None, want_pixels=False,
+                pcm_format="f32"):
         """pcm: [n_streams, capture_channels, >= n_ticks*hop] float32, numpy (host) or CUDA torch tensor.
         Returns dict(db, lin, silent) — or dict(rms=[S, T]) for an INPUT_RMS engine.  want_pixels adds the bar heights
         render_bars draws, pixels=[S, T, capture_channels], and min=[S, T, 2] (miny, minpos).  CUDA tensors without an
-        explicit `stream` run on torch's current stream."""
-        x = _Inputs(pcm, self.cfg.capture_channels, n_ticks * hop, "meter")
+        explicit `stream` run on torch's current stream.  pcm_format="s16": int16 samples instead (an int16 numpy array or
+        a contiguous int16 CUDA tensor), read by the kernels as v * 2**-15; the default converts any numpy array to float32
+        as it is, without scaling."""
+        fmt = _pcm_format(pcm_format)
+        x = _Inputs(pcm, self.cfg.capture_channels, n_ticks * hop, "meter", s16=fmt == PCM_S16)
         S, cc, ns, mk, f32, u8 = x.S, x.cc, x.ns, x.new, x.f32, x.u8
         feed = self.cfg.mode == METER_INPUT_RMS
         out = {"rms": mk((S, n_ticks), f32)} if feed else {
@@ -664,6 +670,7 @@ class MeterEngine(_Handle):
         b.out_lin = _ptr(out["rms"]) if feed else _ptr(out["lin"])
         b.out_silent = None if feed else _ptr(out["silent"])
         b.out_pixels, b.out_min = _ptr(out.get("pixels")), _ptr(out.get("min"))
+        b.pcm_format = fmt
         if stream is None:
             self._check(self.L.wf_meter_process(self.h, C.byref(b)))
         else:
@@ -714,13 +721,16 @@ class WaveEngine(_Handle):
         self._check(self.L.wf_wave_reset(self.h))
 
     def process(self, pcm, n_ticks: int, hop: int, *, input_rms=None, stream=None, want_db=True, want_points=False,
-                want_pixels=False):
+                want_pixels=False, pcm_format="f32"):
         """pcm: [max_streams, capture_channels, >= n_ticks*hop] float32, numpy (host) or CUDA torch tensor.
         Returns dict(out=[S, T, display_channels, width], silent=[S, T]); want_points / want_pixels add what render_curve
         computes from each tick's rows: points (interpolated + smoothed dB), pixels and min=[S, T, 2] (miny, minpos), all
         [S, T, display_channels, width].  want_db=False leaves `out` out (a display-only call).  CUDA tensors without an
-        explicit `stream` run on torch's current stream."""
-        x = _Inputs(pcm, self.cfg.capture_channels, n_ticks * hop)
+        explicit `stream` run on torch's current stream.  pcm_format="s16": int16 samples instead (an int16 numpy array or
+        a contiguous int16 CUDA tensor), read by the kernels as v * 2**-15; the default converts any numpy array to float32
+        as it is, without scaling."""
+        fmt = _pcm_format(pcm_format)
+        x = _Inputs(pcm, self.cfg.capture_channels, n_ticks * hop, s16=fmt == PCM_S16)
         S, cc, ns, mk, f32, u8 = x.S, x.cc, x.ns, x.new, x.f32, x.u8
         input_rms = x.aux(input_rms, f32)
         shape = (S, n_ticks, self.display_channels, self.cfg.width)
@@ -739,6 +749,7 @@ class WaveEngine(_Handle):
         b.pcm, b.stream_stride, b.channel_stride = _ptr(x.pcm), cc * ns, ns
         b.input_rms, b.out, b.out_silent = _ptr(input_rms), _ptr(out.get("out")), _ptr(out["silent"])
         b.out_points, b.out_pixels, b.out_min = _ptr(out.get("points")), _ptr(out.get("pixels")), _ptr(out.get("min"))
+        b.pcm_format = fmt
         if stream is None:
             self._check(self.L.wf_wave_process(self.h, C.byref(b)))
         else:
