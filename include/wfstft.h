@@ -132,6 +132,9 @@ typedef enum wf_pcm_format {
     WF_PCM_S16 = 1  /* int16_t samples; sample v stands for v * 2^-15 exactly ((float)v * 0x1p-15f) */
 } wf_pcm_format;
 
+/* wf_batch.capture_ring value of a capture-ring call ("ring" in ASCII, little-endian); every other value is a plain call. */
+#define WF_CAPTURE_RING 0x676E6972
+
 /* One call = n_streams independent sources x n_frames consecutive ticks.
  *   frame t of capture channel c of stream s = pcm[s*stream_stride + c*channel_stride + t*hop ... + fft_size)
  * i.e. what CircularBuffer::peek_front hands tick_spectrum on successive ticks (src/source_generic.cpp:55-59)
@@ -169,6 +172,22 @@ typedef struct wf_batch {
                                   recorded with jittering frame times replays exactly.  NULL: `seconds` for every tick. */
     int32_t pcm_format;        /* wf_pcm_format of pcm (0 = WF_PCM_F32).  A caller built against the previous header
                                   (struct_size = offsetof(wf_batch, pcm_format)) passes float PCM. */
+    int32_t capture_ring;      /* WF_CAPTURE_RING: pcm holds only the samples captured since the previous call, n_frames*hop per
+                                  capture channel (stream s at s*stream_stride + c*channel_stride, as the level meter reads
+                                  them), and frame t of stream s is the newest fft_size samples of
+                                  ring[first_stream + s] ++ pcm[0 .. (t+1)*hop).  The ring is the engine's copy of the last
+                                  fft_size samples of each stream slot and capture channel: zeros until first used (the
+                                  plugin's start-up zeros), ring ++ new after each ring call.  hop may change between calls;
+                                  hop >= fft_size skips samples.  The call reads no more than n_frames*hop samples per channel.
+                                  WF_PCM_S16 ring calls see the float ring rounded to int16 (lrintf(x * 32768), saturated),
+                                  which is exact for a ring filled by int16 calls.  wf_last_kernel_name() is the name of the
+                                  plain call on the same frames + " ring"; the ring advances before the spectrum kernel is
+                                  launched, so a call that fails at that launch has still advanced it.
+                                  Any other value (0 included) is a plain call.  The field occupies what was the tail padding
+                                  of the previous header's struct, so sizeof(wf_batch) is unchanged and a caller built against
+                                  that header passes the current size: a 32-bit pattern rather than a flag keeps whatever its
+                                  padding holds from reading as a ring call.  struct_size = offsetof(wf_batch, pcm_format)
+                                  makes a plain float call. */
 } wf_batch;
 
 typedef struct wf_engine wf_engine;
@@ -216,6 +235,11 @@ int wf_reset_state(wf_engine *e, int32_t first_stream, int32_t count);
 int wf_get_state(wf_engine *e, int32_t first_stream, int32_t count, float *tsmooth, float *hold_db, uint8_t *flags);
 int wf_set_state(wf_engine *e, int32_t first_stream, int32_t count, const float *tsmooth, const float *hold_db,
                  const uint8_t *flags);
+/* Checkpoint / restore / priming of the capture rings of wf_batch.capture_ring (host buffers, float samples):
+ *   samples  [count][capture_channels][fft_size]   the last fft_size samples of each stream slot, oldest first
+ * With wf_get_state / wf_set_state this is a complete checkpoint of a stream.  wf_reset_state leaves the rings alone. */
+int wf_get_ring(wf_engine *e, int32_t first_stream, int32_t count, float *samples);
+int wf_set_ring(wf_engine *e, int32_t first_stream, int32_t count, const float *samples);
 
 /* Cross-channel peak normalisation (BASELINE config 5; generalises the single-source volume normalisation of
  * src/source_generic.cpp:161-167 to a peak shared by all channels on all GPUs):

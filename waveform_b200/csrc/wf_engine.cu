@@ -62,6 +62,7 @@ struct wf_engine : HostCore {
     // per-stream state
     DevBuf<float> d_state, d_hold;
     DevBuf<unsigned char> d_flags;
+    DevBuf<float> d_ring; // [max_streams][capture_channels][N] capture rings (wf_batch.capture_ring), allocated on first use
     // staging for host-pointer batches (grown on demand)
     DevBuf<float> s_pcm, s_out_db, s_out_points, s_rms, s_peak, s_px, s_min;
     DevBuf<unsigned char> s_skip, s_silent;
@@ -69,6 +70,7 @@ struct wf_engine : HostCore {
     std::vector<float> h_gtab;
     DevBuf<float> s_scratch; // any-N kernel work buffers when N/2 complex points x 2 exceed shared memory
     DevBuf<float> s_render;  // wf_render: one dB row per group when a row does not fit in shared memory
+    DevBuf<float> s_window;  // frames of a ring call in the plain layout, in the call's sample type (counts floats, as s_pcm)
     // zero-copy verdict of the last host-pointer batch (live ticks reuse the same buffers every call)
     const void *zc_ptrs[9] = {};
     bool zc_ok = false, zc_dev = false, zc_valid = false;
@@ -137,6 +139,64 @@ static __global__ void peak_normalize_kernel(float *data, int n_streams, int n_f
         for(int k = 1 + threadIdx.x; k < row_len; k += blockDim.x)
             row[k] += gain;
     }
+}
+
+// float ring sample -> the sample type of a ring call: an int16 call sees the ring rounded to int16 (exact for a ring that
+// int16 calls or the start-up zeros filled)
+__device__ __forceinline__ float ring_sample(float x, float) { return x; }
+__device__ __forceinline__ int16_t ring_sample(float x, int16_t)
+{
+    return (int16_t)max(-32768l, min(32767l, lrintf(x * 32768.0f)));
+}
+__device__ __forceinline__ float widen_sample(float x) { return x; }
+__device__ __forceinline__ float widen_sample(int16_t v) { return (float)v * 0x1p-15f; }
+
+// Copies n bytes, 16 at a time when both ends are 16-byte aligned (the caller's layout decides), else one sample at a time.
+template<typename TS>
+__device__ __forceinline__ void copy_samples(TS *dst, const TS *src, long long n)
+{
+    if((((uintptr_t)dst | (uintptr_t)src) & 15u) == 0)
+    {
+        constexpr int V = 16 / sizeof(TS);
+        const long long nv = n / V;
+        for(long long i = threadIdx.x; i < nv; i += blockDim.x)
+            reinterpret_cast<uint4 *>(dst)[i] = __ldg(reinterpret_cast<const uint4 *>(src) + i);
+        for(long long i = nv * V + threadIdx.x; i < n; i += blockDim.x)
+            dst[i] = src[i];
+    }
+    else
+        for(long long i = threadIdx.x; i < n; i += blockDim.x)
+            dst[i] = src[i];
+}
+
+// Capture-ring splice of a ring call (wf_batch.capture_ring), one CTA per (stream, capture channel), before the spectrum
+// kernel.  With hop < N (win_cs > 0):
+//   1. window := ring[hop .. N) ++ new[0 .. T*hop) in the call's sample type: the call's frames in the plain layout, frame t
+//      at window[t*hop];
+//   2. ring := window[W - N .. W), the last N samples of ring ++ new (W = N - hop + T*hop >= N), read behind the barrier.
+// With hop >= N the frames lie wholly in the new samples and there is no window: ring := new[T*hop - N .. T*hop).
+// Either way the new samples are read at most T*hop per channel.
+template<typename TS>
+__global__ void __launch_bounds__(256) ring_splice_kernel(float *ring, TS *win, const TS *pcm, long long stream_stride,
+                                                          long long channel_stride, long long win_cs, int N, int hop, int T)
+{
+    const int s = blockIdx.x, c = blockIdx.y, cc = gridDim.y;
+    float *ring_sc = ring + ((size_t)s * cc + c) * N;
+    const TS *new_sc = pcm + (size_t)s * stream_stride + (size_t)c * channel_stride;
+    const long long L = (long long)T * hop;
+    const TS *tail = new_sc + (L - N); // the last N samples of ring ++ new, when they are all new
+    if(win_cs > 0)
+    {
+        TS *win_sc = win + ((size_t)s * cc + c) * win_cs;
+        const int keep = N - hop;
+        for(int i = threadIdx.x; i < keep; i += blockDim.x)
+            win_sc[i] = ring_sample(ring_sc[hop + i], TS{});
+        copy_samples(win_sc + keep, new_sc, L);
+        __syncthreads();
+        tail = win_sc + (keep + L - N);
+    }
+    for(int i = threadIdx.x; i < N; i += blockDim.x)
+        ring_sc[i] = widen_sample(tail[i]);
 }
 
 } // namespace wf
@@ -491,6 +551,46 @@ int init_state(wf_engine *e, int first, int count, cudaStream_t st)
     return WF_OK;
 }
 
+// Samples per (stream, capture channel) of a ring call's window, ring[hop .. N) ++ new[0 .. T*hop) = (T-1)*hop + N, rounded
+// up to 16 bytes so that the window's frames are 16-byte aligned whenever hop allows; 0 when hop >= N, where every frame
+// lies wholly in the new samples and the kernel reads them in place.
+long long ring_window(int N, int hop, int T, bool s16)
+{
+    if(hop >= N)
+        return 0;
+    const long long len = (long long)N - hop + (long long)T * hop, q = s16 ? 8 : 4;
+    return (len + q - 1) / q * q;
+}
+
+// The capture rings, allocated and zeroed (the plugin's start-up zeros, src/source.cpp:1243-1248) on first use.
+int ensure_ring(wf_engine *e, cudaStream_t st)
+{
+    if(e->d_ring.p)
+        return WF_OK;
+    const Tables &t = e->tab;
+    const size_t n = (size_t)t.cfg.max_streams * t.cfg.capture_channels * t.N;
+    if(int rc = e->d_ring.reserve(e, n))
+        return rc;
+    WF_CHECK(e, cudaMemsetAsync(e->d_ring, 0, n * sizeof(float), st));
+    return WF_OK;
+}
+
+// wf_get_ring / wf_set_ring: checks, the rings, and the stream order of the copies
+int ring_access(wf_engine *e, int32_t first, int32_t count, const void *samples)
+{
+    if(!e)
+        return WF_ERR_INVALID_ARG;
+    if(first < 0 || count < 0 || (int64_t)first + count > e->tab.cfg.max_streams)
+        return fail(e, WF_ERR_CAPACITY, "ring range out of bounds");
+    if(count > 0 && !samples)
+        return fail(e, WF_ERR_INVALID_ARG, "samples is null");
+    WF_CHECK(e, cudaSetDevice(e->device));
+    if(int rc = ensure_ring(e, e->stream))
+        return rc;
+    WF_CHECK(e, cudaStreamSynchronize(e->stream));
+    return WF_OK;
+}
+
 } // namespace
 
 extern "C" {
@@ -781,7 +881,7 @@ static int launch_route(wf_engine *e, const Route &r, const CallFacts &f, KParam
 }
 
 // pcm + `samples` samples of the batch's format (the pointer stays `const float *`, as in wf_batch and KParams)
-static const float *pcm_offset(const float *pcm, size_t samples, bool s16)
+static const float *pcm_offset(const float *pcm, long long samples, bool s16)
 {
     return reinterpret_cast<const float *>(reinterpret_cast<const char *>(pcm) + samples * (s16 ? 2 : 4));
 }
@@ -794,17 +894,29 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
     const Tables &t = e->tab;
     const int cc = t.cfg.capture_channels, dch = t.display_channels, och = t.output_channels, B = t.B;
     const size_t T = (size_t)b->n_frames;
-    const bool s16 = b->pcm_format == WF_PCM_S16;
+    const bool s16 = b->pcm_format == WF_PCM_S16, ring = b->capture_ring == WF_CAPTURE_RING;
+    const float *new_pcm = pcm_offset(pcm, (long long)s0 * b->stream_stride, s16);
     KParams kp{};
-    kp.pcm = pcm_offset(pcm, (size_t)s0 * (size_t)b->stream_stride, s16);
+    kp.pcm = new_pcm;
     kp.stream_stride = b->stream_stride;
     kp.channel_stride = b->channel_stride;
+    // A ring call runs the plain kernel on plain-layout frames: the splice's window (hop < N), or the new samples themselves
+    // with frame t at new[t*hop + hop - N] (hop >= N).  The alignment facts below are those of what the kernel reads.
+    const long long win_cs = ring ? ring_window(t.N, b->hop, b->n_frames, s16) : 0;
+    if(win_cs > 0)
+    {
+        kp.pcm = pcm_offset(e->s_window, (long long)s0 * cc * win_cs, s16);
+        kp.stream_stride = cc * win_cs;
+        kp.channel_stride = win_cs;
+    }
+    else if(ring)
+        kp.pcm = pcm_offset(new_pcm, (long long)b->hop - t.N, s16);
     kp.n_streams = count;
     kp.n_frames = b->n_frames;
     kp.hop = b->hop;
     // every frame starts at an 8-byte boundary: 2 float samples, 4 int16 samples
     const long long q = s16 ? 3 : 1;
-    kp.aligned8 = (((uintptr_t)kp.pcm & 7u) == 0) && ((b->stream_stride & q) == 0) && ((b->channel_stride & q) == 0) &&
+    kp.aligned8 = (((uintptr_t)kp.pcm & 7u) == 0) && ((kp.stream_stride & q) == 0) && ((kp.channel_stride & q) == 0) &&
                   ((b->hop & q) == 0);
     kp.input_rms = rms ? rms + (size_t)s0 * T : nullptr;
     kp.skip_mask = skip ? skip + (size_t)s0 * T : nullptr;
@@ -845,7 +957,25 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
     const CallFacts f = call_facts(kp, s16);
     Route r = choose_route(e, kp, f);
     r.s16 = s16;
-    return launch_route(e, r, f, kp, st);
+    if(ring)
+    {
+        float *ring_p = e->d_ring + slot * cc * t.N;
+        const dim3 grid((unsigned)count, (unsigned)cc);
+        if(s16)
+            ring_splice_kernel<<<grid, 256, 0, st>>>(ring_p, const_cast<int16_t *>(reinterpret_cast<const int16_t *>(kp.pcm)),
+                                                     reinterpret_cast<const int16_t *>(new_pcm), b->stream_stride,
+                                                     b->channel_stride, win_cs, t.N, b->hop, b->n_frames);
+        else
+            ring_splice_kernel<<<grid, 256, 0, st>>>(ring_p, const_cast<float *>(kp.pcm), new_pcm, b->stream_stride,
+                                                     b->channel_stride, win_cs, t.N, b->hop, b->n_frames);
+        WF_CHECK(e, cudaGetLastError());
+        e->launches++;
+    }
+    if(int rc = launch_route(e, r, f, kp, st))
+        return rc;
+    if(ring)
+        e->last_kernel += " ring";
+    return WF_OK;
 }
 
 
@@ -855,7 +985,8 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
     if(!e || !b_in)
         return WF_ERR_INVALID_ARG;
     NvtxRange nvtx("wf_process");
-    // the current struct or the previous one (which ends before pcm_format: float PCM)
+    // the current struct or the one ending before pcm_format (float PCM).  capture_ring took the previous struct's tail
+    // padding, so the previous size is the current one.
     wf_batch bv;
     if(!accept_struct(b_in, {offsetof(wf_batch, pcm_format)}, bv))
         return fail(e, WF_ERR_ABI, "wf_batch.struct_size %u != %zu", b_in->struct_size, sizeof(wf_batch));
@@ -886,6 +1017,16 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
     WF_CHECK(e, cudaSetDevice(e->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : e->stream;
     const size_t S = (size_t)b->n_streams, T = (size_t)b->n_frames;
+    const bool ring = b->capture_ring == WF_CAPTURE_RING;
+    if(ring)
+    {
+        if(int rc = ensure_ring(e, st))
+            return rc;
+        // the window of every stream of the call (chunks of a staged call take their own parts of it)
+        const size_t win = S * cc * (size_t)ring_window(N, b->hop, b->n_frames, s16) * sample_bytes;
+        if(int rc = e->s_window.reserve(e, (win + sizeof(float) - 1) / sizeof(float)))
+            return rc;
+    }
     // per-tick gravity (TVEXPONENTIAL only): evaluated on the host exactly as get_gravity(seconds) does, one pair per tick
     const float *d_gtab = nullptr;
     if(b->frame_seconds != nullptr && t.cfg.tsmoothing == WF_TSMOOTH_TVEXPONENTIAL)
@@ -947,7 +1088,9 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
     // ---- host buffers: stage through device memory, chunked over streams so that the H2D copy of chunk i+1, the
     //      kernel of chunk i and the D2H copy of chunk i-1 overlap (PCIe is full duplex; pinned memory required for
     //      real overlap, pageable memory still works but serialises) ----
-    const size_t per_stream_span = (size_t)(cc - 1) * (size_t)b->channel_stride + (T - 1) * (size_t)b->hop + (size_t)N;
+    // a ring call's stream holds only its new samples: T*hop per channel
+    const size_t per_stream_span = (size_t)(cc - 1) * (size_t)b->channel_stride +
+                                   (ring ? T * (size_t)b->hop : (T - 1) * (size_t)b->hop + (size_t)N);
     const size_t span = (S - 1) * (size_t)b->stream_stride + per_stream_span;
     // device buffer of each host buffer the batch carries (null where the batch has none)
     int rc;
@@ -1108,6 +1251,24 @@ int wf_get_state(wf_engine *e, int32_t first, int32_t count, float *tsmooth, flo
         for(int i = 0; i < count; ++i)
             flags[i] &= 1u;
     }
+    return WF_OK;
+}
+
+int wf_get_ring(wf_engine *e, int32_t first, int32_t count, float *samples)
+{
+    if(int rc = ring_access(e, first, count, samples))
+        return rc;
+    const size_t n = (size_t)e->tab.cfg.capture_channels * e->tab.N;
+    WF_CHECK(e, cudaMemcpy(samples, e->d_ring + first * n, count * n * sizeof(float), cudaMemcpyDeviceToHost));
+    return WF_OK;
+}
+
+int wf_set_ring(wf_engine *e, int32_t first, int32_t count, const float *samples)
+{
+    if(int rc = ring_access(e, first, count, samples))
+        return rc;
+    const size_t n = (size_t)e->tab.cfg.capture_channels * e->tab.N;
+    WF_CHECK(e, cudaMemcpy(e->d_ring + first * n, samples, count * n * sizeof(float), cudaMemcpyHostToDevice));
     return WF_OK;
 }
 

@@ -42,7 +42,7 @@ TABLE_WINDOW, TABLE_SLOPE, TABLE_ROLLOFF, TABLE_INTERP_INDICES, TABLE_INTERP_WEI
 EXPORTS = [
     "wf_abi_version", "wf_strerror", "wf_last_error", "wf_config_init", "wf_create", "wf_destroy", "wf_get_info",
     "wf_get_table", "wf_gravity", "wf_process", "wf_process_async", "wf_synchronize", "wf_reset_state",
-    "wf_get_state", "wf_set_state", "wf_peak_normalize", "wf_launch_count", "wf_last_kernel_ms", "wf_last_kernel_name",
+    "wf_get_state", "wf_set_state", "wf_get_ring", "wf_set_ring", "wf_peak_normalize", "wf_launch_count", "wf_last_kernel_ms", "wf_last_kernel_name",
     "wf_host_alloc", "wf_host_free", "wf_preview_table", "wf_render",
     "wf_meter_config_init", "wf_meter_create", "wf_meter_destroy", "wf_meter_last_error", "wf_meter_window",
     "wf_meter_process", "wf_meter_process_async", "wf_meter_reset", "wf_meter_launch_count", "wf_meter_last_kernel_ms",
@@ -133,9 +133,21 @@ class WfBatch(C.Structure):
         ("pcm_format", C.c_int32),
     ]
 
+    # wf_batch.capture_ring fills what was the struct's tail padding, so sizeof(wf_batch) is unchanged: it is reached as a
+    # property over those 4 bytes, and the declared fields stay those of the previous header (whose size is the same)
+    @property
+    def capture_ring(self) -> int:
+        return C.c_uint32.from_buffer(self, type(self).pcm_format.offset + 4).value
+
+    @capture_ring.setter
+    def capture_ring(self, v: int):
+        C.c_uint32.from_buffer(self, type(self).pcm_format.offset + 4).value = v
+
 
 # wf_pcm_format: the sample type of wf_batch.pcm, wf_meter_batch.pcm and wf_wave_batch.pcm
 PCM_F32, PCM_S16 = 0, 1
+# wf_batch.capture_ring of a capture-ring call (WF_CAPTURE_RING)
+CAPTURE_RING = 0x676E6972
 _PCM_FORMATS = {"f32": PCM_F32, "s16": PCM_S16}
 
 
@@ -194,6 +206,8 @@ def load_library():
     L.wf_reset_state.argtypes = [vp, C.c_int32, C.c_int32]
     L.wf_get_state.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp]
     L.wf_set_state.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp]
+    L.wf_get_ring.argtypes = [vp, C.c_int32, C.c_int32, vp]
+    L.wf_set_ring.argtypes = [vp, C.c_int32, C.c_int32, vp]
     L.wf_peak_normalize.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, C.c_float, C.c_float, vp]
     L.wf_render.argtypes = [vp, C.POINTER(WfRenderBatch), vp]
     L.wf_launch_count.restype = C.c_int64
@@ -462,9 +476,10 @@ class Engine(_Handle):
     def process_raw(self, pcm_ptr, n_streams, n_frames, hop, stream_stride, channel_stride, *, first_stream=0,
                     seconds=1.0 / 60.0, input_rms=None, skip_mask=None, out_db=None, out_points=None,
                     out_silent=None, out_peak=None, out_pixels=None, out_min=None, stream=None, sync=True,
-                    frame_seconds=None, pcm_format="f32"):
+                    frame_seconds=None, pcm_format="f32", capture_ring=False):
         """Thin wrapper over wf_process / wf_process_async with raw pointers (ints).  pcm_format: "f32" (float samples) or
-        "s16" (int16 samples, v * 2**-15); strides and hop count samples either way."""
+        "s16" (int16 samples, v * 2**-15); strides and hop count samples either way.  capture_ring: pcm holds only the
+        new samples (wf_batch.capture_ring)."""
         b = WfBatch()
         b.struct_size = C.sizeof(WfBatch)
         b.n_streams, b.n_frames, b.hop, b.first_stream = n_streams, n_frames, hop, first_stream
@@ -476,6 +491,7 @@ class Engine(_Handle):
         b.out_pixels, b.out_min = out_pixels, out_min
         b.frame_seconds = frame_seconds  # host pointer (int) or None
         b.pcm_format = _pcm_format(pcm_format)
+        b.capture_ring = CAPTURE_RING if capture_ring else 0
         if sync and stream is None:
             self._check(self.L.wf_process(self.h, C.byref(b)))
         else:
@@ -485,13 +501,15 @@ class Engine(_Handle):
 
     def process(self, pcm, n_frames: int, hop: int, *, first_stream=0, seconds=1.0 / 60.0, input_rms=None,
                 skip_mask=None, want_db=True, want_points=False, want_silent=True, want_peak=False, want_pixels=False,
-                frame_seconds=None, pcm_format="f32"):
+                frame_seconds=None, pcm_format="f32", capture_ring=False):
         """pcm: [n_streams, capture_channels, samples] float32 — numpy (host path, staged inside the C call)
         or a CUDA torch tensor (device path, outputs are CUDA tensors).  pcm_format="s16": int16 samples instead (an int16
         numpy array or contiguous int16 CUDA tensor), read by the kernels as v * 2**-15; the default converts any numpy
-        array to float32 as it is, without scaling."""
+        array to float32 as it is, without scaling.  capture_ring=True: pcm holds only the samples captured since the last
+        call, n_frames * hop per channel, and the frames reach back into each stream slot's capture ring (get_ring)."""
         s16 = _pcm_format(pcm_format) == PCM_S16
-        x = _Inputs(pcm, self.capture_channels, (n_frames - 1) * hop + self.fft_size, s16=s16)
+        need = n_frames * hop if capture_ring else (n_frames - 1) * hop + self.fft_size
+        x = _Inputs(pcm, self.capture_channels, need, s16=s16)
         S, cc, ns, mk, f32, u8 = x.S, x.cc, x.ns, x.new, x.f32, x.u8
         input_rms, skip_mask = x.aux(input_rms, f32), x.aux(skip_mask, u8)
         dch, B, P = self.display_channels, self.bins, self.num_points
@@ -519,7 +537,7 @@ class Engine(_Handle):
                          out_points=_ptr(out.get("points")), out_silent=_ptr(out.get("silent")),
                          out_peak=_ptr(out.get("peak")), out_pixels=_ptr(out.get("pixels")), out_min=_ptr(out.get("min")),
                          stream=x.stream, sync=not x.is_torch, frame_seconds=None if fs is None else fs.ctypes.data,
-                         pcm_format=pcm_format)
+                         pcm_format=pcm_format, capture_ring=capture_ring)
         return out
 
     def synchronize(self):
@@ -543,6 +561,22 @@ class Engine(_Handle):
         flags = np.ascontiguousarray(state["flags"], dtype=np.uint8) if state.get("flags") is not None else None
         count = len(ts if ts is not None else (hold if hold is not None else flags))
         self._check(self.L.wf_set_state(self.h, first_stream, count, _ptr(ts), _ptr(hold), _ptr(flags)))
+
+    def get_ring(self, first_stream=0, count=None):
+        """The capture rings of slots [first_stream, first_stream + count): float32 [count, capture_channels, fft_size],
+        oldest sample first."""
+        count = self.cfg.max_streams - first_stream if count is None else count
+        ring = np.zeros((count, self.capture_channels, self.fft_size), dtype=np.float32)
+        self._check(self.L.wf_get_ring(self.h, first_stream, count, ring.ctypes.data))
+        return ring
+
+    def set_ring(self, samples, first_stream=0):
+        """Replace the capture rings of slots [first_stream, first_stream + len(samples)) with float samples shaped
+        [count, capture_channels, fft_size], e.g. to prime a stream with the audio before a cut."""
+        ring = np.ascontiguousarray(samples, dtype=np.float32)
+        if ring.ndim != 3 or ring.shape[1:] != (self.capture_channels, self.fft_size):
+            raise ValueError(f"ring samples must be [count, {self.capture_channels}, {self.fft_size}], got {ring.shape}")
+        self._check(self.L.wf_set_ring(self.h, first_stream, ring.shape[0], ring.ctypes.data))
 
     def peak_normalize(self, data, peak, target_db: float, max_gain: float, stream=None):
         """In-place: data[s, t, ch, k>=1] += min(target_db - peak[t], max_gain).  CUDA tensors run on torch's current
