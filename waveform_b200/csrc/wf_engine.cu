@@ -63,16 +63,18 @@ struct wf_engine : HostCore {
     DevBuf<float> d_state, d_hold;
     DevBuf<unsigned char> d_flags;
     DevBuf<float> d_ring; // [max_streams][capture_channels][N] capture rings (wf_batch.capture_ring), allocated on first use
-    // staging for host-pointer batches (grown on demand)
-    DevBuf<float> s_pcm, s_out_db, s_out_points, s_rms, s_peak, s_px, s_min;
-    DevBuf<unsigned char> s_skip, s_silent;
+    // staging for host-pointer batches (grown on demand); each counts floats whatever it holds (int16 PCM, skip_mask and
+    // out_silent bytes), so that batch_bufs can name any of them
+    DevBuf<float> s_pcm, s_out_db, s_out_points, s_rms, s_skip, s_silent, s_peak, s_px, s_min;
     DevBuf<float> s_gtab; // [n_frames][2] per-tick (g, 1-g) of a TV-exponential batch with frame_seconds
     std::vector<float> h_gtab;
     DevBuf<float> s_scratch; // any-N kernel work buffers when N/2 complex points x 2 exceed shared memory
     DevBuf<float> s_render;  // wf_render: one dB row per group when a row does not fit in shared memory
     DevBuf<float> s_window;  // frames of a ring call in the plain layout, in the call's sample type (counts floats, as s_pcm)
-    // zero-copy verdict of the last host-pointer batch (live ticks reuse the same buffers every call)
-    const void *zc_ptrs[9] = {};
+    // zero-copy verdict of the last host-pointer batch (live ticks reuse the same buffers every call): pcm, then the
+    // buffers of batch_bufs
+    static constexpr int kBatchBufs = 8;
+    const void *zc_ptrs[1 + kBatchBufs] = {};
     bool zc_ok = false, zc_dev = false, zc_valid = false;
     // copy/compute pipeline for host-pointer batches
     static constexpr int kMaxChunks = 16;
@@ -886,16 +888,62 @@ static const float *pcm_offset(const float *pcm, long long samples, bool s16)
     return reinterpret_cast<const float *>(reinterpret_cast<const char *>(pcm) + samples * (s16 ? 2 : 4));
 }
 
-// Runs streams [s0, s0+count) of the batch; all pointers are DEVICE pointers already offset to stream 0 of the batch.
-static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0, int count, const float *pcm,
-                        const float *rms, const unsigned char *skip, float *out_db, float *out_points,
-                        unsigned char *silent, float *out_peak, float *px_dev, float *min_dev, const float *g_tab_dev)
+// `buf` grown to at least `bytes` bytes (the staging buffers count floats)
+static int reserve_bytes(wf_engine *e, DevBuf<float> &buf, size_t bytes)
+{
+    return buf.reserve(e, (bytes + sizeof(float) - 1) / sizeof(float));
+}
+
+// One buffer of a wf_batch other than pcm: its pointer field, which way a staged call copies it, its extent and the engine's
+// staging buffer for it.  PCM is strided rather than contiguous per stream, so it keeps its own span (wf_process_async) and
+// offset (launch_range).
+struct BatchBuf {
+    size_t field;         // offsetof(wf_batch, <pointer>)
+    bool in;              // read by the kernels (host -> device) or written by them (device -> host)
+    bool per_stream;      // `bytes` per stream of the call, or for the whole call (out_peak)
+    size_t bytes;
+    DevBuf<float> *stage;
+
+    // the batch's pointer in this field, as bytes (every data pointer of wf_batch has the same representation)
+    char *of(const wf_batch &b) const
+    {
+        char *p;
+        memcpy(&p, reinterpret_cast<const char *>(&b) + field, sizeof p);
+        return p;
+    }
+    void set(wf_batch &b, const void *p) const { memcpy(reinterpret_cast<char *>(&b) + field, &p, sizeof p); }
+};
+using BatchBufs = std::array<BatchBuf, wf_engine::kBatchBufs>;
+
+// The buffers of a call of n_frames = T, in wf_batch's order; the host path reserves, copies and offsets them from this
+// table alone.
+static BatchBufs batch_bufs(wf_engine *e, size_t T)
 {
     const Tables &t = e->tab;
-    const int cc = t.cfg.capture_channels, dch = t.display_channels, och = t.output_channels, B = t.B;
-    const size_t T = (size_t)b->n_frames;
+    const size_t f = sizeof(float), rows = T * t.display_channels;
+    return {{{offsetof(wf_batch, input_rms), true, true, T * f, &e->s_rms},
+             {offsetof(wf_batch, skip_mask), true, true, T, &e->s_skip},
+             {offsetof(wf_batch, out_db), false, true, rows * t.B * f, &e->s_out_db},
+             {offsetof(wf_batch, out_points), false, true, rows * t.num_points * f, &e->s_out_points},
+             {offsetof(wf_batch, out_silent), false, true, T, &e->s_silent},
+             {offsetof(wf_batch, out_peak), false, false, T * f, &e->s_peak},
+             {offsetof(wf_batch, out_pixels), false, true, rows * t.num_points * f, &e->s_px},
+             {offsetof(wf_batch, out_min), false, true, T * 2 * f, &e->s_min}}};
+}
+
+// Runs streams [s0, s0+count) of `b`, whose pointers the device can address: the caller's own, or the staging buffers of a
+// host batch laid out as the caller's buffers.  Every pointer is offset to stream s0 here.
+static int launch_range(wf_engine *e, const wf_batch *b, const BatchBufs &bufs, cudaStream_t st, int s0, int count,
+                        const float *g_tab_dev)
+{
+    const Tables &t = e->tab;
+    const int cc = t.cfg.capture_channels, och = t.output_channels, B = t.B;
     const bool s16 = b->pcm_format == WF_PCM_S16, ring = b->capture_ring == WF_CAPTURE_RING;
-    const float *new_pcm = pcm_offset(pcm, (long long)s0 * b->stream_stride, s16);
+    wf_batch at = *b; // b's buffers from stream s0 on
+    for(const BatchBuf &u : bufs)
+        if(char *p = u.of(*b); p && u.per_stream)
+            u.set(at, p + (size_t)s0 * u.bytes);
+    const float *new_pcm = pcm_offset(b->pcm, (long long)s0 * b->stream_stride, s16);
     KParams kp{};
     kp.pcm = new_pcm;
     kp.stream_stride = b->stream_stride;
@@ -918,8 +966,8 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
     const long long q = s16 ? 3 : 1;
     kp.aligned8 = (((uintptr_t)kp.pcm & 7u) == 0) && ((kp.stream_stride & q) == 0) && ((kp.channel_stride & q) == 0) &&
                   ((b->hop & q) == 0);
-    kp.input_rms = rms ? rms + (size_t)s0 * T : nullptr;
-    kp.skip_mask = skip ? skip + (size_t)s0 * T : nullptr;
+    kp.input_rms = at.input_rms;
+    kp.skip_mask = at.skip_mask;
     kp.window = e->d_window;
     kp.window2 = reinterpret_cast<const float2 *>(e->d_window.p);
     kp.tw = reinterpret_cast<const float2 *>(e->d_tw.p);
@@ -930,10 +978,12 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
     kp.state = e->d_state + slot * cc * B;
     kp.hold_db = e->d_hold + slot * och * B;
     kp.flags = e->d_flags + slot;
-    kp.out_db = out_db ? out_db + (size_t)s0 * T * dch * B : nullptr;
-    kp.out_points = out_points ? out_points + (size_t)s0 * T * dch * t.num_points : nullptr;
-    kp.out_silent = silent ? silent + (size_t)s0 * T : nullptr;
-    kp.out_peak = out_peak;
+    kp.out_db = at.out_db;
+    kp.out_points = at.out_points;
+    kp.out_silent = at.out_silent;
+    kp.out_peak = at.out_peak;
+    kp.out_pixels = at.out_pixels;
+    kp.out_min = at.out_min;
     kp.coef_half = (2.0f / t.window_sum) * 0.5f; // mag_coefficient/2: the split pass leaves 2*X (src/source_generic.cpp:110)
     kp.g = (t.cfg.tsmoothing == WF_TSMOOTH_NONE) ? 0.0f : gravity_for(t.cfg, b->seconds);
     kp.g2 = 1.0f - kp.g;
@@ -942,7 +992,7 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
     kp.fast_peaks = t.cfg.fast_peaks;
     kp.stereo = t.cfg.stereo;
     kp.och = och;
-    kp.dch = dch;
+    kp.dch = t.display_channels;
     kp.gate = t.cfg.silence_gate;
     kp.floor_m10 = (float)(t.cfg.floor_db - 10);
     kp.db_min = t.db_min;
@@ -951,8 +1001,6 @@ static int launch_range(wf_engine *e, const wf_batch *b, cudaStream_t st, int s0
     kp.max_gain = t.cfg.max_gain;
     kp.write_hold = 1;
     set_display_params(e, kp);
-    kp.out_pixels = b->out_pixels ? px_dev + (size_t)s0 * T * dch * t.num_points : nullptr;
-    kp.out_min = b->out_min ? min_dev + (size_t)s0 * T * 2 : nullptr;
 
     const CallFacts f = call_facts(kp, s16);
     Route r = choose_route(e, kp, f);
@@ -992,7 +1040,7 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
         return fail(e, WF_ERR_ABI, "wf_batch.struct_size %u != %zu", b_in->struct_size, sizeof(wf_batch));
     const wf_batch *b = &bv;
     const Tables &t = e->tab;
-    const int cc = t.cfg.capture_channels, dch = t.display_channels, B = t.B, N = t.N;
+    const int cc = t.cfg.capture_channels, N = t.N;
     if(b->n_streams < 0 || b->n_frames < 0 || b->hop < 1)
         return fail(e, WF_ERR_INVALID_ARG, "n_streams/n_frames must be >= 0 and hop >= 1");
     if(b->first_stream < 0 || (int64_t)b->first_stream + b->n_streams > t.cfg.max_streams)
@@ -1024,7 +1072,7 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
             return rc;
         // the window of every stream of the call (chunks of a staged call take their own parts of it)
         const size_t win = S * cc * (size_t)ring_window(N, b->hop, b->n_frames, s16) * sample_bytes;
-        if(int rc = e->s_window.reserve(e, (win + sizeof(float) - 1) / sizeof(float)))
+        if(int rc = reserve_bytes(e, e->s_window, win))
             return rc;
     }
     // per-tick gravity (TVEXPONENTIAL only): evaluated on the host exactly as get_gravity(seconds) does, one pair per tick
@@ -1043,13 +1091,15 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
         WF_CHECK(e, cudaMemcpyAsync(e->s_gtab, e->h_gtab.data(), 2 * T * sizeof(float), cudaMemcpyHostToDevice, st));
         d_gtab = e->s_gtab;
     }
+    const BatchBufs bufs = batch_bufs(e, T);
     bool dev_ptrs = false;
     {
         // Live ticks (one source, one frame: tens of KB) in page-locked, device-mapped host buffers (wf_host_alloc) skip the
         // staging copies altogether: the kernel reads the frame and writes the spectrum over PCIe itself, so a tick costs one
         // launch + one synchronisation.  Every buffer of the batch must be device-addressable for that.
-        const void *ptrs[9] = {b->pcm, b->input_rms, b->skip_mask, b->out_db, b->out_points, b->out_silent, b->out_peak, b->out_pixels,
-                               b->out_min};
+        const void *ptrs[1 + wf_engine::kBatchBufs] = {b->pcm};
+        for(int i = 0; i < wf_engine::kBatchBufs; ++i)
+            ptrs[1 + i] = bufs[i].of(*b);
         const bool small = S * T * (size_t)cc * (size_t)N * sample_bytes <= (1u << 20);
         if(e->zc_valid && memcmp(ptrs, e->zc_ptrs, sizeof(ptrs)) == 0)
             dev_ptrs = e->zc_dev || (e->zc_ok && small && e->knobs.zero_copy); // same buffers as the last call, already classified
@@ -1057,7 +1107,7 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
         {
             const int kpcm = ptr_kind(b->pcm);
             bool zc = (kpcm == 2); // every buffer device-addressable?
-            for(int i = 1; i < 9 && zc; ++i)
+            for(int i = 1; i <= wf_engine::kBatchBufs && zc; ++i)
                 zc = (ptrs[i] == nullptr) || (ptr_kind(ptrs[i]) != 0);
             memcpy(e->zc_ptrs, ptrs, sizeof(ptrs));
             e->zc_dev = (kpcm == 1);
@@ -1076,9 +1126,7 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
             if(rc)
                 return rc;
         }
-        int rc = launch_range(e, b, st, 0, b->n_streams, b->pcm, b->input_rms, b->skip_mask, b->out_db, b->out_points,
-                              b->out_silent, b->out_peak, b->out_pixels, b->out_min, d_gtab);
-        if(rc)
+        if(int rc = launch_range(e, b, bufs, st, 0, b->n_streams, d_gtab))
             return rc;
         WF_CHECK(e, cudaEventRecord(e->ev1, st));
         e->ev_valid = true;
@@ -1092,23 +1140,16 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
     const size_t per_stream_span = (size_t)(cc - 1) * (size_t)b->channel_stride +
                                    (ring ? T * (size_t)b->hop : (T - 1) * (size_t)b->hop + (size_t)N);
     const size_t span = (S - 1) * (size_t)b->stream_stride + per_stream_span;
-    // device buffer of each host buffer the batch carries (null where the batch has none)
-    int rc;
-    auto stage = [&](auto &buf, const void *host, size_t n) -> decltype(buf.p) {
-        if(!host || rc)
-            return nullptr;
-        rc = buf.reserve(e, n);
-        return buf.p;
-    };
-    rc = e->s_pcm.reserve(e, (span * sample_bytes + sizeof(float) - 1) / sizeof(float)); // s_pcm counts floats
-    float *d_out_db = stage(e->s_out_db, b->out_db, S * T * dch * B);
-    float *d_out_points = stage(e->s_out_points, b->out_points, S * T * dch * t.num_points);
-    float *d_rms = stage(e->s_rms, b->input_rms, S * T);
-    unsigned char *d_skip = stage(e->s_skip, b->skip_mask, S * T);
-    unsigned char *d_silent = stage(e->s_silent, b->out_silent, S * T);
-    float *d_peak = stage(e->s_peak, b->out_peak, T);
-    float *d_px = stage(e->s_px, b->out_pixels, S * T * dch * t.num_points);
-    float *d_min = stage(e->s_min, b->out_min, S * T * 2);
+    // the batch the kernels run on: the staging buffers in place of the caller's, null where the caller passed none
+    wf_batch staged = *b;
+    int rc = reserve_bytes(e, e->s_pcm, span * sample_bytes);
+    staged.pcm = e->s_pcm;
+    for(const BatchBuf &u : bufs)
+        if(u.of(*b) && !rc)
+        {
+            rc = reserve_bytes(e, *u.stage, u.per_stream ? S * u.bytes : u.bytes);
+            u.set(staged, u.stage->p);
+        }
     if(rc)
         return rc;
     if(!e->s_h2d)
@@ -1131,9 +1172,9 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
     WF_CHECK(e, cudaEventRecord(e->ev_fork, st));
     WF_CHECK(e, cudaStreamWaitEvent(e->s_h2d, e->ev_fork, 0));
     WF_CHECK(e, cudaStreamWaitEvent(e->s_d2h, e->ev_fork, 0));
-    if(d_peak)
+    if(staged.out_peak)
     {
-        if((rc = fill_device(e, d_peak, (long long)T, -INFINITY, st)))
+        if((rc = fill_device(e, staged.out_peak, (long long)T, -INFINITY, st)))
             return rc;
     }
     for(int c = 0; c < nchunks; ++c)
@@ -1144,41 +1185,26 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
         const size_t cspan = (size_t)(cnt - 1) * (size_t)b->stream_stride + per_stream_span;
         WF_CHECK(e, cudaMemcpyAsync(const_cast<float *>(pcm_offset(e->s_pcm, off, s16)), pcm_offset(b->pcm, off, s16),
                                    cspan * sample_bytes, cudaMemcpyHostToDevice, e->s_h2d));
-        if(d_rms)
-            WF_CHECK(e, cudaMemcpyAsync(d_rms + (size_t)s0 * T, b->input_rms + (size_t)s0 * T, (size_t)cnt * T * sizeof(float),
-                                       cudaMemcpyHostToDevice, e->s_h2d));
-        if(d_skip)
-            WF_CHECK(e, cudaMemcpyAsync(d_skip + (size_t)s0 * T, b->skip_mask + (size_t)s0 * T, (size_t)cnt * T,
-                                       cudaMemcpyHostToDevice, e->s_h2d));
+        for(const BatchBuf &u : bufs)
+            if(char *h = u.of(*b); h && u.in && u.per_stream)
+                WF_CHECK(e, cudaMemcpyAsync(u.of(staged) + s0 * u.bytes, h + s0 * u.bytes, cnt * u.bytes,
+                                           cudaMemcpyHostToDevice, e->s_h2d));
         WF_CHECK(e, cudaEventRecord(e->chunk_in[c], e->s_h2d));
         WF_CHECK(e, cudaStreamWaitEvent(st, e->chunk_in[c], 0));
-        if((rc = launch_range(e, b, st, s0, cnt, e->s_pcm, d_rms, d_skip, d_out_db, d_out_points, d_silent, d_peak, d_px,
-                              d_min, d_gtab)))
+        if((rc = launch_range(e, &staged, bufs, st, s0, cnt, d_gtab)))
             return rc;
         WF_CHECK(e, cudaEventRecord(e->chunk_k[c], st));
         WF_CHECK(e, cudaStreamWaitEvent(e->s_d2h, e->chunk_k[c], 0));
-        if(b->out_db)
-            WF_CHECK(e, cudaMemcpyAsync(b->out_db + (size_t)s0 * T * dch * B, d_out_db + (size_t)s0 * T * dch * B,
-                                       (size_t)cnt * T * dch * B * sizeof(float), cudaMemcpyDeviceToHost, e->s_d2h));
-        if(b->out_points)
-            WF_CHECK(e, cudaMemcpyAsync(b->out_points + (size_t)s0 * T * dch * t.num_points,
-                                       d_out_points + (size_t)s0 * T * dch * t.num_points,
-                                       (size_t)cnt * T * dch * t.num_points * sizeof(float), cudaMemcpyDeviceToHost, e->s_d2h));
-        if(b->out_silent)
-            WF_CHECK(e, cudaMemcpyAsync(b->out_silent + (size_t)s0 * T, d_silent + (size_t)s0 * T, (size_t)cnt * T,
-                                       cudaMemcpyDeviceToHost, e->s_d2h));
-        if(b->out_pixels)
-            WF_CHECK(e, cudaMemcpyAsync(b->out_pixels + (size_t)s0 * T * dch * t.num_points,
-                                       d_px + (size_t)s0 * T * dch * t.num_points,
-                                       (size_t)cnt * T * dch * t.num_points * sizeof(float), cudaMemcpyDeviceToHost, e->s_d2h));
-        if(b->out_min)
-            WF_CHECK(e, cudaMemcpyAsync(b->out_min + (size_t)s0 * T * 2, d_min + (size_t)s0 * T * 2,
-                                       (size_t)cnt * T * 2 * sizeof(float), cudaMemcpyDeviceToHost, e->s_d2h));
+        for(const BatchBuf &u : bufs)
+            if(char *h = u.of(*b); h && !u.in && u.per_stream)
+                WF_CHECK(e, cudaMemcpyAsync(h + s0 * u.bytes, u.of(staged) + s0 * u.bytes, cnt * u.bytes,
+                                           cudaMemcpyDeviceToHost, e->s_d2h));
     }
     WF_CHECK(e, cudaEventRecord(e->ev1, st));
     e->ev_valid = true;
-    if(b->out_peak) // complete only after the last chunk's kernel
-        WF_CHECK(e, cudaMemcpyAsync(b->out_peak, d_peak, T * sizeof(float), cudaMemcpyDeviceToHost, e->s_d2h));
+    for(const BatchBuf &u : bufs) // out_peak: complete only after the last chunk's kernel
+        if(char *h = u.of(*b); h && !u.per_stream)
+            WF_CHECK(e, cudaMemcpyAsync(h, u.of(staged), u.bytes, cudaMemcpyDeviceToHost, e->s_d2h));
     WF_CHECK(e, cudaEventRecord(e->ev_join, e->s_d2h));
     WF_CHECK(e, cudaStreamWaitEvent(st, e->ev_join, 0)); // the caller's stream completes when the results are home
     return WF_OK;
@@ -1337,27 +1363,16 @@ int wf_peak_normalize(wf_engine *e, float *data, int32_t n_streams, int32_t n_fr
     const int rows_per_frame = e->tab.display_channels;
     const size_t total = (size_t)n_streams * n_frames * rows_per_frame * row_len;
     const bool dev = is_device_ptr(data);
-    float *d_data = data;
-    const float *d_peak = peak;
-    if(!dev)
-    {
-        int rc;
-        if((rc = e->s_out_db.reserve(e, total)))
-            return rc;
-        if((rc = e->s_peak.reserve(e, (size_t)n_frames)))
-            return rc;
-        WF_CHECK(e, cudaMemcpyAsync(e->s_out_db, data, total * sizeof(float), cudaMemcpyHostToDevice, st));
-        WF_CHECK(e, cudaMemcpyAsync(e->s_peak, peak, (size_t)n_frames * sizeof(float), cudaMemcpyHostToDevice, st));
-        d_data = e->s_out_db;
-        d_peak = e->s_peak;
-    }
-    else if(!is_device_ptr(peak))
-    {
-        if(int rc = e->s_peak.reserve(e, (size_t)n_frames))
-            return rc;
-        WF_CHECK(e, cudaMemcpyAsync(e->s_peak, peak, (size_t)n_frames * sizeof(float), cudaMemcpyHostToDevice, st));
-        d_peak = e->s_peak;
-    }
+    // host rows go through the engine's staging buffers, in and out on `st`
+    Staging sg(e, st, !dev);
+    float *d_data = const_cast<float *>(sg.in(e->s_out_db, static_cast<const float *>(data), total));
+    Staging sp(e, st, !dev || !is_device_ptr(peak)); // a host peak is copied even with device rows
+    const float *d_peak = sp.in(e->s_peak, peak, (size_t)n_frames);
+    if(sp.rc)
+        return sp.rc;
+    sg.out(e->s_out_db, data, total);
+    if(sg.rc)
+        return sg.rc;
     WF_CHECK(e, cudaEventRecord(e->ev0, st));
     const long long rows = (long long)n_streams * n_frames * rows_per_frame;
     const int grid = (int)std::min<long long>(rows, (long long)e->sm_count * 16);
@@ -1367,11 +1382,11 @@ int wf_peak_normalize(wf_engine *e, float *data, int32_t n_streams, int32_t n_fr
     e->launches++;
     WF_CHECK(e, cudaEventRecord(e->ev1, st));
     e->ev_valid = true;
-    if(!dev)
-    {
-        WF_CHECK(e, cudaMemcpyAsync(data, d_data, total * sizeof(float), cudaMemcpyDeviceToHost, st));
-        WF_CHECK(e, cudaStreamSynchronize(st));
-    }
+    if(dev)
+        return WF_OK;
+    if(int rc = sg.finish())
+        return rc;
+    WF_CHECK(e, cudaStreamSynchronize(st));
     return WF_OK;
 }
 
