@@ -20,6 +20,7 @@
 #include "wf_kernels.cuh"
 #include "wf_fast2048.cuh"
 #include "wf_anyn.cuh"
+#include "wf_v3.cuh"
 #include "wf_wide.hpp"
 #include "wf_v3.hpp"
 #include "wf_team2048.hpp"
@@ -259,8 +260,8 @@ bool supported_fft_size(int n)
     return n <= 65536; // sizes whose work buffers exceed shared memory run from a global (L2) scratch
 }
 
-// What one call runs: the kernel family, its template arguments and the launch shape the host picks for it.  The shapes of
-// the parity, CTA-per-tick, wide and fused kernels follow from their template arguments.
+// What one call runs: the kernel family, its template arguments and the launch shape the host picks for it.  The rest of the
+// shape follows from the template arguments (plan_launch).
 enum class Family { fast, team, parity, warp2, v3, wide, fused, anyn };
 struct Route {
     Family family;
@@ -283,6 +284,7 @@ struct CallFacts {
     int v3_x;       // the CTA-per-tick kernel's level of options: 0, 1 (peak output only) or 3
     bool aligned16; // frames can be loaded in 16-byte units (pcm, stream stride and hop)
     bool db16;      // out_db is 16-byte aligned (the N=2048 kernels write each dB row with one bulk copy)
+    bool s16;       // int16 samples
 };
 
 // Frames start at 16-byte boundaries (TMA) when pcm does and the stream stride and hop are whole multiples of 16 bytes:
@@ -295,7 +297,8 @@ CallFacts call_facts(const KParams &kp, bool s16)
             .opts = opts_but_peak || kp.out_peak,
             .v3_x = opts_but_peak ? 3 : (kp.out_peak ? 1 : 0),
             .aligned16 = (((uintptr_t)kp.pcm & 15u) == 0) && ((kp.stream_stride & q) == 0) && ((kp.hop & q) == 0),
-            .db16 = ((uintptr_t)kp.out_db & 15u) == 0};
+            .db16 = ((uintptr_t)kp.out_db & 15u) == 0,
+            .s16 = s16};
 }
 
 // The display stage's settings (src/source.cpp:1381-1424, 1473-1565) in KParams: set here for the spectrum kernels and for
@@ -335,12 +338,10 @@ size_t display_smem(const KParams &kp, const CallFacts &f, int groups)
 
 // Cluster size of the wide kernel (wf_wide.cuh) for this launch, 1 = use the one-group-per-stream kernel.
 // The wide kernel pays off when there are too few streams to fill the GPU: R CTAs per stream work on R ticks at once.
-int pick_wide_r(const wf_engine *e, const KParams &kp, bool display)
+int pick_wide_r(const wf_engine *e, const KParams &kp, const CallFacts &f)
 {
-    const int N = e->tab.N;
-    if(!wide_supported(N) || e->knobs.wide_r == 1)
-        return 1;
-    if(wide_smem_bytes(N, kp.dch, kp.scratch_q, display) > 227 * 1024)
+    const KernelRef k = wide_kernel(e->tab.N, e->tab.cfg.capture_channels, 2, f.s16, kp, f.display);
+    if(!k.kernel || e->knobs.wide_r == 1 || k.smem > 227 * 1024)
         return 1;
     if(e->knobs.wide_r == 2 || e->knobs.wide_r == 4 || e->knobs.wide_r == 8)
         return e->knobs.wide_r;
@@ -448,9 +449,9 @@ Route choose_route(const wf_engine *e, const KParams &kp, const CallFacts &f)
         if(fit_warp2(e, kp, f.display, r))
             return r;
     }
-    if(k.v3 && e->d_tw1 != nullptr && v3_smem_bytes(N, kp.dch, kp.scratch_q, f.display, cc, 8) <= 227 * 1024)
+    if(k.v3 && e->d_tw1 != nullptr && v3_kernel(N, cc, 8, f.v3_x, f.s16, kp, f.display).smem <= 227 * 1024)
         return {.family = Family::v3, .x = f.v3_x, .r = pick_v3_r(e, kp)};
-    if(const int R = pick_wide_r(e, kp, f.display); R > 1)
+    if(const int R = pick_wide_r(e, kp, f); R > 1)
         return {.family = Family::wide, .r = R};
     if(pow2)
         return {.family = Family::fused};
@@ -461,65 +462,121 @@ Route choose_route(const wf_engine *e, const KParams &kp, const CallFacts &f)
             .smem = in_smem ? work + extra : extra, .scratch = !in_smem};
 }
 
-// last_kernel_name() of a route
-std::string route_name(const wf_engine *e, const Route &r, int n_streams)
-{
-    const int N = e->tab.N, cc = e->tab.cfg.capture_channels;
-    char buf[128];
-    switch(r.family)
-    {
-    case Family::fast:
-        snprintf(buf, sizeof buf, "stft2048_fast_kernel<%d,%d,%d,%d> grid %d x %d warps", fast::kMaxWarpsPerCta, (int)r.tsm,
-                 (int)r.gate, r.x, r.grid, r.w);
-        break;
-    case Family::team:
-        snprintf(buf, sizeof buf, "stft2048_team_kernel<%d,%d> grid %d x %d teams", r.w, r.x, r.grid, 16 / r.w);
-        break;
-    case Family::parity: snprintf(buf, sizeof buf, "stft16384_parity_kernel<%d> %d clusters of 2", r.x, n_streams); break;
-    case Family::warp2:
-        snprintf(buf, sizeof buf, "stft_warp2_kernel<%d,%d%s> N=%d grid %d x %d warps", e->warp2.L, e->warp2.P,
-                 r.display ? ",display" : "", N, r.grid, r.w);
-        break;
-    case Family::v3: snprintf(buf, sizeof buf, "stft_v3_kernel<%d,%d,%d,%d>", N, cc, r.r, r.x); break;
-    case Family::wide: snprintf(buf, sizeof buf, "stft_wide_kernel<%d,%d,%d>", N, cc, r.r); break;
-    case Family::fused: snprintf(buf, sizeof buf, "stft_fused_kernel<%d,%d>", N, cc); break;
-    case Family::anyn: snprintf(buf, sizeof buf, "stft_anyn_kernel<%d> N=%d", cc, N); break;
-    }
-    return r.s16 ? std::string(buf) + " s16" : std::string(buf);
-}
-
+// stft_fused_kernel<N, CC, TS> with its CTA size and exchange buffers; *groups := streams per CTA
 template<int N, int CC, typename TS>
-cudaError_t launch_fused(const wf_engine *e, const KParams &kp, const CallFacts &f, cudaStream_t st)
+KernelRef fused_kernel(int *groups)
 {
     using G = Geo<N>;
-    const size_t smem = (size_t)G::GROUPS * G::BUF * sizeof(float2) + display_smem(kp, f, G::GROUPS);
-    return launch_kernel(stft_fused_kernel<N, CC, TS>, e->device, (kp.n_streams + G::GROUPS - 1) / G::GROUPS, G::CTA, smem, st,
-                         {}, kp);
+    *groups = G::GROUPS;
+    return {(const void *)stft_fused_kernel<N, CC, TS>, G::CTA, (size_t)G::GROUPS * G::BUF * sizeof(float2)};
 }
 
 template<int CC, typename TS>
-cudaError_t launch_fused_n(const wf_engine *e, const KParams &kp, const CallFacts &f, cudaStream_t st)
+KernelRef fused_kernel(int N, int *groups)
 {
-    switch(e->tab.N)
+    switch(N)
     {
-    case 128: return launch_fused<128, CC, TS>(e, kp, f, st);
-    case 256: return launch_fused<256, CC, TS>(e, kp, f, st);
-    case 512: return launch_fused<512, CC, TS>(e, kp, f, st);
-    case 1024: return launch_fused<1024, CC, TS>(e, kp, f, st);
-    case 2048: return launch_fused<2048, CC, TS>(e, kp, f, st);
-    case 4096: return launch_fused<4096, CC, TS>(e, kp, f, st);
-    case 8192: return launch_fused<8192, CC, TS>(e, kp, f, st);
-    case 16384: return launch_fused<16384, CC, TS>(e, kp, f, st);
-    case 32768: return launch_fused<32768, CC, TS>(e, kp, f, st);
-    default: return cudaErrorInvalidValue;
+    case 128: return fused_kernel<128, CC, TS>(groups);
+    case 256: return fused_kernel<256, CC, TS>(groups);
+    case 512: return fused_kernel<512, CC, TS>(groups);
+    case 1024: return fused_kernel<1024, CC, TS>(groups);
+    case 2048: return fused_kernel<2048, CC, TS>(groups);
+    case 4096: return fused_kernel<4096, CC, TS>(groups);
+    case 8192: return fused_kernel<8192, CC, TS>(groups);
+    case 16384: return fused_kernel<16384, CC, TS>(groups);
+    case 32768: return fused_kernel<32768, CC, TS>(groups);
+    default: return {};
     }
 }
 
 // stft2048_fast_kernel<kMaxWarpsPerCta, TSM, GATE, EXTRA, TS>, indexed by TSM * 4 + GATE * 2 + EXTRA
 template<typename TS, int... I>
-std::array<void (*)(KParams), sizeof...(I)> fast_kernels(std::integer_sequence<int, I...>)
+std::array<const void *, sizeof...(I)> fast_kernels(std::integer_sequence<int, I...>)
 {
-    return {stft2048_fast_kernel<fast::kMaxWarpsPerCta, (I & 4) != 0, (I & 2) != 0, (I & 1) != 0, TS>...};
+    return {(const void *)stft2048_fast_kernel<fast::kMaxWarpsPerCta, (I & 4) != 0, (I & 2) != 0, (I & 1) != 0, TS>...};
+}
+
+// How a route launches: the kernel instantiation, its shape and launch mode, the argument it takes after KParams, and its
+// name (wf_last_kernel_name).
+struct Launch {
+    enum class Arg { none, tw3, any }; // after KParams: nothing, the v3 twiddles (v3::Tw3) or the any-N plan (AnyPlan)
+    const void *kernel = nullptr;
+    unsigned grid = 0, block = 0;
+    size_t smem = 0;
+    LaunchMode mode{};
+    Arg arg = Arg::none;
+    std::string name;
+};
+
+// The launch of route r for this call.  The instantiation, the shape and the name all come from the same fields of r, so the
+// name describes the kernel that runs.
+Launch plan_launch(const wf_engine *e, const Route &r, const KParams &kp, const CallFacts &f)
+{
+    using Arg = Launch::Arg;
+    const int N = e->tab.N, cc = e->tab.cfg.capture_channels;
+    const unsigned S = (unsigned)kp.n_streams;
+    Launch l;
+    KernelRef k;
+    char buf[128];
+    switch(r.family)
+    {
+    case Family::fast:
+    {
+        static const std::array kernels = {fast_kernels<float>(std::make_integer_sequence<int, 8>{}),
+                                           fast_kernels<int16_t>(std::make_integer_sequence<int, 8>{})};
+        l = {kernels[r.s16][r.tsm * 4 + r.gate * 2 + r.x], (unsigned)r.grid, r.w * 32u, (size_t)fast::smem_bytes(r.w),
+             {.pdl = true}};
+        snprintf(buf, sizeof buf, "stft2048_fast_kernel<%d,%d,%d,%d> grid %d x %d warps", fast::kMaxWarpsPerCta, (int)r.tsm,
+                 (int)r.gate, r.x, r.grid, r.w);
+        break;
+    }
+    case Family::team:
+        k = team2048_kernel(r.w, r.x, r.s16);
+        l = {k.kernel, (unsigned)r.grid, k.block, k.smem, {.pdl = true}};
+        snprintf(buf, sizeof buf, "stft2048_team_kernel<%d,%d> grid %d x %d teams", r.w, r.x, r.grid, 16 / r.w);
+        break;
+    case Family::parity:
+        k = par16384_kernel(r.x, r.s16);
+        l = {k.kernel, 2 * S, k.block, k.smem, {}, Arg::tw3};
+        snprintf(buf, sizeof buf, "stft16384_parity_kernel<%d> %d clusters of 2", r.x, kp.n_streams);
+        break;
+    case Family::warp2:
+        l = {e->warp2.kernel[r.s16][r.x][r.display], (unsigned)r.grid, r.w * 32u, r.smem, {.pdl = true}};
+        snprintf(buf, sizeof buf, "stft_warp2_kernel<%d,%d%s> N=%d grid %d x %d warps", e->warp2.L, e->warp2.P,
+                 r.display ? ",display" : "", N, r.grid, r.w);
+        break;
+    case Family::v3:
+        k = v3_kernel(N, cc, r.r, r.x, r.s16, kp, f.display);
+        l = {k.kernel, S * r.r, k.block, k.smem, {.cluster = (unsigned)r.r}, Arg::tw3};
+        snprintf(buf, sizeof buf, "stft_v3_kernel<%d,%d,%d,%d>", N, cc, r.r, r.x);
+        break;
+    case Family::wide:
+        k = wide_kernel(N, cc, r.r, r.s16, kp, f.display);
+        l = {k.kernel, S * r.r, k.block, k.smem, {.cluster = (unsigned)r.r}};
+        snprintf(buf, sizeof buf, "stft_wide_kernel<%d,%d,%d>", N, cc, r.r);
+        break;
+    case Family::fused:
+    {
+        static constexpr KernelRef (*kernels[2][2])(int, int *) = {{fused_kernel<1, float>, fused_kernel<2, float>},
+                                                                   {fused_kernel<1, int16_t>, fused_kernel<2, int16_t>}};
+        int groups = 1;
+        k = kernels[r.s16][cc - 1](N, &groups);
+        l = {k.kernel, (S + groups - 1) / groups, k.block, k.smem + display_smem(kp, f, groups)};
+        snprintf(buf, sizeof buf, "stft_fused_kernel<%d,%d>", N, cc);
+        break;
+    }
+    case Family::anyn:
+    {
+        static const void *const kernels[2][2] = {
+            {(const void *)stft_anyn_kernel<1, float>, (const void *)stft_anyn_kernel<2, float>},
+            {(const void *)stft_anyn_kernel<1, int16_t>, (const void *)stft_anyn_kernel<2, int16_t>}};
+        l = {kernels[r.s16][cc - 1], (unsigned)r.grid, kAnyThreads, r.smem, {}, Arg::any};
+        snprintf(buf, sizeof buf, "stft_anyn_kernel<%d> N=%d", cc, N);
+        break;
+    }
+    }
+    l.name = r.s16 ? std::string(buf) + " s16" : std::string(buf);
+    return l;
 }
 
 // Write out every implicit m_decibels mirror (see materialize_hold_kernel) before something other than the N=2048
@@ -681,8 +738,7 @@ int wf_create(const wf_config *cfg, wf_engine **out)
 
         const Tables &t = e->tab;
         std::vector<float> tw1, tw2, tw0; // stay empty (and d_tw1 null) for sizes without the CTA-per-tick kernel
-        if(v3_supported(t.N))
-            v3_build_twiddles(t.N, tw1, tw2, tw0);
+        v3_build_twiddles(t.N, tw1, tw2, tw0);
         for(auto [buf, v] : {std::pair{&e->d_window, &t.window}, {&e->d_slope, &t.slope}, {&e->d_rolloff, &t.rolloff},
                              {&e->d_tw, &t.tw}, {&e->d_tw_post, &t.tw_post}, {&e->d_tw1, &tw1}, {&e->d_tw2, &tw2},
                              {&e->d_tw0, &tw0}, {&e->d_interp_idx, &t.interp_indices}, {&e->d_interp_w, &t.interp_weights},
@@ -815,16 +871,15 @@ int64_t wf_preview_table(const wf_config *cfg, int which, float *out, int64_t ca
 
 // Runs a route: writes out the implicit m_decibels mirrors first unless the route is one of the N=2048 kernels (the other
 // kernels read hold_db as it is), sets the route's own KParams fields, launches, and names the kernel.
-static int launch_route(wf_engine *e, const Route &r, const CallFacts &f, KParams kp, cudaStream_t st)
+static int launch_route(wf_engine *e, const Route &r, const Launch &l, KParams kp, cudaStream_t st)
 {
-    const Tables &t = e->tab;
-    const int N = t.N, cc = t.cfg.capture_channels, dev = e->device;
     if(r.family != Family::fast && r.family != Family::team)
     {
         if(int rc = materialize_hold(e, st))
             return rc;
     }
-    cudaError_t err = cudaSuccess;
+    AnyPlan plan = e->any;
+    plan.scratch = nullptr;
     switch(r.family)
     {
     case Family::fast:
@@ -832,53 +887,32 @@ static int launch_route(wf_engine *e, const Route &r, const CallFacts &f, KParam
         kp.split = e->knobs.split ? 1 : 0;
         kp.lazy_hold = 1;
         e->hold_implicit = true;
-        if(r.family == Family::team)
-            err = team2048_launch(r.w, r.x, r.s16, kp, r.grid, st, dev);
-        else
-        {
-            static const auto kernels = fast_kernels<float>(std::make_integer_sequence<int, 8>{});
-            static const auto kernels_s16 = fast_kernels<int16_t>(std::make_integer_sequence<int, 8>{});
-            err = launch_kernel((r.s16 ? kernels_s16 : kernels)[r.tsm * 4 + r.gate * 2 + r.x], dev, r.grid, r.w * 32,
-                                fast::smem_bytes(r.w), st, {.pdl = true}, kp);
-        }
         break;
-    case Family::parity: err = par16384_launch(r.x, r.s16, kp, e->d_tw1, e->d_tw2, e->d_tw0, st, dev); break;
     case Family::warp2:
         kp.split = e->knobs.split ? 1 : 0;
         kp.disp_tab_bytes = r.disp_tab_bytes;
         kp.disp_bytes = r.disp_bytes;
-        err = e->warp2.launch[r.s16][r.x][r.display](kp, r.grid, r.w, r.smem, st, dev);
-        break;
-    case Family::v3: err = v3_launch(N, cc, r.r, r.x, r.s16, kp, e->d_tw1, e->d_tw2, e->d_tw0, st, f.display, dev); break;
-    case Family::wide: err = wide_launch(N, cc, r.r, r.s16, kp, st, f.display, dev); break;
-    case Family::fused:
-        if(r.s16)
-            err = (cc == 2) ? launch_fused_n<2, int16_t>(e, kp, f, st) : launch_fused_n<1, int16_t>(e, kp, f, st);
-        else
-            err = (cc == 2) ? launch_fused_n<2, float>(e, kp, f, st) : launch_fused_n<1, float>(e, kp, f, st);
         break;
     case Family::anyn:
-    {
-        AnyPlan plan = e->any;
-        plan.scratch = nullptr;
         if(r.scratch)
         {
             if(int rc = e->s_scratch.reserve(e, (size_t)r.grid * 2 * plan.M * 2))
                 return rc;
             plan.scratch = reinterpret_cast<float2 *>(e->s_scratch.p);
         }
-        if(r.s16)
-            err = (cc == 2) ? launch_kernel(stft_anyn_kernel<2, int16_t>, dev, r.grid, kAnyThreads, r.smem, st, {}, kp, plan)
-                            : launch_kernel(stft_anyn_kernel<1, int16_t>, dev, r.grid, kAnyThreads, r.smem, st, {}, kp, plan);
-        else
-            err = (cc == 2) ? launch_kernel(stft_anyn_kernel<2, float>, dev, r.grid, kAnyThreads, r.smem, st, {}, kp, plan)
-                            : launch_kernel(stft_anyn_kernel<1, float>, dev, r.grid, kAnyThreads, r.smem, st, {}, kp, plan);
         break;
+    default: break;
     }
-    }
-    WF_CHECK(e, err);
+    v3::Tw3 tw{reinterpret_cast<const float2 *>(e->d_tw1.p), reinterpret_cast<const float2 *>(e->d_tw2.p),
+               reinterpret_cast<const float2 *>(e->d_tw0.p)};
+    void *args[2] = {&kp, nullptr};
+    if(l.arg == Launch::Arg::tw3)
+        args[1] = &tw;
+    else if(l.arg == Launch::Arg::any)
+        args[1] = &plan;
+    WF_CHECK(e, launch_kernel(l.kernel, e->device, l.grid, l.block, l.smem, st, l.mode, args));
     e->launches++;
-    e->last_kernel = route_name(e, r, kp.n_streams);
+    e->last_kernel = l.name;
     return WF_OK;
 }
 
@@ -1005,6 +1039,7 @@ static int launch_range(wf_engine *e, const wf_batch *b, const BatchBufs &bufs, 
     const CallFacts f = call_facts(kp, s16);
     Route r = choose_route(e, kp, f);
     r.s16 = s16;
+    const Launch l = plan_launch(e, r, kp, f);
     if(ring)
     {
         float *ring_p = e->d_ring + slot * cc * t.N;
@@ -1019,7 +1054,7 @@ static int launch_range(wf_engine *e, const wf_batch *b, const BatchBufs &bufs, 
         WF_CHECK(e, cudaGetLastError());
         e->launches++;
     }
-    if(int rc = launch_route(e, r, f, kp, st))
+    if(int rc = launch_route(e, r, l, kp, st))
         return rc;
     if(ring)
         e->last_kernel += " ring";

@@ -106,6 +106,35 @@ cudaError_t opt_in_smem(const void *kernel, int device, size_t bytes)
     return err;
 }
 
+cudaError_t launch_kernel(const void *kernel, int device, unsigned grid, unsigned block, size_t smem, cudaStream_t st,
+                          LaunchMode mode, void **args)
+{
+    if(!kernel)
+        return cudaErrorInvalidDeviceFunction;
+    if(cudaError_t err = opt_in_smem(kernel, device, smem))
+        return err;
+    cudaLaunchAttribute attr[2] = {};
+    unsigned n = 0;
+    if(mode.pdl)
+    {
+        attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[n++].val.programmaticStreamSerializationAllowed = 1;
+    }
+    if(mode.cluster > 1)
+    {
+        attr[n].id = cudaLaunchAttributeClusterDimension;
+        attr[n++].val.clusterDim = {mode.cluster, 1, 1};
+    }
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(block);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cfg.attrs = attr;
+    cfg.numAttrs = n;
+    return cudaLaunchKernelExC(&cfg, kernel, args);
+}
+
 int pcm_sample_bytes(HostCore *c, int32_t format, const void *pcm, size_t *bytes)
 {
     if(format != WF_PCM_F32 && format != WF_PCM_S16)

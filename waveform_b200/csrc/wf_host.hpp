@@ -169,34 +169,29 @@ struct LaunchMode {
     unsigned cluster = 1;
 };
 
-// kernel<<<grid, block, smem, st>>>(args...) on `device` (the current one), opted in to `smem` first.
+// kernel<<<grid, block, smem, st>>>(*args[0], *args[1], ...) on `device` (the current one), opted in to `smem` first.  A
+// null kernel (no instantiation for the asked template arguments) is cudaErrorInvalidDeviceFunction.
+cudaError_t launch_kernel(const void *kernel, int device, unsigned grid, unsigned block, size_t smem, cudaStream_t st,
+                          LaunchMode mode, void **args);
+
+// The same for a typed kernel and its arguments.
 template<class... P, class... A>
 cudaError_t launch_kernel(void (*kernel)(P...), int device, unsigned grid, unsigned block, size_t smem, cudaStream_t st,
                           LaunchMode mode, A &&...args)
 {
-    if(cudaError_t err = opt_in_smem((const void *)kernel, device, smem))
-        return err;
-    cudaLaunchAttribute attr[2] = {};
-    unsigned n = 0;
-    if(mode.pdl)
-    {
-        attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[n++].val.programmaticStreamSerializationAllowed = 1;
-    }
-    if(mode.cluster > 1)
-    {
-        attr[n].id = cudaLaunchAttributeClusterDimension;
-        attr[n++].val.clusterDim = {mode.cluster, 1, 1};
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(block);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cfg.attrs = attr;
-    cfg.numAttrs = n;
-    return cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...);
+    return [&](P... a) {
+        void *argv[] = {&a...};
+        return launch_kernel((const void *)kernel, device, grid, block, smem, st, mode, argv);
+    }(std::forward<A>(args)...);
 }
+
+// One compiled instantiation of a spectrum kernel family, as the unit that compiles it hands it out: the kernel and the
+// sizes of its launch shape that follow from its template arguments.  kernel == nullptr: none is compiled for them.
+struct KernelRef {
+    const void *kernel = nullptr;
+    unsigned block = 0; // threads per CTA
+    size_t smem = 0;    // dynamic shared memory per CTA
+};
 
 // Environment knobs (A/B switches for tests and tools).  A flag that is on by default is switched off by a value starting
 // with '0'; one that is off by default is switched on by a value starting with '1'.

@@ -1,32 +1,31 @@
-// wf_team2048.cu — instantiations + launcher of stft2048_team_kernel (its own translation unit: compiles in parallel)
+// wf_team2048.cu — instantiations of stft2048_team_kernel (its own translation unit: compiles in parallel)
 #include "wf_host.hpp"
 #include "wf_team2048.cuh"
 #include "wf_team2048.hpp"
 
 namespace wf {
 
-template<int W, bool EXTRA, typename TS>
-static cudaError_t launch(const KParams &kp, int grid, cudaStream_t st, int device)
+template<int W, typename TS>
+static const void *kernel(bool extra)
 {
-    return launch_kernel(stft2048_team_kernel<W, EXTRA, TS>, device, grid, team::kWarps * 32, team::smem_bytes(), st,
-                         {.pdl = true}, kp);
+    return extra ? (const void *)stft2048_team_kernel<W, true, TS> : (const void *)stft2048_team_kernel<W, false, TS>;
 }
 
 template<typename TS>
-static cudaError_t launch_w(int W, bool extra, const KParams &kp, int grid, cudaStream_t st, int device)
+static const void *kernel_w(int W, bool extra)
 {
     switch(W)
     {
-    case 4: return extra ? launch<4, true, TS>(kp, grid, st, device) : launch<4, false, TS>(kp, grid, st, device);
-    case 8: return extra ? launch<8, true, TS>(kp, grid, st, device) : launch<8, false, TS>(kp, grid, st, device);
-    case 16: return extra ? launch<16, true, TS>(kp, grid, st, device) : launch<16, false, TS>(kp, grid, st, device);
-    default: return cudaErrorInvalidValue;
+    case 4: return kernel<4, TS>(extra);
+    case 8: return kernel<8, TS>(extra);
+    case 16: return kernel<16, TS>(extra);
+    default: return nullptr;
     }
 }
 
-cudaError_t team2048_launch(int W, bool extra, bool s16, const KParams &kp, int grid, cudaStream_t st, int device)
+KernelRef team2048_kernel(int W, bool extra, bool s16)
 {
-    return s16 ? launch_w<int16_t>(W, extra, kp, grid, st, device) : launch_w<float>(W, extra, kp, grid, st, device);
+    return {s16 ? kernel_w<int16_t>(W, extra) : kernel_w<float>(W, extra), team::kWarps * 32, team::smem_bytes()};
 }
 
 } // namespace wf

@@ -1,10 +1,10 @@
 // wf_team2048.hpp — host interface of the team-per-stream N=2048 kernel (wf_team2048.cuh)
 #pragma once
-#include <cuda_runtime.h>
+#include "wf_host.hpp"
 
 namespace wf {
-struct KParams;
-// W = warps per stream (4, 8 or 16); grid = CTAs (one per SM at most); extra = slope / fast peaks / skip mask / volume /
-// roll-off / peak output in use; s16 = int16 samples.  Launches with programmatic dependent launch.
-cudaError_t team2048_launch(int W, bool extra, bool s16, const KParams &kp, int grid, cudaStream_t st, int device);
+// stft2048_team_kernel<W, extra, int16 (s16) or float samples> and its CTA size and shared memory.  W = warps per stream (4, 8
+// or 16); extra = slope / fast peaks / skip mask / volume / roll-off / peak output in use.  It launches with programmatic
+// dependent launch, at most one CTA per SM.
+KernelRef team2048_kernel(int W, bool extra, bool s16);
 } // namespace wf

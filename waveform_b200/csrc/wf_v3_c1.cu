@@ -6,26 +6,16 @@
 
 namespace wf {
 
-cudaError_t v3_launch_c2(int N, int R, int extra, const KParams &kp, const v3::Tw3 &tw, cudaStream_t st, bool display,
-                         int device);
-cudaError_t v3_launch_s16(int N, int cc, int R, int extra, const KParams &kp, const v3::Tw3 &tw, cudaStream_t st, bool display,
-                          int device);
+template KernelRef v3_kernel<1, float>(int N, int R, int extra, const KParams &kp, bool display);
 
-bool v3_supported(int N) { return N == 1024 || N == 2048 || N == 4096 || N == 8192 || N == 16384; }
-int v3_min_cluster(int N) { return (N <= 8192) ? 1 : 2; }
-
-size_t v3_smem_bytes(int N, int dch, int n_points, bool display, int cc, int R)
+KernelRef v3_kernel(int N, int cc, int R, int extra, bool s16, const KParams &kp, bool display)
 {
-    switch(N)
-    {
-    case 1024: return v3::smem_bytes<1024>(dch, n_points, display, cc, R);
-    case 2048: return v3::smem_bytes<2048>(dch, n_points, display, cc, R);
-    case 4096: return v3::smem_bytes<4096>(dch, n_points, display, cc, R);
-    case 8192: return v3::smem_bytes<8192>(dch, n_points, display, cc, R);
-    case 16384: return v3::smem_bytes<16384>(dch, n_points, display, cc, R);
-    default: return 0;
-    }
+    if(s16)
+        return (cc == 2) ? v3_kernel<2, int16_t>(N, R, extra, kp, display) : v3_kernel<1, int16_t>(N, R, extra, kp, display);
+    return (cc == 2) ? v3_kernel<2, float>(N, R, extra, kp, display) : v3_kernel<1, float>(N, R, extra, kp, display);
 }
+
+int v3_min_cluster(int N) { return (N <= 8192) ? 1 : 2; }
 
 template<int NN>
 static void build_tw(std::vector<float> &tw1, std::vector<float> &tw2, std::vector<float> &tw0)
@@ -75,18 +65,6 @@ void v3_build_twiddles(int N, std::vector<float> &tw1, std::vector<float> &tw2, 
     case 16384: build_tw<16384>(tw1, tw2, tw0); break;
     default: tw1.clear(); tw2.clear(); tw0.clear(); break;
     }
-}
-
-cudaError_t v3_launch(int N, int cc, int R, int extra, bool s16, const KParams &kp, const float *d_tw1, const float *d_tw2,
-                      const float *d_tw0, cudaStream_t st, bool display, int device)
-{
-    v3::Tw3 tw{reinterpret_cast<const float2 *>(d_tw1), reinterpret_cast<const float2 *>(d_tw2),
-               reinterpret_cast<const float2 *>(d_tw0)};
-    if(s16)
-        return v3_launch_s16(N, cc, R, extra, kp, tw, st, display, device);
-    if(cc == 2)
-        return v3_launch_c2(N, R, extra, kp, tw, st, display, device);
-    return v3impl::launch_cc<1, float>(N, R, extra, kp, tw, st, display, device);
 }
 
 } // namespace wf

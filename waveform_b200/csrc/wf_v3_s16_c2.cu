@@ -3,10 +3,6 @@
 
 namespace wf {
 
-cudaError_t v3_launch_s16_c2(int N, int R, int extra, const KParams &kp, const v3::Tw3 &tw, cudaStream_t st, bool display,
-                             int device)
-{
-    return v3impl::launch_cc<2, int16_t>(N, R, extra, kp, tw, st, display, device);
-}
+template KernelRef v3_kernel<2, int16_t>(int N, int R, int extra, const KParams &kp, bool display);
 
 } // namespace wf

@@ -3,10 +3,11 @@
 #include <cuda_runtime.h>
 #include <stddef.h>
 
+#include "wf_host.hpp"
+
 namespace wf {
 struct KParams;
-bool wide_supported(int N);
-size_t wide_smem_bytes(int N, int dch, int n_points, bool display);
-// R = cluster size (2, 4 or 8 CTAs per stream); grid = n_streams * R; s16 = int16 samples
-cudaError_t wide_launch(int N, int cc, int R, bool s16, const KParams &kp, cudaStream_t st, bool display, int device);
+// stft_wide_kernel<N, cc, R, int16 (s16) or float samples> with its threads per CTA and its shared memory at kp's display
+// settings (dch, scratch_q); R = cluster size (2, 4 or 8 CTAs per stream)
+KernelRef wide_kernel(int N, int cc, int R, bool s16, const KParams &kp, bool display);
 } // namespace wf
