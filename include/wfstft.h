@@ -96,6 +96,12 @@ typedef struct wf_config {
     int32_t channel_spacing;   /* m_channel_spacing (get_settings zeroes it unless stereo, src/source.cpp:579-580) */
     int32_t rounded_caps;      /* m_rounded_caps (bars only) */
     int32_t min_bar_height;    /* m_min_bar_height */
+    int32_t sync_offset_ms;    /* m_ts_offset in ms, the plugin's audio sync offset (P_AUDIO_SYNC_OFFSET, src/source.cpp:556), in
+                                  [-1000, 1000] (else WF_ERR_INVALID_ARG).  An offset > 0 holds back
+                                  D = ns_to_audio_frames(sample_rate, offset * 10^6) samples, as tick_spectrum does
+                                  (src/source_generic.cpp:50-61).  Only capture-ring calls honour it (see wf_batch.capture_ring);
+                                  plain calls name their frames.  <= 0: D = 0.  A caller built against the previous header
+                                  (struct_size = offsetof(wf_config, sync_offset_ms)) gets 0. */
 } wf_config;
 
 /* Facts derived at create time. */
@@ -183,6 +189,13 @@ typedef struct wf_batch {
                                   which is exact for a ring filled by int16 calls.  wf_last_kernel_name() is the name of the
                                   plain call on the same frames + " ring"; the ring advances before the spectrum kernel is
                                   launched, so a call that fails at that launch has still advanced it.
+                                  With an audio sync offset (wf_config.sync_offset_ms, D samples > 0) the ring holds the last
+                                  fft_size + D samples and frame t is the OLDEST fft_size of the newest fft_size + D samples of
+                                  ring ++ pcm[0 .. (t+1)*hop), which is what tick_spectrum peeks (src/source_generic.cpp:50-61).
+                                  Each slot also counts the samples still owed before its first real tick: D at creation, less
+                                  every new sample, never below 0.  A tick while the count is above 0 is a "not enough audio"
+                                  tick (skip_mask semantics, ORed with the caller's skip_mask), as in the plugin while its
+                                  capture buffer holds fewer than fft_size + D samples.
                                   Any other value (0 included) is a plain call.  The field occupies what was the tail padding
                                   of the previous header's struct, so sizeof(wf_batch) is unchanged and a caller built against
                                   that header passes the current size: a 32-bit pattern rather than a flag keeps whatever its
@@ -236,8 +249,11 @@ int wf_get_state(wf_engine *e, int32_t first_stream, int32_t count, float *tsmoo
 int wf_set_state(wf_engine *e, int32_t first_stream, int32_t count, const float *tsmooth, const float *hold_db,
                  const uint8_t *flags);
 /* Checkpoint / restore / priming of the capture rings of wf_batch.capture_ring (host buffers, float samples):
- *   samples  [count][capture_channels][fft_size]   the last fft_size samples of each stream slot, oldest first
- * With wf_get_state / wf_set_state this is a complete checkpoint of a stream.  wf_reset_state leaves the rings alone. */
+ *   samples  [count][capture_channels][fft_size + D]   the last fft_size + D samples of each stream slot, oldest first
+ *                                                      (D: the sync offset's delay, wf_config.sync_offset_ms; 0 without one)
+ * With wf_get_state / wf_set_state this is a complete checkpoint of a stream.  wf_set_ring also clears the slots' counts of
+ * samples owed before their first real tick (a primed stream has its delay's worth of audio).  wf_reset_state leaves the
+ * rings and the counts alone. */
 int wf_get_ring(wf_engine *e, int32_t first_stream, int32_t count, float *samples);
 int wf_set_ring(wf_engine *e, int32_t first_stream, int32_t count, const float *samples);
 
@@ -328,6 +344,14 @@ typedef struct wf_meter_config {
     int32_t bar_width;        /* m_bar_width: cap radius = bar_width / 2 */
     int32_t rounded_caps;     /* m_rounded_caps */
     int32_t min_bar_height;   /* m_min_bar_height */
+    int32_t sync_offset_ms;   /* the plugin's audio sync offset in ms, in [-1000, 1000] (else WF_ERR_INVALID_ARG).  An offset > 0
+                                 holds back D = ns_to_audio_frames(sample_rate, offset * 10^6) samples per stream slot and capture
+                                 channel in a delay line (zeros at creation), as tick_meter / sync_rms_buffer consume everything but
+                                 the newest D samples (src/source_generic.cpp:202-222, src/source.cpp:810-835): a call consumes
+                                 (line ++ pcm)[0 .. n_ticks*hop) and the line keeps the last D samples of line ++ pcm.  That is
+                                 the engine without an offset fed zeros(D) ++ stream.  first_stream ranges apply to the lines;
+                                 wf_meter_reset leaves them alone.  <= 0: D = 0.  A config of the previous size
+                                 (struct_size = offsetof(wf_meter_config, sync_offset_ms)) gets 0. */
 } wf_meter_config;
 
 typedef struct wf_meter_batch {
@@ -384,7 +408,7 @@ float wf_meter_last_kernel_ms(wf_meter *m);
  * A wf_wave keeps, per stream, the scrolling buffer m_decibels[2][width] and m_last_silent, and per ENGINE the clock the
  * reference derives from packet timestamps (m_audio_ts, m_waveform_ts).  One call = n_streams sources x n_ticks ticks; tick t
  * is preceded by a capture packet of samples [t*hop, (t+1)*hop) of each channel whose end is stamped "now" (get_audio_sync
- * == 0).  Every stream of the engine ticks in every call (the timing state is shared).  The nearest-sample resampling is
+ * equals the configured sync offset).  Every stream of the engine ticks in every call (the timing state is shared).  The nearest-sample resampling is
  * integer arithmetic on nanosecond timestamps (bit-exact); the dBFS conversion uses log10f (last-bit differences). */
 typedef struct wf_wave_config {
     uint32_t struct_size;     /* = sizeof(wf_wave_config) */
@@ -409,6 +433,13 @@ typedef struct wf_wave_config {
     int32_t floor_db;         /* m_floor */
     int32_t ceiling_db;       /* m_ceiling */
     int32_t channel_spacing;  /* m_channel_spacing (zeroed unless stereo, src/source.cpp:579-580) */
+    int32_t sync_offset_ms;   /* the plugin's audio sync offset in ms, in [-1000, 1000] (else WF_ERR_INVALID_ARG).  An offset > 0
+                                 reserves D = ns_to_audio_frames(sample_rate, offset * 10^6) samples as tick_waveform does
+                                 (src/source_generic.cpp:290-332): a tick while no more than D samples are buffered emits nothing
+                                 and leaves the clock alone, the buffer keeps m_waveform_samples + D samples, the clock stops at
+                                 audio_ts - D and points take samples older than the newest D.  The engine carries the last D
+                                 samples of each stream and channel into the next call.  <= 0: D = 0.  A config of the previous
+                                 size (struct_size = offsetof(wf_wave_config, sync_offset_ms)) gets 0. */
 } wf_wave_config;
 
 typedef struct wf_wave_batch {
@@ -449,7 +480,8 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *batch, void *cuda_str
 int wf_wave_reset(wf_wave *w);
 /* The host-side plan of a call made right after wf_wave_create (no device needed; lets a CPU-only test check the integer
  * timestamp walk against the plugin): counts[t] = points emitted by tick t; src (optional, `capacity` entries) = for every
- * point in order the index of the sample it takes in the call's PCM, or -1 for a start-up zero.  Returns the total number of
+ * point in order the index of the sample it takes in the call's PCM, or -1 for a start-up zero (with a sync offset, also
+ * for the zeros the delay holds before the first samples).  Returns the total number of
  * points or a negative status. */
 int64_t wf_wave_preview_plan(const wf_wave_config *cfg, int32_t n_ticks, int32_t hop, int32_t *counts, int32_t *src,
                              int64_t capacity);

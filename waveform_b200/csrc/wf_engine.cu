@@ -27,6 +27,7 @@
 #include "wf_warp2.hpp"
 #include "wf_par16384.hpp"
 #include "wf_render.hpp"
+#include "wf_splice.hpp"
 #include "wf_nvtx.hpp"
 #include "wf_tables.hpp"
 #include "wfstft.h"
@@ -63,7 +64,12 @@ struct wf_engine : HostCore {
     // per-stream state
     DevBuf<float> d_state, d_hold;
     DevBuf<unsigned char> d_flags;
-    DevBuf<float> d_ring; // [max_streams][capture_channels][N] capture rings (wf_batch.capture_ring), allocated on first use
+    DevBuf<float> d_ring; // [max_streams][capture_channels][N + D] capture rings (wf_batch.capture_ring), allocated on first use
+    int D = 0;            // samples the audio sync offset holds back (wf_config.sync_offset_ms; 0 without one)
+    std::vector<long long> owed; // [max_streams] samples each ring slot still needs before its first real tick (D at creation)
+    std::vector<int> h_nskip;    // [n_streams] start-up ticks of the current ring call, uploaded to s_nskip
+    DevBuf<int> s_nskip;
+    DevBuf<unsigned char> s_mask; // [n_streams][n_frames] start-up ticks ORed with the caller's skip_mask
     // staging for host-pointer batches (grown on demand); each counts floats whatever it holds (int16 PCM, skip_mask and
     // out_silent bytes), so that batch_bufs can name any of them
     DevBuf<float> s_pcm, s_out_db, s_out_points, s_rms, s_skip, s_silent, s_peak, s_px, s_min;
@@ -144,62 +150,13 @@ static __global__ void peak_normalize_kernel(float *data, int n_streams, int n_f
     }
 }
 
-// float ring sample -> the sample type of a ring call: an int16 call sees the ring rounded to int16 (exact for a ring that
-// int16 calls or the start-up zeros filled)
-__device__ __forceinline__ float ring_sample(float x, float) { return x; }
-__device__ __forceinline__ int16_t ring_sample(float x, int16_t)
+// skip_mask of a ring call during the sync offset's start-up: mask[s][t] = (t < nskip[s]) | caller[s][t]
+static __global__ void startup_mask_kernel(unsigned char *mask, const unsigned char *caller, const int *nskip, int n_streams,
+                                           int T)
 {
-    return (int16_t)max(-32768l, min(32767l, lrintf(x * 32768.0f)));
-}
-__device__ __forceinline__ float widen_sample(float x) { return x; }
-__device__ __forceinline__ float widen_sample(int16_t v) { return (float)v * 0x1p-15f; }
-
-// Copies n bytes, 16 at a time when both ends are 16-byte aligned (the caller's layout decides), else one sample at a time.
-template<typename TS>
-__device__ __forceinline__ void copy_samples(TS *dst, const TS *src, long long n)
-{
-    if((((uintptr_t)dst | (uintptr_t)src) & 15u) == 0)
-    {
-        constexpr int V = 16 / sizeof(TS);
-        const long long nv = n / V;
-        for(long long i = threadIdx.x; i < nv; i += blockDim.x)
-            reinterpret_cast<uint4 *>(dst)[i] = __ldg(reinterpret_cast<const uint4 *>(src) + i);
-        for(long long i = nv * V + threadIdx.x; i < n; i += blockDim.x)
-            dst[i] = src[i];
-    }
-    else
-        for(long long i = threadIdx.x; i < n; i += blockDim.x)
-            dst[i] = src[i];
-}
-
-// Capture-ring splice of a ring call (wf_batch.capture_ring), one CTA per (stream, capture channel), before the spectrum
-// kernel.  With hop < N (win_cs > 0):
-//   1. window := ring[hop .. N) ++ new[0 .. T*hop) in the call's sample type: the call's frames in the plain layout, frame t
-//      at window[t*hop];
-//   2. ring := window[W - N .. W), the last N samples of ring ++ new (W = N - hop + T*hop >= N), read behind the barrier.
-// With hop >= N the frames lie wholly in the new samples and there is no window: ring := new[T*hop - N .. T*hop).
-// Either way the new samples are read at most T*hop per channel.
-template<typename TS>
-__global__ void __launch_bounds__(256) ring_splice_kernel(float *ring, TS *win, const TS *pcm, long long stream_stride,
-                                                          long long channel_stride, long long win_cs, int N, int hop, int T)
-{
-    const int s = blockIdx.x, c = blockIdx.y, cc = gridDim.y;
-    float *ring_sc = ring + ((size_t)s * cc + c) * N;
-    const TS *new_sc = pcm + (size_t)s * stream_stride + (size_t)c * channel_stride;
-    const long long L = (long long)T * hop;
-    const TS *tail = new_sc + (L - N); // the last N samples of ring ++ new, when they are all new
-    if(win_cs > 0)
-    {
-        TS *win_sc = win + ((size_t)s * cc + c) * win_cs;
-        const int keep = N - hop;
-        for(int i = threadIdx.x; i < keep; i += blockDim.x)
-            win_sc[i] = ring_sample(ring_sc[hop + i], TS{});
-        copy_samples(win_sc + keep, new_sc, L);
-        __syncthreads();
-        tail = win_sc + (keep + L - N);
-    }
-    for(int i = threadIdx.x; i < N; i += blockDim.x)
-        ring_sc[i] = widen_sample(tail[i]);
+    for(long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < (long long)n_streams * T;
+        i += (long long)gridDim.x * blockDim.x)
+        mask[i] = ((int)(i % T) < nskip[i / T]) || (caller && caller[i]);
 }
 
 } // namespace wf
@@ -610,15 +567,15 @@ int init_state(wf_engine *e, int first, int count, cudaStream_t st)
     return WF_OK;
 }
 
-// Samples per (stream, capture channel) of a ring call's window, ring[hop .. N) ++ new[0 .. T*hop) = (T-1)*hop + N, rounded
-// up to 16 bytes so that the window's frames are 16-byte aligned whenever hop allows; 0 when hop >= N, where every frame
-// lies wholly in the new samples and the kernel reads them in place.
-long long ring_window(int N, int hop, int T, bool s16)
+// A ring call's window (wf_splice.hpp) with ring length R = N + D: C[hop .. hop + (T-1)*hop + N), the call's frames in the
+// plain layout, reaching at least to R so that it holds the part of the next ring that predates the call (D > T*hop).  Its
+// length is 0 when hop >= R: every frame then lies wholly in the new samples and the kernel reads them in place.
+long long ring_window_len(int N, int D, int hop, int T)
 {
-    if(hop >= N)
+    const long long R = (long long)N + D;
+    if(hop >= R)
         return 0;
-    const long long len = (long long)N - hop + (long long)T * hop, q = s16 ? 8 : 4;
-    return (len + q - 1) / q * q;
+    return std::max((long long)(T - 1) * hop + N, R - hop);
 }
 
 // The capture rings, allocated and zeroed (the plugin's start-up zeros, src/source.cpp:1243-1248) on first use.
@@ -627,7 +584,7 @@ int ensure_ring(wf_engine *e, cudaStream_t st)
     if(e->d_ring.p)
         return WF_OK;
     const Tables &t = e->tab;
-    const size_t n = (size_t)t.cfg.max_streams * t.cfg.capture_channels * t.N;
+    const size_t n = (size_t)t.cfg.max_streams * t.cfg.capture_channels * (t.N + e->D);
     if(int rc = e->d_ring.reserve(e, n))
         return rc;
     WF_CHECK(e, cudaMemsetAsync(e->d_ring, 0, n * sizeof(float), st));
@@ -714,6 +671,7 @@ void wf_config_init(wf_config *c)
     c->channel_spacing = 0;
     c->rounded_caps = 0;
     c->min_bar_height = 0;
+    c->sync_offset_ms = 0;
 }
 
 int wf_create(const wf_config *cfg, wf_engine **out)
@@ -721,17 +679,23 @@ int wf_create(const wf_config *cfg, wf_engine **out)
     if(!cfg || !out)
         return WF_ERR_INVALID_ARG;
     *out = nullptr;
-    if(cfg->struct_size != sizeof(wf_config))
+    // the current struct or the previous one, which ends before sync_offset_ms (no offset)
+    wf_config cv;
+    if(!accept_struct(cfg, {offsetof(wf_config, sync_offset_ms)}, cv))
         return WF_ERR_ABI;
     return create_engine(out, g_create_error, wf_destroy, [&](wf_engine *e) -> int {
+        if(!sync_offset_ok(cv.sync_offset_ms))
+            return fail(e, WF_ERR_INVALID_ARG, "sync_offset_ms %d outside [-1000, 1000]", cv.sync_offset_ms);
         const char *why = nullptr;
-        int rc = build_tables(*cfg, e->tab, &why);
+        int rc = build_tables(cv, e->tab, &why);
         if(rc != WF_OK)
             return fail(e, rc, "%s", why ? why : "bad config");
         if(!supported_fft_size(e->tab.N))
             return fail(e, WF_ERR_UNSUPPORTED_FFT_SIZE, "fft_size %d unsupported", e->tab.N);
-        if((rc = open_device(e, cfg->device)))
+        if((rc = open_device(e, cv.device)))
             return rc;
+        e->D = sync_delay(e->tab.cfg.sample_rate, cv.sync_offset_ms);
+        e->owed.assign((size_t)e->tab.cfg.max_streams, e->D);
         e->warp2 = warp2_plan(e->tab.N);
         if(!is_pow2_kernel_size(e->tab.N))
             make_any_plan(e->tab.N, &e->any);
@@ -854,11 +818,17 @@ int64_t wf_preview_table(const wf_config *cfg, int which, float *out, int64_t ca
 {
     if(!cfg)
         return WF_ERR_INVALID_ARG;
-    if(cfg->struct_size != sizeof(wf_config))
+    wf_config cv;
+    if(!accept_struct(cfg, {offsetof(wf_config, sync_offset_ms)}, cv))
         return WF_ERR_ABI;
+    if(!sync_offset_ok(cv.sync_offset_ms))
+    {
+        g_create_error = "sync_offset_ms outside [-1000, 1000]";
+        return WF_ERR_INVALID_ARG;
+    }
     Tables t;
     const char *why = nullptr;
-    int rc = build_tables(*cfg, t, &why);
+    int rc = build_tables(cv, t, &why);
     if(rc != WF_OK)
     {
         g_create_error = why ? why : "bad config";
@@ -982,9 +952,11 @@ static int launch_range(wf_engine *e, const wf_batch *b, const BatchBufs &bufs, 
     kp.pcm = new_pcm;
     kp.stream_stride = b->stream_stride;
     kp.channel_stride = b->channel_stride;
-    // A ring call runs the plain kernel on plain-layout frames: the splice's window (hop < N), or the new samples themselves
-    // with frame t at new[t*hop + hop - N] (hop >= N).  The alignment facts below are those of what the kernel reads.
-    const long long win_cs = ring ? ring_window(t.N, b->hop, b->n_frames, s16) : 0;
+    // A ring call runs the plain kernel on plain-layout frames: the splice's window (hop < R), or the new samples themselves
+    // with frame t at new[t*hop + hop - R] (hop >= R), R = N + D.  The alignment facts below are those of what the kernel reads.
+    const int R = t.N + e->D;
+    const long long win_len = ring ? ring_window_len(t.N, e->D, b->hop, b->n_frames) : 0;
+    const long long win_cs = splice_stride(win_len, s16);
     if(win_cs > 0)
     {
         kp.pcm = pcm_offset(e->s_window, (long long)s0 * cc * win_cs, s16);
@@ -992,7 +964,7 @@ static int launch_range(wf_engine *e, const wf_batch *b, const BatchBufs &bufs, 
         kp.channel_stride = win_cs;
     }
     else if(ring)
-        kp.pcm = pcm_offset(new_pcm, (long long)b->hop - t.N, s16);
+        kp.pcm = pcm_offset(new_pcm, (long long)b->hop - R, s16);
     kp.n_streams = count;
     kp.n_frames = b->n_frames;
     kp.hop = b->hop;
@@ -1002,6 +974,11 @@ static int launch_range(wf_engine *e, const wf_batch *b, const BatchBufs &bufs, 
                   ((b->hop & q) == 0);
     kp.input_rms = at.input_rms;
     kp.skip_mask = at.skip_mask;
+    // a ring call during the sync offset's start-up skips through its own mask (the caller's ORed in), routed as such
+    const bool startup = ring && !e->h_nskip.empty();
+    unsigned char *startup_mask = startup ? e->s_mask + (size_t)s0 * b->n_frames : nullptr;
+    if(startup)
+        kp.skip_mask = startup_mask;
     kp.window = e->d_window;
     kp.window2 = reinterpret_cast<const float2 *>(e->d_window.p);
     kp.tw = reinterpret_cast<const float2 *>(e->d_tw.p);
@@ -1042,17 +1019,27 @@ static int launch_range(wf_engine *e, const wf_batch *b, const BatchBufs &bufs, 
     const Launch l = plan_launch(e, r, kp, f);
     if(ring)
     {
-        float *ring_p = e->d_ring + slot * cc * t.N;
-        const dim3 grid((unsigned)count, (unsigned)cc);
-        if(s16)
-            ring_splice_kernel<<<grid, 256, 0, st>>>(ring_p, const_cast<int16_t *>(reinterpret_cast<const int16_t *>(kp.pcm)),
-                                                     reinterpret_cast<const int16_t *>(new_pcm), b->stream_stride,
-                                                     b->channel_stride, win_cs, t.N, b->hop, b->n_frames);
-        else
-            ring_splice_kernel<<<grid, 256, 0, st>>>(ring_p, const_cast<float *>(kp.pcm), new_pcm, b->stream_stride,
-                                                     b->channel_stride, win_cs, t.N, b->hop, b->n_frames);
-        WF_CHECK(e, cudaGetLastError());
+        Splice sp{};
+        sp.hist = e->d_ring + slot * cc * R;
+        sp.win = win_cs > 0 ? const_cast<float *>(kp.pcm) : nullptr;
+        sp.pcm = new_pcm;
+        sp.stream_stride = b->stream_stride;
+        sp.channel_stride = b->channel_stride;
+        sp.win_cs = win_cs;
+        sp.ws = b->hop;
+        sp.wl = win_len;
+        sp.L = (long long)b->n_frames * b->hop;
+        sp.R = R;
+        WF_CHECK(e, launch_splice(sp, count, cc, s16, st));
         e->launches++;
+        if(startup)
+        {
+            const long long n = (long long)count * b->n_frames;
+            startup_mask_kernel<<<(unsigned)std::min<long long>((n + 255) / 256, 4LL * e->sm_count), 256, 0, st>>>(
+                startup_mask, at.skip_mask, e->s_nskip + s0, count, b->n_frames);
+            WF_CHECK(e, cudaGetLastError());
+            e->launches++;
+        }
     }
     if(int rc = launch_route(e, r, l, kp, st))
         return rc;
@@ -1106,9 +1093,29 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
         if(int rc = ensure_ring(e, st))
             return rc;
         // the window of every stream of the call (chunks of a staged call take their own parts of it)
-        const size_t win = S * cc * (size_t)ring_window(N, b->hop, b->n_frames, s16) * sample_bytes;
+        const size_t win = S * cc * (size_t)splice_stride(ring_window_len(N, e->D, b->hop, b->n_frames), s16) * sample_bytes;
         if(int rc = reserve_bytes(e, e->s_window, win))
             return rc;
+        // start-up ticks of slots still owed samples by the sync offset (none in steady state: no mask work then)
+        e->h_nskip.clear();
+        const long long L = (long long)T * b->hop;
+        for(size_t s = 0; s < S; ++s)
+        {
+            long long &owed = e->owed[(size_t)b->first_stream + s];
+            if(owed > 0 && e->h_nskip.empty())
+                e->h_nskip.assign(S, 0);
+            if(owed > 0) // tick t is short of audio while owed > (t+1)*hop
+                e->h_nskip[s] = (int)std::min<long long>((long long)T, (owed + b->hop - 1) / b->hop - 1);
+            owed = std::max(0LL, owed - L);
+        }
+        if(!e->h_nskip.empty())
+        {
+            if(int rc = e->s_nskip.reserve(e, S))
+                return rc;
+            if(int rc = e->s_mask.reserve(e, S * T))
+                return rc;
+            WF_CHECK(e, cudaMemcpyAsync(e->s_nskip, e->h_nskip.data(), S * sizeof(int), cudaMemcpyHostToDevice, st));
+        }
     }
     // per-tick gravity (TVEXPONENTIAL only): evaluated on the host exactly as get_gravity(seconds) does, one pair per tick
     const float *d_gtab = nullptr;
@@ -1319,7 +1326,7 @@ int wf_get_ring(wf_engine *e, int32_t first, int32_t count, float *samples)
 {
     if(int rc = ring_access(e, first, count, samples))
         return rc;
-    const size_t n = (size_t)e->tab.cfg.capture_channels * e->tab.N;
+    const size_t n = (size_t)e->tab.cfg.capture_channels * (e->tab.N + e->D);
     WF_CHECK(e, cudaMemcpy(samples, e->d_ring + first * n, count * n * sizeof(float), cudaMemcpyDeviceToHost));
     return WF_OK;
 }
@@ -1328,8 +1335,9 @@ int wf_set_ring(wf_engine *e, int32_t first, int32_t count, const float *samples
 {
     if(int rc = ring_access(e, first, count, samples))
         return rc;
-    const size_t n = (size_t)e->tab.cfg.capture_channels * e->tab.N;
+    const size_t n = (size_t)e->tab.cfg.capture_channels * (e->tab.N + e->D);
     WF_CHECK(e, cudaMemcpy(e->d_ring + first * n, samples, count * n * sizeof(float), cudaMemcpyHostToDevice));
+    std::fill(e->owed.begin() + first, e->owed.begin() + first + count, 0LL); // a primed stream has its delay's audio
     return WF_OK;
 }
 

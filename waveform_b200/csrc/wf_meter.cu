@@ -28,6 +28,7 @@
 
 #include "wf_display.cuh"
 #include "wf_host.hpp"
+#include "wf_splice.hpp"
 #include "wf_nvtx.hpp"
 #include "wf_pcm.cuh"
 #include "wf_tables.hpp"
@@ -521,6 +522,10 @@ struct wf_meter : wf::HostCore {
     bool use_fused = true; // WF_METER_FUSED=0: always the three-kernel path (A/B tests)
     wf::DevBuf<float> d_buf;
     wf::DevBuf<unsigned char> d_flags;
+    // audio sync offset: the newest D samples of each stream slot and capture channel, held back for the next call
+    int D = 0;
+    wf::DevBuf<float> d_line;   // [max_streams][cc][D], zeros at creation
+    wf::DevBuf<float> s_window; // (line ++ new) of a call, in its sample type (counts floats)
     // scratch / staging
     wf::DevBuf<float> d_partial, d_raw, s_pcm, s_db, s_lin, s_pixels, s_min;
     wf::DevBuf<unsigned char> s_silent;
@@ -562,6 +567,7 @@ void wf_meter_config_init(wf_meter_config *c)
     c->bar_width = 24;
     c->rounded_caps = 0;
     c->min_bar_height = 0;
+    c->sync_offset_ms = 0;
 }
 
 const char *wf_meter_last_error(const wf_meter *m) { return m ? m->last_error.c_str() : g_meter_create_error.c_str(); }
@@ -572,11 +578,16 @@ int wf_meter_create(const wf_meter_config *cfg_in, wf_meter **out)
         return WF_ERR_INVALID_ARG;
     *out = nullptr;
     return wf::create_engine(out, g_meter_create_error, wf_meter_destroy, [&](wf_meter *m) -> int {
-        // the current struct or the previous one, which ends before height: its display settings are absent
-        bool display_settings = false;
-        if(!wf::accept_struct(cfg_in, {offsetof(wf_meter_config, height)}, m->cfg, &display_settings))
+        // the current struct, the previous one (which ends before sync_offset_ms: no offset) or the one before (which ends
+        // before height: its display settings are absent)
+        bool current = false;
+        if(!wf::accept_struct(cfg_in, {offsetof(wf_meter_config, sync_offset_ms), offsetof(wf_meter_config, height)}, m->cfg,
+                              &current))
             return wf::fail(m, WF_ERR_ABI, "wf_meter_config.struct_size mismatch");
+        const bool display_settings = current || cfg_in->struct_size == offsetof(wf_meter_config, sync_offset_ms);
         const wf_meter_config *cfg = &m->cfg;
+        if(!wf::sync_offset_ok(cfg->sync_offset_ms))
+            return wf::fail(m, WF_ERR_INVALID_ARG, "sync_offset_ms %d outside [-1000, 1000]", cfg->sync_offset_ms);
         if(cfg->capture_channels < 1 || cfg->capture_channels > 2 || cfg->max_streams < 1 || cfg->sample_rate < 16 ||
            cfg->mode < WF_METER_PEAK || cfg->mode > WF_METER_INPUT_RMS)
             return wf::fail(m, WF_ERR_INVALID_ARG, "bad meter config");
@@ -626,6 +637,14 @@ int wf_meter_create(const wf_meter_config *cfg_in, wf_meter **out)
             return rc;
         if((rc = m->d_flags.reserve(m, S)))
             return rc;
+        m->D = wf::sync_delay(cfg->sample_rate, cfg->sync_offset_ms);
+        if(m->D > 0)
+        {
+            const size_t line_n = S * cfg->capture_channels * (size_t)m->D;
+            if((rc = m->d_line.reserve(m, line_n)))
+                return rc;
+            WF_CHECK(m, cudaMemsetAsync(m->d_line, 0, line_n * sizeof(float), m->stream));
+        }
         // ≙ update(): ring := 0 (src/source.cpp:1181), m_meter_buf := DB_MIN (:1124-1125, sic), m_last_silent := false (:1236)
         WF_CHECK(m, cudaMemsetAsync(m->d_hist[0], 0, hist_n * sizeof(float), m->stream));
         WF_CHECK(m, cudaMemsetAsync(m->d_flags, 0, S, m->stream));
@@ -718,11 +737,37 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b_in, void *cuda_s
     if(io.rc)
         return io.rc;
 
+    const size_t slot = (size_t)b->first_stream;
+    WF_CHECK(m, cudaEventRecord(m->ev0, st));
+    // with a sync offset the kernels read (line ++ new)[0 .. T*hop) and the line keeps the last D samples (wf_splice.hpp)
+    long long stream_stride = b->stream_stride, channel_stride = b->channel_stride;
+    if(m->D > 0)
+    {
+        const long long tl = (long long)T * b->hop, wl = std::max<long long>(tl, m->D), cs = wf::splice_stride(wl, s16);
+        if((rc = m->s_window.reserve(m, (S * cc * (size_t)cs * sample_bytes + 3) / 4)))
+            return rc;
+        wf::Splice sp{};
+        sp.hist = m->d_line + slot * cc * m->D;
+        sp.win = m->s_window.p;
+        sp.pcm = d_pcm;
+        sp.stream_stride = b->stream_stride;
+        sp.channel_stride = b->channel_stride;
+        sp.win_cs = cs;
+        sp.ws = 0;
+        sp.wl = wl;
+        sp.L = tl;
+        sp.R = m->D;
+        WF_CHECK(m, wf::launch_splice(sp, (int)S, cc, s16, st));
+        m->launches += 1;
+        d_pcm = m->s_window;
+        stream_stride = cc * cs;
+        channel_stride = cs;
+    }
+
     MParams p{};
     p.pcm = d_pcm;
-    p.stream_stride = b->stream_stride;
-    p.channel_stride = b->channel_stride;
-    const size_t slot = (size_t)b->first_stream;
+    p.stream_stride = stream_stride;
+    p.channel_stride = channel_stride;
     p.hist = m->d_hist[m->cur] + slot * cc * W;
     p.hist_next = m->d_hist[m->cur ^ 1] + slot * cc * W;
     p.partial = m->d_partial;
@@ -761,12 +806,11 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b_in, void *cuda_s
     p.px_hi = m->px_hi;
     p.px_cpos = m->px_cpos;
 
-    WF_CHECK(m, cudaEventRecord(m->ev0, st));
     constexpr int kWarps = 8;
     // 4-sample group loads (128-bit for float, 64-bit for int16) need rows aligned to 4 samples (W is a multiple of 16
     // samples already).  The facts are stated in samples, so an int16 call takes the float call's path and summation order.
-    const int vec4 = (((uintptr_t)d_pcm & (4 * sample_bytes - 1)) == 0) && ((b->stream_stride & 3) == 0) &&
-                     ((b->channel_stride & 3) == 0);
+    const int vec4 = (((uintptr_t)d_pcm & (4 * sample_bytes - 1)) == 0) && ((stream_stride & 3) == 0) &&
+                     ((channel_stride & 3) == 0);
     // one-pass path: the window is a whole number of hops (meter_fused_kernel)
     const size_t fused_smem = ((size_t)pc * ((size_t)(W / b->hop) + T) + T * pc) * sizeof(float);
     const bool fused = m->use_fused && vec4 && (W % b->hop) == 0 && (b->hop % 4) == 0 && fused_smem <= 96 * 1024;

@@ -1,0 +1,76 @@
+// wf_splice.cu — history ++ new splice of wf_splice.hpp, shared by the spectrum, level-meter and waveform engines.
+#include "wf_splice.hpp"
+
+namespace wf {
+namespace {
+
+// float history sample -> the sample type of the call: an int16 call sees the history rounded to int16 (exact for a
+// history that int16 calls or the start-up zeros filled)
+__device__ __forceinline__ float history_sample(float x, float) { return x; }
+__device__ __forceinline__ int16_t history_sample(float x, int16_t)
+{
+    return (int16_t)max(-32768l, min(32767l, lrintf(x * 32768.0f)));
+}
+__device__ __forceinline__ float widen_sample(float x) { return x; }
+__device__ __forceinline__ float widen_sample(int16_t v) { return (float)v * 0x1p-15f; }
+
+// Copies n samples, 16 bytes at a time when both ends are 16-byte aligned (the caller's layout decides), else one sample at
+// a time.
+template<typename TS>
+__device__ __forceinline__ void copy_samples(TS *dst, const TS *src, long long n)
+{
+    if((((uintptr_t)dst | (uintptr_t)src) & 15u) == 0)
+    {
+        constexpr int V = 16 / sizeof(TS);
+        const long long nv = n / V;
+        for(long long i = threadIdx.x; i < nv; i += blockDim.x)
+            reinterpret_cast<uint4 *>(dst)[i] = __ldg(reinterpret_cast<const uint4 *>(src) + i);
+        for(long long i = nv * V + threadIdx.x; i < n; i += blockDim.x)
+            dst[i] = src[i];
+    }
+    else
+        for(long long i = threadIdx.x; i < n; i += blockDim.x)
+            dst[i] = src[i];
+}
+
+// One CTA per (stream, channel):
+//   1. window := C[ws .. ws + wl): the history part (converted to the call's type), then the new part;
+//   2. history := C[L .. L + R), read behind the barrier from the window where it covers them, else from the new samples.
+// The new samples are read at most twice (window, then the history's tail beyond the window) and never beyond L.
+template<typename TS>
+__global__ void __launch_bounds__(256) history_splice_kernel(const Splice p)
+{
+    const int s = blockIdx.x, c = blockIdx.y, cc = gridDim.y, R = p.R;
+    float *hist = p.hist + ((size_t)s * cc + c) * R;
+    const TS *nw = static_cast<const TS *>(p.pcm) + s * p.stream_stride + c * p.channel_stride;
+    TS *win = nullptr;
+    if(p.win)
+    {
+        win = static_cast<TS *>(p.win) + ((size_t)s * cc + c) * p.win_cs;
+        const long long hw = max(0ll, min(p.wl, (long long)R - p.ws)); // window samples taken from the history
+        for(long long i = threadIdx.x; i < hw; i += blockDim.x)
+            win[i] = history_sample(hist[p.ws + i], TS{});
+        copy_samples(win + hw, nw + (p.ws + hw - R), p.wl - hw);
+        __syncthreads();
+    }
+    const long long wend = win ? p.ws + p.wl : 0;
+    for(int i = threadIdx.x; i < R; i += blockDim.x)
+    {
+        const long long j = p.L + i;
+        hist[i] = (j < wend) ? widen_sample(win[j - p.ws]) : widen_sample(nw[j - R]);
+    }
+}
+
+} // namespace
+
+cudaError_t launch_splice(const Splice &s, int streams, int cc, bool s16, cudaStream_t st)
+{
+    const dim3 grid((unsigned)streams, (unsigned)cc);
+    if(s16)
+        history_splice_kernel<int16_t><<<grid, 256, 0, st>>>(s);
+    else
+        history_splice_kernel<float><<<grid, 256, 0, st>>>(s);
+    return cudaGetLastError();
+}
+
+} // namespace wf

@@ -60,7 +60,7 @@ class WfMeterConfig(C.Structure):
         ("capture_channels", C.c_int32), ("mode", C.c_int32), ("meter_ms", C.c_int32), ("tsmoothing", C.c_int32),
         ("gravity", C.c_float), ("fast_peaks", C.c_int32), ("floor_db", C.c_int32),
         ("height", C.c_int32), ("ceiling_db", C.c_int32), ("bar_width", C.c_int32), ("rounded_caps", C.c_int32),
-        ("min_bar_height", C.c_int32),
+        ("min_bar_height", C.c_int32), ("sync_offset_ms", C.c_int32),
     ]
 
 
@@ -70,7 +70,7 @@ class WfWaveConfig(C.Structure):
         ("capture_channels", C.c_int32), ("stereo", C.c_int32), ("width", C.c_int32), ("meter_ms", C.c_int32),
         ("normalize_volume", C.c_int32), ("volume_target", C.c_float), ("max_gain", C.c_float),
         ("interp_mode", C.c_int32), ("filter_mode", C.c_int32), ("filter_radius", C.c_float), ("height", C.c_int32),
-        ("floor_db", C.c_int32), ("ceiling_db", C.c_int32), ("channel_spacing", C.c_int32),
+        ("floor_db", C.c_int32), ("ceiling_db", C.c_int32), ("channel_spacing", C.c_int32), ("sync_offset_ms", C.c_int32),
     ]
 
 
@@ -110,6 +110,7 @@ class WfConfig(C.Structure):
         ("log_scale", C.c_int32), ("mirror_freq_axis", C.c_int32),
         ("interp_mode", C.c_int32), ("filter_mode", C.c_int32), ("filter_radius", C.c_float),
         ("height", C.c_int32), ("channel_spacing", C.c_int32), ("rounded_caps", C.c_int32), ("min_bar_height", C.c_int32),
+        ("sync_offset_ms", C.c_int32),
     ]
 
 
@@ -275,7 +276,7 @@ def make_config(settings: dict | None = None, sample_rate: int = 48000, channels
         "width": "width", "bar_width": "bar_width", "bar_gap": "bar_gap", "log_scale": "log_scale",
         "mirror_freq_axis": "mirror_freq_axis", "filter_radius": "filter_radius", "silence_gate": "silence_gate",
         "height": "height", "channel_spacing": "channel_spacing", "rounded_caps": "rounded_caps",
-        "min_bar_height": "min_bar_height",
+        "min_bar_height": "min_bar_height", "audio_sync_offset": "sync_offset_ms",
     }
     enums = {"window": ("window", WINDOWS), "interp_mode": ("interp_mode", INTERPS),
              "filter_mode": ("filter_mode", FILTERS), "temporal_smoothing": ("tsmoothing", TSMOOTH),
@@ -290,8 +291,8 @@ def make_config(settings: dict | None = None, sample_rate: int = 48000, channels
             if v not in table:
                 raise ValueError(f"{k}={v!r} is not a spectrum-mode value")
             setattr(c, field, table[v])
-        elif k in ("auto_fft_size", "audio_sync_offset"):
-            pass  # display / capture plumbing that stays on the host side of the seam
+        elif k == "auto_fft_size":
+            pass  # display plumbing that stays on the host side of the seam
         else:
             raise KeyError(f"setting {k!r} is outside the spectrum hot path")
     return c
@@ -562,20 +563,28 @@ class Engine(_Handle):
         count = len(ts if ts is not None else (hold if hold is not None else flags))
         self._check(self.L.wf_set_state(self.h, first_stream, count, _ptr(ts), _ptr(hold), _ptr(flags)))
 
+    @property
+    def sync_delay(self) -> int:
+        """Samples the audio sync offset holds back: ns_to_audio_frames(sample_rate, offset) for an offset > 0, else 0."""
+        ms = self.cfg.sync_offset_ms if self.cfg.struct_size == C.sizeof(WfConfig) else 0  # the previous size has none
+        return self.cfg.sample_rate * ms // 1000 if ms > 0 else 0
+
     def get_ring(self, first_stream=0, count=None):
-        """The capture rings of slots [first_stream, first_stream + count): float32 [count, capture_channels, fft_size],
-        oldest sample first."""
+        """The capture rings of slots [first_stream, first_stream + count): float32
+        [count, capture_channels, fft_size + sync_delay], oldest sample first."""
         count = self.cfg.max_streams - first_stream if count is None else count
-        ring = np.zeros((count, self.capture_channels, self.fft_size), dtype=np.float32)
+        ring = np.zeros((count, self.capture_channels, self.fft_size + self.sync_delay), dtype=np.float32)
         self._check(self.L.wf_get_ring(self.h, first_stream, count, ring.ctypes.data))
         return ring
 
     def set_ring(self, samples, first_stream=0):
         """Replace the capture rings of slots [first_stream, first_stream + len(samples)) with float samples shaped
-        [count, capture_channels, fft_size], e.g. to prime a stream with the audio before a cut."""
+        [count, capture_channels, fft_size + sync_delay], e.g. to prime a stream with the audio before a cut.  The slots
+        then owe no start-up samples to the sync offset."""
         ring = np.ascontiguousarray(samples, dtype=np.float32)
-        if ring.ndim != 3 or ring.shape[1:] != (self.capture_channels, self.fft_size):
-            raise ValueError(f"ring samples must be [count, {self.capture_channels}, {self.fft_size}], got {ring.shape}")
+        R = self.fft_size + self.sync_delay
+        if ring.ndim != 3 or ring.shape[1:] != (self.capture_channels, R):
+            raise ValueError(f"ring samples must be [count, {self.capture_channels}, {R}], got {ring.shape}")
         self._check(self.L.wf_set_ring(self.h, first_stream, ring.shape[0], ring.ctypes.data))
 
     def peak_normalize(self, data, peak, target_db: float, max_gain: float, stream=None):
@@ -659,6 +668,7 @@ def make_meter_config(settings: dict | None = None, sample_rate: int = 48000, ch
     c.bar_width = int(s.pop("bar_width", 24))
     c.rounded_caps = int(bool(s.pop("rounded_caps", False)))
     c.min_bar_height = int(s.pop("min_bar_height", 0))
+    c.sync_offset_ms = int(s.pop("audio_sync_offset", 0))
     if s:
         raise KeyError(f"unsupported meter settings: {sorted(s)}")
     return c
@@ -736,6 +746,7 @@ def make_wave_config(settings: dict | None = None, sample_rate: int = 48000, cha
     c.floor_db = int(s.pop("floor", -65))
     c.ceiling_db = int(s.pop("ceiling", 0))
     c.channel_spacing = int(s.pop("channel_spacing", 0))
+    c.sync_offset_ms = int(s.pop("audio_sync_offset", 0))
     if s:
         raise KeyError(f"unsupported waveform settings: {sorted(s)}")
     return c
