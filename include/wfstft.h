@@ -23,6 +23,32 @@
  *     Small batches in device-mapped pinned memory (wf_host_alloc) are processed in place, without copies (live ticks).
  *   - the engine owns all device memory (tables, per-stream EMA state, staging); the caller owns pcm/out.
  *   - there is no CPU fallback: without a CUDA device wf_create fails with WF_ERR_NO_DEVICE.
+ *
+ * CUDA graphs
+ *   - wf_process_async (plain and capture-ring calls, float or int16 PCM, with or without a sync offset, frame_seconds or
+ *     display outputs), wf_render, wf_peak_normalize and wf_meter_process_async (every mode, both kernel paths, subsets of
+ *     the streams) may be enqueued on a stream that is being captured (cudaStreamBeginCapture, torch.cuda.graph), in any
+ *     capture mode, on a fresh engine without a warm-up call.  Each replay then does what the same eager call would do at
+ *     that point, bit for bit: the state that calls carry forward (EMA state, capture rings and their start-up counts,
+ *     meter rings and their block partials) lives on the device and is read and advanced by the kernels.  Replays and eager
+ *     calls may be interleaved on one engine.
+ *   - Pointers: device memory or page-locked host memory the device can address (wf_host_alloc).  Under capture, a pageable
+ *     host buffer is WF_ERR_INVALID_ARG (wf_last_error says why); nothing is enqueued and the capture stays valid.  The
+ *     graph keeps the pointers it was captured with: write new samples into the same buffers before each replay.
+ *     wf_batch.frame_seconds is read during the captured call; its replays apply the gains of those seconds.
+ *   - Lifetime: after an engine has had a call captured it frees no buffer until it is destroyed (a later, larger call
+ *     allocates new ones and keeps the old).  Destroying an engine invalidates every graph that captured one of its calls.
+ *     Each captured spectrum call with frame_seconds (TV-exponential smoothing) also keeps 8 bytes per tick of page-locked
+ *     and of device memory for its gains until the engine is destroyed, even if its graph is destroyed first: an engine
+ *     that is captured again and again accumulates them.
+ *     Replays and other calls on one engine must be stream-ordered, as two eager calls on different streams must be.
+ *   - Buffers a captured call first needs are allocated during the capture, outside the graph (relaxed capture mode);
+ *     the capture rings are zeroed then, on the engine's own stream.
+ *   - A captured call records no timing events: wf_*last_kernel_ms returns < 0 until the next eager call.  Replays are not
+ *     counted by wf_*launch_count.
+ *   - wf_wave_process_async is not capturable: its tick plan is walked on the host from the engine's clock at every call.
+ *     On a capturing stream it returns WF_ERR_INVALID_ARG with that reason and changes nothing (no clock advance, no plan
+ *     slot used); the capture stays valid.
  */
 #ifndef WFSTFT_H
 #define WFSTFT_H
@@ -307,7 +333,8 @@ int64_t wf_launch_count(const wf_engine *e);
  * next call on this engine.  bench.py reports it as roofline.kernel, the tests assert the routing with it. */
 const char *wf_last_kernel_name(const wf_engine *e);
 /* Device time (ms) of the kernel section of the most recent wf_process / wf_process_async / wf_peak_normalize / wf_render
- * call, measured with CUDA events on the launching stream; < 0 if none. Synchronises on the recorded events. */
+ * call, measured with CUDA events on the launching stream; < 0 if none or if that call was captured into a CUDA graph.
+ * Synchronises on the recorded events. */
 float wf_last_kernel_ms(wf_engine *e);
 
 

@@ -21,6 +21,10 @@ HostCore::~HostCore()
         cudaEventDestroy(ev0);
     if(ev1)
         cudaEventDestroy(ev1);
+    for(void *p : kept)
+        cudaFree(p);
+    for(void *p : kept_host)
+        cudaFreeHost(p);
     if(stream)
         cudaStreamDestroy(stream);
 }
@@ -154,6 +158,59 @@ float last_kernel_ms(HostCore *c)
     if(cudaEventElapsedTime(&ms, c->ev0, c->ev1) != cudaSuccess)
         return -1.0f;
     return ms;
+}
+
+cudaError_t begin_call(HostCore *c, cudaStream_t st)
+{
+    cudaStreamCaptureStatus status = cudaStreamCaptureStatusNone;
+    const cudaError_t err = cudaStreamIsCapturing(st, &status);
+    c->capturing = err == cudaSuccess && status == cudaStreamCaptureStatusActive;
+    c->captured = c->captured || c->capturing;
+    return err;
+}
+
+cudaError_t time_begin(HostCore *c, cudaStream_t st)
+{
+    c->ev_valid = false;
+    return c->capturing ? cudaSuccess : cudaEventRecord(c->ev0, st);
+}
+
+cudaError_t time_end(HostCore *c, cudaStream_t st)
+{
+    if(c->capturing)
+        return cudaSuccess;
+    const cudaError_t err = cudaEventRecord(c->ev1, st);
+    c->ev_valid = err == cudaSuccess;
+    return err;
+}
+
+cudaError_t device_alloc(HostCore *c, void **p, size_t bytes)
+{
+    return outside_capture(c, [&] { return cudaMalloc(p, bytes); });
+}
+
+int keep_upload(HostCore *c, const void *src, size_t bytes, cudaStream_t st, void **dev)
+{
+    void *h = nullptr, *d = nullptr;
+    WF_CHECK(c, outside_capture(c, [&] { return cudaHostAlloc(&h, bytes, cudaHostAllocDefault); }));
+    c->kept_host.push_back(h);
+    WF_CHECK(c, device_alloc(c, &d, bytes));
+    c->kept.push_back(d);
+    memcpy(h, src, bytes);
+    WF_CHECK(c, cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, st));
+    *dev = d;
+    return WF_OK;
+}
+
+int refuse_pageable(HostCore *c, std::initializer_list<const void *> ptrs)
+{
+    if(!c->capturing)
+        return WF_OK;
+    for(const void *p : ptrs)
+        if(p && ptr_kind(p) == 0)
+            return fail(c, WF_ERR_INVALID_ARG, "a call captured into a CUDA graph needs device or page-locked host buffers "
+                                               "(wf_host_alloc); a pageable host buffer cannot be replayed");
+    return WF_OK;
 }
 
 } // namespace wf

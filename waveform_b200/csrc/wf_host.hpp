@@ -21,8 +21,8 @@
 namespace wf {
 
 // What every engine owns besides its tables and kernels; the engine structs derive from it.  The destructor releases the
-// stream and the events: the engines' *_destroy synchronise the stream before the handle goes, so nothing is freed while a
-// kernel may still use it.
+// stream, the events and the buffers kept for captured graphs: the engines' *_destroy synchronise the stream before the
+// handle goes, so nothing is freed while a kernel may still use it.
 struct HostCore {
     int device = 0, sm_count = 0;
     cudaStream_t stream = nullptr;            // the engine's own stream (calls without a caller stream)
@@ -30,6 +30,11 @@ struct HostCore {
     bool ev_valid = false;
     int64_t launches = 0;
     std::string last_error;
+    // CUDA graphs: `capturing` while a call is enqueued on a stream that is being captured (begin_call); `captured` once any
+    // call was.  From then on no device buffer is freed before the engine goes, since a graph may still point at it: a
+    // growing DevBuf leaves its old allocation in `kept`, and a captured call's own inputs (keep_upload) stay there too.
+    bool capturing = false, captured = false;
+    std::vector<void *> kept, kept_host;
 
     HostCore() = default;
     HostCore(const HostCore &) = delete;
@@ -83,11 +88,48 @@ inline bool is_device_ptr(const void *p) { return p && ptr_kind(p) == 1; }
 // p[0, n) := v on `st` (fill_kernel); counts as one launch of the engine.
 int fill_device(HostCore *c, float *p, long long n, float v, cudaStream_t st);
 
-// Milliseconds between the events around the last call's kernels, -1 before the first call or when the events fail.
+// Milliseconds between the events around the last call's kernels, -1 before the first call, after a captured call or when
+// the events fail.
 float last_kernel_ms(HostCore *c);
 
+// Starts a call on `st`: sets c->capturing from cudaStreamIsCapturing (and c->captured with it).
+cudaError_t begin_call(HostCore *c, cudaStream_t st);
+
+// The timing events around a call's kernels (ev0 before, ev1 after).  A captured call records none: its replays are not
+// timed, and last_kernel_ms stays < 0 until an eager call.
+cudaError_t time_begin(HostCore *c, cudaStream_t st);
+cudaError_t time_end(HostCore *c, cudaStream_t st);
+
+// cudaMalloc, also while c's call is being captured: cudaMalloc is not stream-ordered, so it runs under the thread's
+// relaxed capture mode and the capture (global mode included) stays valid.
+cudaError_t device_alloc(HostCore *c, void **p, size_t bytes);
+
+// Runs `f` (CUDA calls outside the captured work: allocation, a one-time initialisation on the engine's own stream) under
+// the relaxed capture mode while c's call is being captured, else as it is.
+template<class F>
+cudaError_t outside_capture(HostCore *c, F &&f)
+{
+    if(!c->capturing)
+        return f();
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    if(cudaError_t err = cudaThreadExchangeStreamCaptureMode(&mode))
+        return err;
+    const cudaError_t err = f();
+    cudaThreadExchangeStreamCaptureMode(&mode);
+    return err;
+}
+
+// `bytes` of `src` (host) into fresh device memory on `st`, through fresh page-locked host memory; *dev := the copy.  Both
+// stay until the engine goes, so that a captured call's replays read the values it was captured with whatever later calls do.
+int keep_upload(HostCore *c, const void *src, size_t bytes, cudaStream_t st, void **dev);
+
+// WF_ERR_INVALID_ARG while c's call is being captured and one of `ptrs` (nulls aside) is pageable host memory, which a graph
+// cannot copy: the call then enqueues nothing and the capture stays valid.
+int refuse_pageable(HostCore *c, std::initializer_list<const void *> ptrs);
+
 // A device buffer that only grows: reserve(n) keeps the allocation when it holds n elements already, else frees it and
-// allocates exactly n (the contents are not kept).  Freed with its owner.
+// allocates exactly n (the contents are not kept).  Freed with its owner.  Once the owner has had a call captured, the old
+// allocation goes to HostCore::kept instead of being freed (a graph may still use it).
 template<class T>
 struct DevBuf {
     T *p = nullptr;
@@ -112,11 +154,13 @@ struct DevBuf {
     {
         if(n <= cap)
             return WF_OK;
-        if(p)
+        if(p && c->captured)
+            c->kept.push_back(p);
+        else if(p)
             cudaFree(p);
         p = nullptr;
         cap = 0;
-        WF_CHECK(c, cudaMalloc((void **)&p, n * sizeof(T)));
+        WF_CHECK(c, device_alloc(c, (void **)&p, n * sizeof(T)));
         cap = n;
         return WF_OK;
     }

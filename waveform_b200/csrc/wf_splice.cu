@@ -34,6 +34,7 @@ __device__ __forceinline__ void copy_samples(TS *dst, const TS *src, long long n
 }
 
 // One CTA per (stream, channel):
+//   0. with owed (channel 0's CTA): the stream's skip_mask of the call, then its owed count less L;
 //   1. window := C[ws .. ws + wl): the history part (converted to the call's type), then the new part;
 //   2. history := C[L .. L + R), read behind the barrier from the window where it covers them, else from the new samples.
 // The new samples are read at most twice (window, then the history's tail beyond the window) and never beyond L.
@@ -41,6 +42,18 @@ template<typename TS>
 __global__ void __launch_bounds__(256) history_splice_kernel(const Splice p)
 {
     const int s = blockIdx.x, c = blockIdx.y, cc = gridDim.y, R = p.R;
+    if(p.owed && c == 0)
+    {
+        const long long owed = p.owed[s];
+        // tick t is short of audio while owed > (t+1)*hop
+        const long long nskip = owed > 0 ? min((long long)p.T, (owed + p.hop - 1) / p.hop - 1) : 0;
+        const size_t row = (size_t)s * p.T;
+        for(int t = threadIdx.x; t < p.T; t += blockDim.x)
+            p.mask[row + t] = (t < nskip) || (p.caller && p.caller[row + t]);
+        __syncthreads();
+        if(threadIdx.x == 0)
+            p.owed[s] = max(0ll, owed - p.L);
+    }
     float *hist = p.hist + ((size_t)s * cc + c) * R;
     const TS *nw = static_cast<const TS *>(p.pcm) + s * p.stream_stride + c * p.channel_stride;
     TS *win = nullptr;

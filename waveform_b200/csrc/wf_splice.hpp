@@ -26,6 +26,13 @@ struct Splice {
                                              // keeps and that predates the call lies in the window)
     long long L;                             // new samples per (stream, channel)
     int R;                                   // history length (>= 1)
+    // A spectrum ring call whose slots may still owe samples to the sync offset (else owed is null): the call's skip_mask
+    // is written here from the device-side counts, which then drop by L, so that a replayed graph skips each slot's start-up
+    // ticks exactly once, as the same sequence of eager calls does.
+    long long *owed;                         // [streams] samples each slot still needs before its first real tick
+    unsigned char *mask;                     // [streams][T] := (t < start-up ticks of the slot) | caller[s][t]
+    const unsigned char *caller;             // [streams][T] the caller's skip_mask, or null
+    int T, hop;                              // ticks of the call, samples between ticks
 };
 
 // One CTA per (stream, channel) of `streams` x `cc`.  Returns the launch's error.

@@ -1172,6 +1172,13 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b_in, void *cuda_stre
 
     WF_CHECK(w, cudaSetDevice(w->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : w->stream;
+    // The tick plan and its chunks are a host walk of the nanosecond clock (plan_ticks): a replay would repeat this call's
+    // plan instead of advancing the clock.  Refused before anything is enqueued or advanced; the capture stays valid.
+    cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+    WF_CHECK(w, cudaStreamIsCapturing(st, &capture));
+    if(capture != cudaStreamCaptureStatusNone)
+        return wf::fail(w, WF_ERR_INVALID_ARG, "the waveform engine cannot be captured into a CUDA graph: its tick plan is "
+                                               "walked on the host from the engine's clock at every call");
     const int cc = w->cfg.capture_channels, W = w->cfg.width;
     const size_t S = (size_t)b->n_streams, T = (size_t)b->n_ticks;
     std::vector<int> src, off;
