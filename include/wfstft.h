@@ -46,9 +46,13 @@
  *     the capture rings are zeroed then, on the engine's own stream.
  *   - A captured call records no timing events: wf_*last_kernel_ms returns < 0 until the next eager call.  Replays are not
  *     counted by wf_*launch_count.
- *   - wf_wave_process_async is not capturable: its tick plan is walked on the host from the engine's clock at every call.
- *     On a capturing stream it returns WF_ERR_INVALID_ARG with that reason and changes nothing (no clock advance, no plan
- *     slot used); the capture stays valid.
+ *   - wf_wave_process_async is capturable on an engine created by wf_wave_create_with_clock with device_clock = 1, under
+ *     the rules above: its clock (clock, audio and waveform timestamps, buffered samples) lives on the device, and the
+ *     call's first kernel walks the tick plan from it and advances it.  Such an engine reserves plan space for
+ *     n_ticks * width points (4 bytes each) per call shape, and refuses a call with n_ticks * width > 2^31 - 1.  On any
+ *     other engine the tick plan is walked on the host from the engine's clock at every call, so on a capturing stream the
+ *     call returns WF_ERR_INVALID_ARG with that reason and changes nothing (no clock advance, no plan slot used); the
+ *     capture stays valid.
  */
 #ifndef WFSTFT_H
 #define WFSTFT_H
@@ -498,6 +502,14 @@ typedef struct wf_wave wf_wave;
 
 void wf_wave_config_init(wf_wave_config *cfg); /* plugin defaults: width 800, 150 ms (src/source.cpp:119-174) */
 int wf_wave_create(const wf_wave_config *cfg, wf_wave **out); /* ≙ WAVSource::update in waveform mode */
+/* wf_wave_create with the place of the engine's clock and tick plan chosen for its lifetime.  device_clock 0: on the host,
+ * exactly wf_wave_create (every call walks the plan on the host and uploads it; wf_wave_process_async refuses capture).
+ * 1: on the device: each call makes one more launch (the plan kernel, which walks the plan from the clock and advances it)
+ * and may be captured into a CUDA graph; it reserves plan space for n_ticks * width points (4 bytes each), whatever the
+ * clock, so a call with n_ticks * width > 2^31 - 1 is WF_ERR_INVALID_ARG there (a host-clock engine takes it).  Otherwise
+ * the outputs are the same either way.  Any other device_clock is WF_ERR_INVALID_ARG, checked with the config's own
+ * limits, before the device. */
+int wf_wave_create_with_clock(const wf_wave_config *cfg, int32_t device_clock, wf_wave **out);
 void wf_wave_destroy(wf_wave *w);
 const char *wf_wave_last_error(const wf_wave *w);
 int wf_wave_process(wf_wave *w, const wf_wave_batch *batch);

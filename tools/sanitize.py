@@ -75,6 +75,20 @@ for chunk in ("1", "0"):
         torch.cuda.synchronize()
         print("wave display", chunk, st["width"], ch, hop, "ok", float(b["min"][..., 0].mean()), flush=True)
 os.environ.pop("WF_WAVE_CHUNK")
+# device-clock waveform engine: the plan kernel, a call captured into a graph (sync offset: start-up ticks, then points) and
+# replayed between eager calls
+w = WaveEngine({"width": 301, "meter_buf": 40, "channel_mode": "stereo", "audio_sync_offset": 20}, channels=2, max_streams=2,
+               device_clock=True)
+xin = torch.zeros((2, 2, 3 * 441), device="cuda")
+g = torch.cuda.CUDAGraph()
+with torch.cuda.graph(g):
+    o = w.process(xin, 3, 441, want_pixels=True)
+for i in range(4):
+    xin.copy_(torch.from_numpy(synth_pcm(2, 2, 3 * 441, seed=i)))
+    g.replay()
+    w.process(torch.from_numpy(synth_pcm(2, 2, 5 * 97, seed=10 + i)).cuda(), 5, 97)
+torch.cuda.synchronize()
+print("wave device clock graph ok", float(o["min"][..., 0].mean()), flush=True)
 for hop in (441, 480):
     m = MeterEngine({"meter_buf": 20, "rounded_caps": True}, channels=2, max_streams=3)
     x = synth_pcm(3, 2, 9 * hop)

@@ -46,9 +46,9 @@ EXPORTS = [
     "wf_host_alloc", "wf_host_free", "wf_preview_table", "wf_render",
     "wf_meter_config_init", "wf_meter_create", "wf_meter_destroy", "wf_meter_last_error", "wf_meter_window",
     "wf_meter_process", "wf_meter_process_async", "wf_meter_reset", "wf_meter_launch_count", "wf_meter_last_kernel_ms",
-    "wf_wave_config_init", "wf_wave_create", "wf_wave_destroy", "wf_wave_last_error", "wf_wave_process",
-    "wf_wave_process_async", "wf_wave_reset", "wf_wave_launch_count", "wf_wave_last_kernel_ms", "wf_wave_preview_plan",
-    "wf_wave_preview_table",
+    "wf_wave_config_init", "wf_wave_create", "wf_wave_create_with_clock", "wf_wave_destroy", "wf_wave_last_error",
+    "wf_wave_process", "wf_wave_process_async", "wf_wave_reset", "wf_wave_launch_count", "wf_wave_last_kernel_ms",
+    "wf_wave_preview_plan", "wf_wave_preview_table",
 ]
 
 METER_PEAK, METER_RMS, METER_INPUT_RMS = 0, 1, 2
@@ -236,6 +236,7 @@ def load_library():
     L.wf_meter_last_kernel_ms.argtypes = [vp]
     L.wf_wave_config_init.argtypes = [C.POINTER(WfWaveConfig)]
     L.wf_wave_create.argtypes = [C.POINTER(WfWaveConfig), C.POINTER(vp)]
+    L.wf_wave_create_with_clock.argtypes = [C.POINTER(WfWaveConfig), C.c_int32, C.POINTER(vp)]
     L.wf_wave_destroy.argtypes = [vp]
     L.wf_wave_last_error.restype = C.c_char_p
     L.wf_wave_last_error.argtypes = [vp]
@@ -336,11 +337,12 @@ class _Handle:
     def _fn(self, name):
         return getattr(self.L, f"{self._prefix}_{name}")
 
-    def _create(self, cfg):
+    def _create(self, cfg, create="create", *args):
+        """`create`: the C function (after the prefix) that makes the handle from cfg, `args` and the handle's address."""
         self.L = load_library()
         self.cfg = cfg
         h = C.c_void_p()
-        rc = self._fn("create")(C.byref(cfg), C.byref(h))
+        rc = self._fn(create)(C.byref(cfg), *args, C.byref(h))
         if rc != WF_OK:
             raise WfError(rc, f"{self.L.wf_strerror(rc).decode()}: {self._fn('last_error')(None).decode()}")
         self.h = h
@@ -753,13 +755,17 @@ def make_wave_config(settings: dict | None = None, sample_rate: int = 48000, cha
 
 
 class WaveEngine(_Handle):
-    """Waveform (oscilloscope) mode (tick_waveform) on the GPU: ctypes over wf_wave_*; no DSP here."""
+    """Waveform (oscilloscope) mode (tick_waveform) on the GPU: ctypes over wf_wave_*; no DSP here.  device_clock=True
+    keeps the engine's clock and tick plan on the GPU (wf_wave_create_with_clock), so that its calls can be captured into a
+    CUDA graph; it is not a plugin setting, and the outputs are the same either way."""
 
     _prefix = "wf_wave"
 
     def __init__(self, settings: dict | None = None, sample_rate: int = 48000, channels: int = 2, max_streams: int = 1,
-                 device: int = -1):
-        self._create(make_wave_config(settings, sample_rate, channels, max_streams, device))
+                 device: int = -1, device_clock: bool = False):
+        self.device_clock = bool(device_clock)
+        self._create(make_wave_config(settings, sample_rate, channels, max_streams, device), "create_with_clock",
+                     int(self.device_clock))
         self.display_channels = 2 if self.cfg.stereo else 1
 
     def reset(self):
