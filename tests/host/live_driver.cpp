@@ -1,5 +1,5 @@
 // live_driver: feeds packets / ticks to wfhost::SpectrumSourceCUDA the way OBS would and dumps m_decibels per tick.
-// usage: live_driver <pcm.f32> <channels> <samples_per_channel> <fft_size> <packet> <fps> <ticks> <out.f32> [stereo] [normalize_volume]
+// usage: live_driver <pcm.f32> <channels> <samples_per_channel> <fft_size> <packet> <fps> <ticks> <out.f32> [stereo] [normalize_volume] [sample_rate]
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -17,6 +17,7 @@ int main(int argc, char **argv)
     const char *out = argv[8];
     const bool stereo = argc > 9 && atoi(argv[9]) != 0;
     const bool normalize = argc > 10 && atoi(argv[10]) != 0;
+    const uint64_t sr = argc > 11 ? strtoull(argv[11], nullptr, 10) : 48000ull;
     std::vector<float> pcm((size_t)cc * ns);
     FILE *f = fopen(in, "rb");
     if(!f || fread(pcm.data(), sizeof(float), pcm.size(), f) != pcm.size())
@@ -25,6 +26,7 @@ int main(int argc, char **argv)
 
     wf_config cfg;
     wf_config_init(&cfg);
+    cfg.sample_rate = (uint32_t)sr;
     cfg.fft_size = N;
     cfg.capture_channels = cc;
     cfg.stereo = stereo;
@@ -39,7 +41,7 @@ int main(int argc, char **argv)
     }
     FILE *fo = fopen(out, "wb");
     const uint64_t tick_ns = 1000000000ull / (uint64_t)fps;
-    const uint64_t pkt_ns = (uint64_t)packet * 1000000000ull / 48000ull;
+    const uint64_t pkt_ns = (uint64_t)packet * 1000000000ull / sr;
     uint64_t next_pkt = now, audio_clock = now;
     long pos = 0;
     for(int t = 0; t < ticks; ++t)

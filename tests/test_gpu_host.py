@@ -30,7 +30,7 @@ def _reference_live(settings, cc, pcm, N, packet, fps, ticks):
     ref = refbind.RefSource(settings, impl=refbind.IMPL_GENERIC, channels=cc)
     L, h = ref.L, ref.h
     now = 10 * 10**9
-    tick_ns, pkt_ns = 10**9 // fps, packet * 10**9 // 48000
+    tick_ns, pkt_ns = 10**9 // fps, packet * 10**9 // ref.sample_rate
     next_pkt, pos = now, 0
     clock = now
     ns = pcm.shape[1]

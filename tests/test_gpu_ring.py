@@ -390,7 +390,7 @@ def test_ring_against_the_plugin(case):
         got_sil.append(o["silent"][0].cpu().numpy())
         for t in range(T_):
             seg = x[:, pos + t * hop: pos + (t + 1) * hop]
-            ref.advance(hop / 48000.0)
+            ref.advance(hop / ref.sample_rate)
             ref.push(seg[0], seg[1] if cc == 2 else None)
             ref.tick(1.0 / 60.0)
             want_db.append(np.stack([ref.decibels(c) for c in range(dch)]))

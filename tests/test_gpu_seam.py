@@ -63,7 +63,7 @@ def test_wavsource_cuda_volume_normalisation_live_rms_and_hide_show():
                 src.set_showing(False)
             if t == 50:
                 src.set_showing(True)
-            src.advance(hop / 48000.0)
+            src.advance(hop / src.sample_rate)
             src.push(pcm[0, t * hop:(t + 1) * hop], pcm[1, t * hop:(t + 1) * hop])
             src.tick(1.0 / 60.0)
             rows.append(np.stack([src.decibels(0), src.decibels(1)]))

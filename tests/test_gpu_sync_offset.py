@@ -220,7 +220,7 @@ def test_spectrum_offset_against_the_plugin(N, cc, stereo, window, ms):
         want, sil = [], []
         for t in range(T_):
             seg = x[:, pos + t * hop: pos + (t + 1) * hop]
-            pk.advance(hop / SR)
+            pk.advance(hop / pk.sample_rate)
             pk.push(seg[0], seg[1] if cc == 2 else None)
             pk.tick(1.0 / 60.0)
             want.append(np.stack([pk.decibels(c) for c in range(dch)]))

@@ -147,7 +147,7 @@ def test_av_sync_offset_selects_older_frame():
 
     def live():
         ref = _ref(settings=s, channels=1)
-        ref.advance(4 * N / 48000)
+        ref.advance(4 * N / ref.sample_rate)
         ref.push(x[0])                      # packet ends "now"
         ref.tick()
         return {"latest": ref.decibels(0)}
@@ -180,7 +180,7 @@ def test_display_stage_matches_reference_render(settings, channels):
         N, cc = ref.fft_size, ref.capture_channels
         x = synth_pcm(1, cc, T * N, seed=4)[0]
         for t in range(T):
-            ref.advance(N / 48000)
+            ref.advance(N / ref.sample_rate)
             ref.push(x[0, t * N:(t + 1) * N], x[1, t * N:(t + 1) * N] if cc > 1 else None)
             ref.tick()
         ref.render()

@@ -71,7 +71,7 @@ def _packets_vs_plain(N, cc, settings, calls, seed):
         got_db, got_sil = [], []
         for t in range(T_):
             seg = x[:, pos + t * hop: pos + (t + 1) * hop]
-            pk.advance(hop / 48000.0)
+            pk.advance(hop / pk.sample_rate)
             pk.push(seg[0], seg[1] if cc == 2 else None)
             pk.tick(1.0 / 60.0)
             got_db.append(np.stack([pk.decibels(c) for c in range(dch)]))
