@@ -428,6 +428,23 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *batch, void *cuda_
 /* ≙ the capture-timeout branch of tick_meter (src/source_generic.cpp:184-199): unless already silent, zero the ring,
  * m_meter_buf := 0, m_meter_val := DB_MIN, m_last_silent := true. */
 int wf_meter_reset(wf_meter *m, int32_t first_stream, int32_t count);
+/* Checkpoint / restore of the per-stream state of slots [first, first+count) (host buffers, oldest sample first):
+ *   ring   [count][capture_channels][W]  the last W samples of each capture channel (W = wf_meter_window)
+ *   line   [count][capture_channels][D]  the sync offset's delay line (D of wf_meter_config.sync_offset_ms; D = 0: ignored)
+ *   ema    [count][capture_channels]     m_meter_buf (ignored for INPUT_RMS, which has none)
+ *   flags  [count]                       bit0 = m_last_silent
+ * Any pointer may be NULL to skip that part.  A fresh engine shows zero rings and lines, m_meter_buf = DB_MIN (the
+ * reference's start-up value, sic) and flags 0; wf_meter_reset leaves what it documents (the line untouched).  After
+ * wf_meter_set_state the slots continue exactly as if their history had produced the values: the restored ring is the one
+ * the next call reads, whichever half of the double-buffered ring that is, and the slots' block partials of the one-pass
+ * path are dropped (the next call reduces the restored ring again, as after a reset).  Other bits of flags are ignored.
+ * The work is enqueued on the engine's own stream, which is synchronised before the call returns (ordering against the
+ * caller's streams is the caller's job).  WF_ERR_CAPACITY when the range exceeds max_streams; a refused call changes
+ * nothing.  The buffers keep their allocations, so a graph captured earlier reads what wf_meter_set_state wrote. */
+int wf_meter_get_state(wf_meter *m, int32_t first_stream, int32_t count, float *ring, float *line, float *ema,
+                       uint8_t *flags);
+int wf_meter_set_state(wf_meter *m, int32_t first_stream, int32_t count, const float *ring, const float *line,
+                       const float *ema, const uint8_t *flags);
 int64_t wf_meter_launch_count(const wf_meter *m);
 float wf_meter_last_kernel_ms(wf_meter *m);
 
@@ -517,6 +534,35 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *batch, void *cuda_str
 /* ≙ the hidden / capture-timeout branch (src/source_generic.cpp:280-289): unless already silent, buffers := DB_MIN,
  * m_last_silent := true, for every stream. */
 int wf_wave_reset(wf_wave *w);
+/* Checkpoint / restore of the per-stream state of slots [first, first+count) (host buffers):
+ *   db     [count][C][width]               m_decibels, oldest point first; C = 2 when capture_channels > 1 or stereo, else 1.
+ *                                          Row d < display_channels is the last tick's wf_wave_batch.out row d; a second
+ *                                          row of a stereo capture shown mixed holds that channel's raw samples, which the
+ *                                          silent rule reads
+ *   hold   [count][capture_channels][D]    the sync offset's holdback, oldest first (D of sync_offset_ms; D = 0: ignored)
+ *   flags  [count]                         bit0 = m_last_silent (other bits are ignored)
+ * Any pointer may be NULL to skip that part.  A fresh engine shows DB_MIN rows, zero holdbacks and flags 0.  A waveform
+ * source's checkpoint is its slot state AND the engine's clock (wf_wave_get_clock), which every stream of an engine shares:
+ * a call still ticks all streams.  Stream order, the range check and the no-change-on-refusal rule are wf_meter_get_state's. */
+int wf_wave_get_state(wf_wave *w, int32_t first_stream, int32_t count, float *db, float *hold, uint8_t *flags);
+int wf_wave_set_state(wf_wave *w, int32_t first_stream, int32_t count, const float *db, const float *hold,
+                      const uint8_t *flags);
+/* The engine-wide clock of tick_waveform, field for field: the capture clock, m_audio_ts, m_waveform_ts and the samples in
+ * the capture buffer after the last tick.  A fresh engine's is {10^10, 0, 0, width}. */
+typedef struct wf_wave_clock {
+    uint64_t clock_ns, audio_ts, waveform_ts, buffered;
+} wf_wave_clock;
+/* Read / replace the clock, on the host or (device_clock = 1) on the device alike; a clock of either kind of engine restores
+ * into the other.  wf_wave_set_clock refuses with WF_ERR_INVALID_ARG, changing nothing, a clock the timestamp walk of this
+ * engine's config cannot have left:
+ *   - audio_ts == 0 (no tick yet) with anything but the fresh engine's clock {10^10, 0, 0, width}; else audio_ts != clock_ns
+ *     (a tick sets both), or a clock_ns below the 10^10 ns it starts from (ticks only advance it);
+ *   - buffered > max(width, D), unless the tick stopped at the rollover guard (a buffer span above audio_ts, possible when
+ *     meter_ms exceeds the clock's 10 s start), which keeps at most m_waveform_samples + D;
+ *   - waveform_ts + D_ns > audio_ts + step_ns (D_ns: the offset in ns; step_ns = meter_ms * 10^6 / width): a tick leaves
+ *     waveform_ts at most one step past its stop, audio_ts - D_ns. */
+int wf_wave_get_clock(wf_wave *w, wf_wave_clock *clk);
+int wf_wave_set_clock(wf_wave *w, const wf_wave_clock *clk);
 /* The host-side plan of a call made right after wf_wave_create (no device needed; lets a CPU-only test check the integer
  * timestamp walk against the plugin): counts[t] = points emitted by tick t; src (optional, `capacity` entries) = for every
  * point in order the index of the sample it takes in the call's PCM, or -1 for a start-up zero (with a sync offset, also

@@ -94,3 +94,19 @@ for hop in (441, 480):
     x = synth_pcm(3, 2, 9 * hop)
     a = m.process(x, 9, hop, want_pixels=True)
     print("meter display", hop, "ok", float(a["pixels"].mean()), flush=True)
+# checkpoints: meter and waveform state (ring halves picked on the device, delay lines, holdbacks) and the waveform clock,
+# moved from one engine into slots of a larger one and run on; the device-clock engine's graph replays after a restore
+for mode in (None, METER_INPUT_RMS):
+    src, dst = (MeterEngine({"meter_buf": 20, "audio_sync_offset": 15}, channels=2, max_streams=n, mode=mode) for n in (2, 5))
+    src.process(synth_pcm(2, 2, 7 * 480), 7, 480)
+    dst.set_state(src.get_state(), first_stream=3)
+    dst.process(synth_pcm(2, 2, 3 * 441), 3, 441, first_stream=3)
+    print("meter state", mode, "ok", float(dst.get_state(3, 2)["ring"].mean()), flush=True)
+src = WaveEngine({"width": 301, "meter_buf": 40, "channel_mode": "stereo", "audio_sync_offset": 20}, channels=2, max_streams=3)
+src.process(synth_pcm(3, 2, 4 * 441), 4, 441)
+w.set_state(src.get_state(1, 2))
+w.set_clock(src.get_clock())
+xin.copy_(torch.from_numpy(synth_pcm(2, 2, 3 * 441, seed=20)))
+g.replay()
+torch.cuda.synchronize()
+print("wave state", "ok", float(w.get_state()["db"].mean()), w.get_clock(), flush=True)

@@ -317,4 +317,67 @@ class Staging {
     }
 };
 
+// The host buffers of a state call (wf_meter_get_state, wf_wave_set_state, ...) as the sections of one staging buffer, so
+// that the call makes one copy and one launch.  add() places a section 16-byte aligned (null or empty: skipped); after
+// reserve(), dev() gives a section's device pointer (null when skipped).  run() does the call on `st`: a set call packs
+// the sections, copies them to the device and launches; a get call launches, copies them back and unpacks them.  The
+// stream is synchronised before it returns, and the launch counts as one of the engine's.
+class StateSections {
+  public:
+    int add(const void *host, size_t bytes)
+    {
+        if(!host || !bytes)
+            return -1;
+        sec[n] = {const_cast<void *>(host), total, bytes};
+        total = (total + bytes + 15) & ~(size_t)15;
+        return n++;
+    }
+    int reserve(HostCore *c, DevBuf<unsigned char> &d, std::vector<unsigned char> &h)
+    {
+        if(int rc = d.reserve(c, total))
+            return rc;
+        if(h.size() < total)
+            h.resize(total);
+        dbase = d.p;
+        hbase = h.data();
+        return WF_OK;
+    }
+    template<class T>
+    T *dev(int i) const
+    {
+        return (i < 0) ? nullptr : reinterpret_cast<T *>(dbase + sec[i].off);
+    }
+    bool empty() const { return n == 0; }
+    // `launch` enqueues the kernel on `st` and returns cudaGetLastError()
+    template<class Launch>
+    int run(HostCore *c, cudaStream_t st, bool set, Launch &&launch)
+    {
+        if(set)
+        {
+            for(int i = 0; i < n; ++i)
+                memcpy(hbase + sec[i].off, sec[i].host, sec[i].bytes);
+            WF_CHECK(c, cudaMemcpyAsync(dbase, hbase, total, cudaMemcpyHostToDevice, st));
+        }
+        WF_CHECK(c, launch());
+        c->launches++;
+        if(!set)
+            WF_CHECK(c, cudaMemcpyAsync(hbase, dbase, total, cudaMemcpyDeviceToHost, st));
+        WF_CHECK(c, cudaStreamSynchronize(st));
+        if(!set)
+            for(int i = 0; i < n; ++i)
+                memcpy(sec[i].host, hbase + sec[i].off, sec[i].bytes);
+        return WF_OK;
+    }
+
+  private:
+    struct Sec {
+        void *host;
+        size_t off, bytes;
+    };
+    Sec sec[4]{};
+    int n = 0;
+    size_t total = 0;
+    unsigned char *dbase = nullptr, *hbase = nullptr;
+};
+
 } // namespace wf

@@ -28,6 +28,7 @@
 #include <cstddef>
 #include <cstring>
 #include <string>
+#include <vector>
 
 #include "wf_display.cuh"
 #include "wf_host.hpp"
@@ -542,6 +543,60 @@ __global__ void meter_reset_kernel(float *ring0, float *ring1, const unsigned ch
     }
 }
 
+// wf_meter_get_state / wf_meter_set_state: the state of streams [first, first+count) between the device layouts and the
+// sections of one staging buffer (x_*, null = skipped), one CTA per stream.  The ring is the half the stream's parity
+// selects, read here because after graph replays only the device knows it.  SET also drops the stream's block partials
+// (as a reset does): the next one-pass call reduces the restored ring again, block by block in the order it reduced those
+// samples as new PCM, so it gets the partials the stream's history would have left bit for bit.
+struct MStateIO {
+    float *ring[2];
+    const unsigned char *par;
+    long long *ptag;
+    float *buf, *line;
+    unsigned char *flags;
+    float *x_ring, *x_line, *x_ema; // [count][cc][W], [count][cc][D], [count][cc]
+    unsigned char *x_flags;         // [count]
+    int first, count, cc, W, D;
+};
+template<bool SET>
+__device__ __forceinline__ void move_state(float *dev, float *x, long long n)
+{
+    for(long long k = threadIdx.x; k < n; k += blockDim.x)
+    {
+        if(SET)
+            dev[k] = x[k];
+        else
+            x[k] = dev[k];
+    }
+}
+template<bool SET>
+__global__ void meter_state_kernel(const MStateIO q)
+{
+    for(int i = blockIdx.x; i < q.count; i += gridDim.x)
+    {
+        const int s = q.first + i;
+        const long long rn = (long long)q.cc * q.W, ln = (long long)q.cc * q.D;
+        if(q.x_ring)
+            move_state<SET>(((q.par[s] & 1) ? q.ring[1] : q.ring[0]) + (size_t)s * rn, q.x_ring + (size_t)i * rn, rn);
+        if(q.x_line)
+            move_state<SET>(q.line + (size_t)s * ln, q.x_line + (size_t)i * ln, ln);
+        if(q.x_ema)
+            move_state<SET>(q.buf + 2 * (size_t)s, q.x_ema + (size_t)i * q.cc, q.cc);
+        if(threadIdx.x == 0)
+        {
+            if(q.x_flags)
+            {
+                if(SET)
+                    q.flags[s] = q.x_flags[i] & 1;
+                else
+                    q.x_flags[i] = q.flags[s] & 1;
+            }
+            if(SET)
+                q.ptag[s] = 0;
+        }
+    }
+}
+
 } // namespace
 
 struct wf_meter : wf::HostCore {
@@ -568,6 +623,9 @@ struct wf_meter : wf::HostCore {
     // scratch / staging
     wf::DevBuf<float> d_partial, d_raw, s_pcm, s_db, s_lin, s_pixels, s_min;
     wf::DevBuf<unsigned char> s_silent;
+    // wf_meter_get_state / wf_meter_set_state: the sections of a call, on the device and on the host
+    wf::DevBuf<unsigned char> s_state;
+    std::vector<unsigned char> h_state;
     // display stage: only when the config carried display settings (current struct size)
     bool display = false;
     float ceiling_f = 0.0f, dbrange_f = 1.0f, px_lo = 0.0f, px_hi = 0.0f, px_cpos = 0.0f;
@@ -958,6 +1016,73 @@ int wf_meter_reset(wf_meter *m, int32_t first, int32_t count)
     m->launches++;
     WF_CHECK(m, cudaStreamSynchronize(m->stream));
     return WF_OK;
+}
+
+} // extern "C"
+
+namespace {
+
+// wf_meter_get_state (set = false) / wf_meter_set_state (set = true): the range check, then one copy and one launch on the
+// engine's stream, which is synchronised
+int meter_state(wf_meter *m, int32_t first, int32_t count, const float *ring, const float *line, const float *ema,
+                const uint8_t *flags, bool set)
+{
+    if(!m)
+        return WF_ERR_INVALID_ARG;
+    if(first < 0 || count < 0 || (int64_t)first + count > m->cfg.max_streams)
+        return wf::fail(m, WF_ERR_CAPACITY, "state range [%d, %lld) exceeds max_streams %d", first, (long long)first + count,
+                        m->cfg.max_streams);
+    const size_t n = (size_t)count, cc = (size_t)m->cfg.capture_channels;
+    wf::StateSections io;
+    const int i_ring = io.add(ring, n * cc * m->W * sizeof(float));
+    const int i_line = io.add(line, n * cc * m->D * sizeof(float));
+    const int i_ema = io.add((m->cfg.mode == WF_METER_INPUT_RMS) ? nullptr : ema, n * cc * sizeof(float));
+    const int i_flags = io.add(flags, n);
+    if(io.empty())
+        return WF_OK;
+    WF_CHECK(m, cudaSetDevice(m->device));
+    if(int rc = io.reserve(m, m->s_state, m->h_state))
+        return rc;
+    MStateIO q{};
+    q.ring[0] = m->d_hist[0];
+    q.ring[1] = m->d_hist[1];
+    q.par = m->d_par;
+    q.ptag = m->d_ptag;
+    q.buf = m->d_buf;
+    q.line = m->d_line;
+    q.flags = m->d_flags;
+    q.x_ring = io.dev<float>(i_ring);
+    q.x_line = io.dev<float>(i_line);
+    q.x_ema = io.dev<float>(i_ema);
+    q.x_flags = io.dev<unsigned char>(i_flags);
+    q.first = first;
+    q.count = count;
+    q.cc = (int)cc;
+    q.W = m->W;
+    q.D = m->D;
+    const int grid = std::min(count, m->sm_count * 4);
+    return io.run(m, m->stream, set, [&] {
+        if(set)
+            meter_state_kernel<true><<<grid, 256, 0, m->stream>>>(q);
+        else
+            meter_state_kernel<false><<<grid, 256, 0, m->stream>>>(q);
+        return cudaGetLastError();
+    });
+}
+
+} // namespace
+
+extern "C" {
+
+int wf_meter_get_state(wf_meter *m, int32_t first, int32_t count, float *ring, float *line, float *ema, uint8_t *flags)
+{
+    return meter_state(m, first, count, ring, line, ema, flags, false);
+}
+
+int wf_meter_set_state(wf_meter *m, int32_t first, int32_t count, const float *ring, const float *line, const float *ema,
+                       const uint8_t *flags)
+{
+    return meter_state(m, first, count, ring, line, ema, flags, true);
 }
 
 int64_t wf_meter_launch_count(const wf_meter *m) { return m ? m->launches : 0; }

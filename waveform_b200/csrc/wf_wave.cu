@@ -843,6 +843,53 @@ __global__ void wave_reset_kernel(float *state, unsigned char *flags, int n_stre
     }
 }
 
+// wf_wave_get_state / wf_wave_set_state: the state of streams [first, first+count) between the device layouts and the
+// sections of one staging buffer (x_*, null = skipped), one CTA per stream.  Rows d < och of the [2][width] scrolling
+// buffers (row 1 of a one-channel engine shown as one is never used).
+struct WStateIO {
+    float *state, *hold;
+    unsigned char *flags;
+    float *x_db, *x_hold;    // [count][och][width], [count][cc][D]
+    unsigned char *x_flags;  // [count]
+    int first, count, och, width, cc, D;
+};
+template<bool SET>
+__global__ void wave_state_kernel(const WStateIO q)
+{
+    for(int i = blockIdx.x; i < q.count; i += gridDim.x)
+    {
+        const int s = q.first + i;
+        if(q.x_db)
+            for(int k = threadIdx.x; k < q.och * q.width; k += blockDim.x)
+            {
+                float *d = q.state + (size_t)s * 2 * q.width + k, *x = q.x_db + (size_t)i * q.och * q.width + k;
+                if(SET)
+                    *d = *x;
+                else
+                    *x = *d;
+            }
+        if(q.x_hold)
+        {
+            const long long n = (long long)q.cc * q.D;
+            for(long long k = threadIdx.x; k < n; k += blockDim.x)
+            {
+                float *d = q.hold + (size_t)s * n + k, *x = q.x_hold + (size_t)i * n + k;
+                if(SET)
+                    *d = *x;
+                else
+                    *x = *d;
+            }
+        }
+        if(q.x_flags && threadIdx.x == 0)
+        {
+            if(SET)
+                q.flags[s] = q.x_flags[i] & 1;
+            else
+                q.x_flags[i] = q.flags[s] & 1;
+        }
+    }
+}
+
 // util.hpp's audio_frames_to_ns / ns_to_audio_frames (128-bit multiply-divide).  The 64-bit form is the same quotient
 // whenever the product fits, which it does for everything but multi-day spans; the 128-bit division costs ~50 ns and the
 // plan evaluates one per point.
@@ -865,6 +912,7 @@ __host__ __device__ inline uint64_t ns_to_frames(uint64_t sr, uint64_t ns)
 struct WaveClock {
     uint64_t clock, audio_ts, waveform_ts, buffered;
 };
+constexpr uint64_t kClockStart = 10ull * 1000000000ull; // the capture clock of a new engine, in ns (10 s)
 // What a call's walk depends on besides the clock: the config, the sync offset's D and the call's hop (wave_walk).
 struct WaveWalk {
     uint64_t sr, ws, D, width, step_ns, hop, hop_ns, D_ns;
@@ -1125,7 +1173,7 @@ struct wf_wave : wf::HostCore {
     float db_min = 0.0f;
     // the clock the reference derives from packet timestamps (shared by all streams: they tick together); `buffered` holds
     // the start-up zeros at first (src/source.cpp:1243-1248), then at most D (tick_waveform keeps the reserve)
-    WaveClock clk{10ull * 1000000000ull, 0, 0, 0};
+    WaveClock clk{kClockStart, 0, 0, 0};
     int D = 0;            // samples the audio sync offset reserves (wf_wave_config.sync_offset_ms)
     // device_clock of wf_wave_create_with_clock: the clock lives in d_clock (created as clk is), and wave_plan_kernel plans
     // every call from it
@@ -1139,6 +1187,9 @@ struct wf_wave : wf::HostCore {
     wf::DevBuf<int> d_src, d_off;
     wf::DevBuf<float> s_pcm, s_out, s_rms, s_points, s_pixels, s_min;
     wf::DevBuf<unsigned char> s_silent;
+    // wf_wave_get_state / wf_wave_set_state: the sections of a call, on the device and on the host
+    wf::DevBuf<unsigned char> s_state;
+    std::vector<unsigned char> h_state;
     struct PlanSlot {
         int *h = nullptr; // pinned: off[] then src[]
         size_t cap = 0;
@@ -1619,6 +1670,132 @@ int wf_wave_reset(wf_wave *w)
     WF_CHECK(w, cudaGetLastError());
     w->launches++;
     WF_CHECK(w, cudaStreamSynchronize(w->stream));
+    return WF_OK;
+}
+
+} // extern "C"
+
+namespace {
+
+static_assert(sizeof(wf_wave_clock) == sizeof(WaveClock) && offsetof(wf_wave_clock, clock_ns) == offsetof(WaveClock, clock) &&
+                  offsetof(wf_wave_clock, audio_ts) == offsetof(WaveClock, audio_ts) &&
+                  offsetof(wf_wave_clock, waveform_ts) == offsetof(WaveClock, waveform_ts) &&
+                  offsetof(wf_wave_clock, buffered) == offsetof(WaveClock, buffered),
+              "wf_wave_clock is WaveClock field for field");
+
+// wf_wave_get_state (set = false) / wf_wave_set_state (set = true): the range check, then one copy and one launch on the
+// engine's stream, which is synchronised
+int wave_state(wf_wave *w, int32_t first, int32_t count, const float *db, const float *hold, const uint8_t *flags, bool set)
+{
+    if(!w)
+        return WF_ERR_INVALID_ARG;
+    if(first < 0 || count < 0 || (int64_t)first + count > w->cfg.max_streams)
+        return wf::fail(w, WF_ERR_CAPACITY, "state range [%d, %lld) exceeds max_streams %d", first, (long long)first + count,
+                        w->cfg.max_streams);
+    const size_t n = (size_t)count, cc = (size_t)w->cfg.capture_channels;
+    wf::StateSections io;
+    const int i_db = io.add(db, n * w->och * w->cfg.width * sizeof(float));
+    const int i_hold = io.add(hold, n * cc * w->D * sizeof(float));
+    const int i_flags = io.add(flags, n);
+    if(io.empty())
+        return WF_OK;
+    WF_CHECK(w, cudaSetDevice(w->device));
+    if(int rc = io.reserve(w, w->s_state, w->h_state))
+        return rc;
+    WStateIO q{};
+    q.state = w->d_state;
+    q.hold = w->d_hold;
+    q.flags = w->d_flags;
+    q.x_db = io.dev<float>(i_db);
+    q.x_hold = io.dev<float>(i_hold);
+    q.x_flags = io.dev<unsigned char>(i_flags);
+    q.first = first;
+    q.count = count;
+    q.och = w->och;
+    q.width = w->cfg.width;
+    q.cc = (int)cc;
+    q.D = w->D;
+    const int grid = std::min(count, w->sm_count * 4);
+    return io.run(w, w->stream, set, [&] {
+        if(set)
+            wave_state_kernel<true><<<grid, 256, 0, w->stream>>>(q);
+        else
+            wave_state_kernel<false><<<grid, 256, 0, w->stream>>>(q);
+        return cudaGetLastError();
+    });
+}
+
+// Whether the timestamp walk (wave_tick from the creation clock) can have left `c`; the rules are wf_wave_set_clock's in
+// wfstft.h.  Before the first tick the clock is the creation clock.  Every tick advances the clock from kClockStart and
+// sets audio_ts := clock; a tick that passes the rollover guard leaves buffered <= D (none emitted:
+// the buffer, at most D; else the reserve D) and waveform_ts at most one step past its stop audio_ts - D_ns (the desync
+// reset catches anything further); one stopped by the guard keeps its buffer (at most ws + D) and waveform_ts.
+bool wave_clock_valid(const wf_wave *w, const WaveClock &c)
+{
+    const uint64_t width = (uint64_t)w->cfg.width, D = (uint64_t)w->D, sr = w->cfg.sample_rate;
+    if(c.audio_ts == 0)
+        return c.clock == kClockStart && c.waveform_ts == 0 && c.buffered == width;
+    if(c.audio_ts != c.clock || c.clock < kClockStart)
+        return false;
+    if(c.buffered > std::max(width, D))
+    {
+        const uint64_t total_ns = frames_to_ns(sr, c.buffered), D_ns = frames_to_ns(sr, D);
+        const bool guard = (c.audio_ts - total_ns >= c.audio_ts) || (c.audio_ts - D_ns > c.audio_ts);
+        if(!guard || c.buffered > w->ws + D)
+            return false;
+    }
+    const uint64_t step_ns = ((uint64_t)w->cfg.meter_ms * 1000000ull) / width;
+    return (unsigned __int128)c.waveform_ts + frames_to_ns(sr, D) <= (unsigned __int128)c.audio_ts + step_ns;
+}
+
+} // namespace
+
+extern "C" {
+
+int wf_wave_get_state(wf_wave *w, int32_t first, int32_t count, float *db, float *hold, uint8_t *flags)
+{
+    return wave_state(w, first, count, db, hold, flags, false);
+}
+
+int wf_wave_set_state(wf_wave *w, int32_t first, int32_t count, const float *db, const float *hold, const uint8_t *flags)
+{
+    return wave_state(w, first, count, db, hold, flags, true);
+}
+
+int wf_wave_get_clock(wf_wave *w, wf_wave_clock *clk)
+{
+    if(!w || !clk)
+        return WF_ERR_INVALID_ARG;
+    WaveClock c = w->clk;
+    if(w->dev_clock)
+    {
+        WF_CHECK(w, cudaSetDevice(w->device));
+        WF_CHECK(w, cudaMemcpyAsync(&c, w->d_clock.p, sizeof(WaveClock), cudaMemcpyDeviceToHost, w->stream));
+        WF_CHECK(w, cudaStreamSynchronize(w->stream));
+    }
+    memcpy(clk, &c, sizeof(c));
+    return WF_OK;
+}
+
+int wf_wave_set_clock(wf_wave *w, const wf_wave_clock *clk)
+{
+    if(!w || !clk)
+        return WF_ERR_INVALID_ARG;
+    WaveClock c;
+    memcpy(&c, clk, sizeof(c));
+    if(!wave_clock_valid(w, c))
+        return wf::fail(w, WF_ERR_INVALID_ARG,
+                        "clock {%llu, %llu, %llu, %llu} cannot come from this engine's timestamp walk (see wfstft.h)",
+                        (unsigned long long)c.clock, (unsigned long long)c.audio_ts, (unsigned long long)c.waveform_ts,
+                        (unsigned long long)c.buffered);
+    if(w->dev_clock)
+    {
+        WF_CHECK(w, cudaSetDevice(w->device));
+        WF_CHECK(w, cudaMemcpyAsync(w->d_clock.p, &c, sizeof(WaveClock), cudaMemcpyHostToDevice, w->stream));
+        WF_CHECK(w, cudaStreamSynchronize(w->stream));
+    }
+    else
+        w->clk = c;
     return WF_OK;
 }
 

@@ -45,9 +45,11 @@ EXPORTS = [
     "wf_get_state", "wf_set_state", "wf_get_ring", "wf_set_ring", "wf_peak_normalize", "wf_launch_count", "wf_last_kernel_ms", "wf_last_kernel_name",
     "wf_host_alloc", "wf_host_free", "wf_preview_table", "wf_render",
     "wf_meter_config_init", "wf_meter_create", "wf_meter_destroy", "wf_meter_last_error", "wf_meter_window",
-    "wf_meter_process", "wf_meter_process_async", "wf_meter_reset", "wf_meter_launch_count", "wf_meter_last_kernel_ms",
+    "wf_meter_process", "wf_meter_process_async", "wf_meter_reset", "wf_meter_get_state", "wf_meter_set_state",
+    "wf_meter_launch_count", "wf_meter_last_kernel_ms",
     "wf_wave_config_init", "wf_wave_create", "wf_wave_create_with_clock", "wf_wave_destroy", "wf_wave_last_error",
-    "wf_wave_process", "wf_wave_process_async", "wf_wave_reset", "wf_wave_launch_count", "wf_wave_last_kernel_ms",
+    "wf_wave_process", "wf_wave_process_async", "wf_wave_reset", "wf_wave_get_state", "wf_wave_set_state",
+    "wf_wave_get_clock", "wf_wave_set_clock", "wf_wave_launch_count", "wf_wave_last_kernel_ms",
     "wf_wave_preview_plan", "wf_wave_preview_table",
 ]
 
@@ -82,6 +84,11 @@ class WfWaveBatch(C.Structure):
         ("out_points", C.c_void_p), ("out_pixels", C.c_void_p), ("out_min", C.c_void_p),
         ("pcm_format", C.c_int32),
     ]
+
+
+class WfWaveClock(C.Structure):
+    """wf_wave_clock: the engine-wide clock of tick_waveform (WaveEngine.get_clock / set_clock)."""
+    _fields_ = [("clock_ns", C.c_uint64), ("audio_ts", C.c_uint64), ("waveform_ts", C.c_uint64), ("buffered", C.c_uint64)]
 
 
 class WfMeterBatch(C.Structure):
@@ -230,6 +237,8 @@ def load_library():
     L.wf_meter_process.argtypes = [vp, C.POINTER(WfMeterBatch)]
     L.wf_meter_process_async.argtypes = [vp, C.POINTER(WfMeterBatch), vp]
     L.wf_meter_reset.argtypes = [vp, C.c_int32, C.c_int32]
+    L.wf_meter_get_state.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp, vp]
+    L.wf_meter_set_state.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp, vp]
     L.wf_meter_launch_count.restype = C.c_int64
     L.wf_meter_launch_count.argtypes = [vp]
     L.wf_meter_last_kernel_ms.restype = C.c_float
@@ -243,6 +252,10 @@ def load_library():
     L.wf_wave_process.argtypes = [vp, C.POINTER(WfWaveBatch)]
     L.wf_wave_process_async.argtypes = [vp, C.POINTER(WfWaveBatch), vp]
     L.wf_wave_reset.argtypes = [vp]
+    L.wf_wave_get_state.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp]
+    L.wf_wave_set_state.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp]
+    L.wf_wave_get_clock.argtypes = [vp, C.POINTER(WfWaveClock)]
+    L.wf_wave_set_clock.argtypes = [vp, C.POINTER(WfWaveClock)]
     L.wf_wave_launch_count.restype = C.c_int64
     L.wf_wave_launch_count.argtypes = [vp]
     L.wf_wave_last_kernel_ms.restype = C.c_float
@@ -368,6 +381,29 @@ class _Handle:
 
     def last_kernel_ms(self) -> float:
         return float(self._fn("last_kernel_ms")(self.h))
+
+
+def _sync_delay(sample_rate: int, ms: int) -> int:
+    """Samples an audio sync offset of `ms` holds back: ns_to_audio_frames(sample_rate, ms * 10**6) for ms > 0, else 0."""
+    return sample_rate * ms // 1000 if ms > 0 else 0
+
+
+def _state_parts(state: dict, parts: dict):
+    """The host arrays of a meter / waveform checkpoint for a set call: `parts` maps each key to (per-slot shape, dtype).
+    A missing or None part is skipped; the others must be [count, *per-slot shape] with one count, else ValueError (before
+    any library call).  Returns (count, {key: contiguous array or None})."""
+    out, count = {}, None
+    for key, (shape, dtype) in parts.items():
+        a = state.get(key)
+        if a is not None:
+            a = np.ascontiguousarray(a, dtype=dtype)
+            if a.ndim != 1 + len(shape) or a.shape[1:] != tuple(shape):
+                raise ValueError(f"state[{key!r}] must be [count, {', '.join(map(str, shape))}], got {list(a.shape)}")
+            if count is not None and a.shape[0] != count:
+                raise ValueError(f"state[{key!r}] holds {a.shape[0]} slots, another part {count}")
+            count = a.shape[0]
+        out[key] = a
+    return (0 if count is None else count), out
 
 
 class _Inputs:
@@ -569,7 +605,7 @@ class Engine(_Handle):
     def sync_delay(self) -> int:
         """Samples the audio sync offset holds back: ns_to_audio_frames(sample_rate, offset) for an offset > 0, else 0."""
         ms = self.cfg.sync_offset_ms if self.cfg.struct_size == C.sizeof(WfConfig) else 0  # the previous size has none
-        return self.cfg.sample_rate * ms // 1000 if ms > 0 else 0
+        return _sync_delay(self.cfg.sample_rate, ms)
 
     def get_ring(self, first_stream=0, count=None):
         """The capture rings of slots [first_stream, first_stream + count): float32
@@ -690,6 +726,31 @@ class MeterEngine(_Handle):
         count = self.cfg.max_streams - first_stream if count is None else count
         self._check(self.L.wf_meter_reset(self.h, first_stream, count))
 
+    def _state_shapes(self):
+        cc, D = self.cfg.capture_channels, _sync_delay(self.cfg.sample_rate, self.cfg.sync_offset_ms)
+        parts = {"ring": ((cc, self.window), np.float32), "line": ((cc, D), np.float32), "ema": ((cc,), np.float32),
+                 "flags": ((), np.uint8)}
+        if self.cfg.mode == METER_INPUT_RMS:
+            del parts["ema"]  # the RMS feed has no EMA
+        return parts
+
+    def get_state(self, first_stream=0, count=None) -> dict:
+        """The state of slots [first_stream, first_stream + count) (wf_meter_get_state): ring [count, cc, window] (the last
+        window samples, oldest first), line [count, cc, D] (the sync offset's delay line), ema [count, cc] (m_meter_buf;
+        None for INPUT_RMS) and flags [count] (bit0 = m_last_silent)."""
+        count = self.cfg.max_streams - first_stream if count is None else count
+        st = {k: np.zeros((max(count, 0), *shape), dtype) for k, (shape, dtype) in self._state_shapes().items()}
+        self._check(self.L.wf_meter_get_state(self.h, first_stream, count, st["ring"].ctypes.data, st["line"].ctypes.data,
+                                              _ptr(st.get("ema")), st["flags"].ctypes.data))
+        return {"ring": st["ring"], "line": st["line"], "ema": st.get("ema"), "flags": st["flags"]}
+
+    def set_state(self, state: dict, first_stream=0):
+        """Restore slots [first_stream, first_stream + count) from a get_state dict (of this or another engine with the
+        same config); a missing or None part is left as it is."""
+        count, a = _state_parts(state, self._state_shapes())
+        self._check(self.L.wf_meter_set_state(self.h, first_stream, count, _ptr(a["ring"]), _ptr(a["line"]),
+                                              _ptr(a.get("ema")), _ptr(a["flags"])))
+
     def process(self, pcm, n_ticks: int, hop: int, *, first_stream=0, seconds=1.0 / 60.0, stream=None, want_pixels=False,
                 pcm_format="f32"):
         """pcm: [n_streams, capture_channels, >= n_ticks*hop] float32, numpy (host) or CUDA torch tensor.
@@ -770,6 +831,44 @@ class WaveEngine(_Handle):
 
     def reset(self):
         self._check(self.L.wf_wave_reset(self.h))
+
+    def _state_shapes(self):
+        cc, W = self.cfg.capture_channels, self.cfg.width
+        och = 2 if (cc > 1 or self.cfg.stereo) else 1  # the m_decibels rows
+        D = _sync_delay(self.cfg.sample_rate, self.cfg.sync_offset_ms)
+        return {"db": ((och, W), np.float32), "hold": ((cc, D), np.float32), "flags": ((), np.uint8)}
+
+    def get_state(self, first_stream=0, count=None) -> dict:
+        """The state of slots [first_stream, first_stream + count) (wf_wave_get_state): db [count, C, width] (m_decibels,
+        oldest point first; C = 2 for a stereo capture or stereo display, else 1), hold [count, cc, D] (the sync offset's
+        holdback) and flags [count] (bit0 = m_last_silent).  A source's checkpoint also needs the engine's get_clock()."""
+        count = self.cfg.max_streams - first_stream if count is None else count
+        st = {k: np.zeros((max(count, 0), *shape), dtype) for k, (shape, dtype) in self._state_shapes().items()}
+        self._check(self.L.wf_wave_get_state(self.h, first_stream, count, st["db"].ctypes.data, st["hold"].ctypes.data,
+                                             st["flags"].ctypes.data))
+        return st
+
+    def set_state(self, state: dict, first_stream=0):
+        """Restore slots [first_stream, first_stream + count) from a get_state dict; a missing or None part is left as it
+        is.  The engine's clock is restored separately (set_clock)."""
+        count, a = _state_parts(state, self._state_shapes())
+        self._check(self.L.wf_wave_set_state(self.h, first_stream, count, _ptr(a["db"]), _ptr(a["hold"]), _ptr(a["flags"])))
+
+    def get_clock(self) -> dict:
+        """The engine-wide clock (wf_wave_get_clock) as dict(clock_ns, audio_ts, waveform_ts, buffered)."""
+        c = WfWaveClock()
+        self._check(self.L.wf_wave_get_clock(self.h, C.byref(c)))
+        return {name: int(getattr(c, name)) for name, _ in WfWaveClock._fields_}
+
+    def set_clock(self, clk):
+        """Replace the engine-wide clock with a get_clock() dict, or a (clock_ns, audio_ts, waveform_ts, buffered) tuple,
+        of this engine or another with the same config, host or device clock alike.  WfError (WF_ERR_INVALID_ARG) for a
+        clock this config's timestamp walk cannot have left; the clock then stays as it was."""
+        names = [name for name, _ in WfWaveClock._fields_]
+        values = [clk[n] for n in names] if isinstance(clk, dict) else list(clk)
+        if len(values) != len(names):
+            raise ValueError(f"a clock has {len(names)} fields {names}, got {len(values)}")
+        self._check(self.L.wf_wave_set_clock(self.h, C.byref(WfWaveClock(*(int(v) for v in values)))))
 
     def process(self, pcm, n_ticks: int, hop: int, *, input_rms=None, stream=None, want_db=True, want_points=False,
                 want_pixels=False, pcm_format="f32"):
