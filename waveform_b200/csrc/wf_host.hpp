@@ -202,6 +202,37 @@ bool accept_struct(const T *in, std::initializer_list<size_t> prev_sizes, T &out
 // address.
 int pcm_sample_bytes(HostCore *c, int32_t format, const void *pcm, size_t *bytes);
 
+// A call's PCM as the kernels read it: `pcm` in the call's sample type (behind a `const float *`), strides in samples.
+struct PcmView {
+    const float *pcm;
+    long long stream_stride, channel_stride;
+};
+
+// What check_pcm_batch finds of a level-meter or waveform batch's PCM.
+struct PcmBatch {
+    size_t sample_bytes = 0;
+    bool s16 = false;
+    size_t span = 0; // samples from pcm to the end of the last row: (S-1)*stream_stride + (cc-1)*channel_stride + T*hop
+};
+
+// The checks of a wf_meter_batch or wf_wave_batch `b` (at least one stream, `cc` capture channels) that both engines make
+// alike, in this order: no negative stride, the sample format (pcm_sample_bytes), and n_ticks * hop within int range with
+// `reserve` samples ahead of the call's own in every row the kernels index (the meter's window, the waveform's holdback).
+template<class B>
+int check_pcm_batch(HostCore *c, const B &b, int cc, int reserve, PcmBatch *out)
+{
+    if(b.stream_stride < 0 || b.channel_stride < 0)
+        return fail(c, WF_ERR_INVALID_ARG, "negative strides are not supported");
+    if(int rc = pcm_sample_bytes(c, b.pcm_format, b.pcm, &out->sample_bytes))
+        return rc;
+    out->s16 = b.pcm_format == WF_PCM_S16;
+    if((long long)b.n_ticks * b.hop > 0x7fffffffLL - reserve)
+        return fail(c, WF_ERR_INVALID_ARG, "n_ticks * hop too large for one call");
+    out->span = (size_t)(b.n_streams - 1) * (size_t)b.stream_stride + (size_t)(cc - 1) * (size_t)b.channel_stride +
+                (size_t)b.n_ticks * (size_t)b.hop;
+    return WF_OK;
+}
+
 // Lets `kernel` use `bytes` of dynamic shared memory on `device` (the opt-in above the default 48 KB).  Asks CUDA once per
 // kernel, device and size: a size at or below one already granted returns at once.
 cudaError_t opt_in_smem(const void *kernel, int device, size_t bytes);
@@ -348,7 +379,7 @@ class StateSections {
         return (i < 0) ? nullptr : reinterpret_cast<T *>(dbase + sec[i].off);
     }
     bool empty() const { return n == 0; }
-    // `launch` enqueues the kernel on `st` and returns cudaGetLastError()
+    // `launch` enqueues the kernel on `st` and returns the launch's error
     template<class Launch>
     int run(HostCore *c, cudaStream_t st, bool set, Launch &&launch)
     {

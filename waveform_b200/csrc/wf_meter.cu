@@ -597,6 +597,18 @@ __global__ void meter_state_kernel(const MStateIO q)
     }
 }
 
+// The kernels of one mode and sample type: the one-pass kernel, and K1 and K2 of the three-kernel path (K3,
+// meter_scan_kernel, reads no PCM and has one instantiation)
+struct MeterKernels {
+    void (*fused)(MParams);
+    void (*block)(MParams, int);
+    void (*window)(MParams);
+};
+template<int MODE>
+constexpr MeterKernels kMeterKernels[2] = { // [s16]
+    {meter_fused_kernel<MODE, float>, meter_block_kernel<MODE, float>, meter_window_kernel<MODE, float>},
+    {meter_fused_kernel<MODE, int16_t>, meter_block_kernel<MODE, int16_t>, meter_window_kernel<MODE, int16_t>}};
+
 } // namespace
 
 struct wf_meter : wf::HostCore {
@@ -614,6 +626,7 @@ struct wf_meter : wf::HostCore {
     long long part_gen = 0;
     int part_nbk = 0;
     bool use_fused = true; // WF_METER_FUSED=0: always the three-kernel path (A/B tests)
+    const MeterKernels *kern = nullptr; // [s16]: the instantiations of the engine's mode
     wf::DevBuf<float> d_buf;
     wf::DevBuf<unsigned char> d_flags;
     // audio sync offset: the newest D samples of each stream slot and capture channel, held back for the next call
@@ -725,6 +738,9 @@ int wf_meter_create(const wf_meter_config *cfg_in, wf_meter **out)
             m->px_cpos = cpos;
         }
         m->use_fused = wf::env_flag("WF_METER_FUSED", true);
+        m->kern = (cfg->mode == WF_METER_PEAK) ? kMeterKernels<WF_METER_PEAK>
+                  : (cfg->mode == WF_METER_RMS) ? kMeterKernels<WF_METER_RMS>
+                                                 : kMeterKernels<WF_METER_INPUT_RMS>;
         const size_t S = (size_t)cfg->max_streams, hist_n = S * cfg->capture_channels * (size_t)W;
         int rc;
         for(auto &h : m->d_hist)
@@ -794,14 +810,9 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b_in, void *cuda_s
         return WF_OK;
     if(!b->pcm)
         return wf::fail(m, WF_ERR_INVALID_ARG, "pcm is null");
-    if(b->stream_stride < 0 || b->channel_stride < 0)
-        return wf::fail(m, WF_ERR_INVALID_ARG, "negative strides are not supported");
-    size_t sample_bytes = 0;
-    if(int rc = wf::pcm_sample_bytes(m, b->pcm_format, b->pcm, &sample_bytes))
+    wf::PcmBatch pb;
+    if(int rc = wf::check_pcm_batch(m, *b, m->cfg.capture_channels, m->W, &pb))
         return rc;
-    const bool s16 = b->pcm_format == WF_PCM_S16;
-    if((long long)b->n_ticks * b->hop > 0x7fffffffLL - m->W)
-        return wf::fail(m, WF_ERR_INVALID_ARG, "n_ticks * hop too large for one call");
 
     WF_CHECK(m, cudaSetDevice(m->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->stream;
@@ -830,9 +841,8 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b_in, void *cuda_s
     if((rc = m->d_raw.reserve(m, S * T * pc)))
         return rc;
     // a call with host buffers (told by pcm alone) is staged through device memory; the RMS feed has no dB / silent outputs
-    const size_t span = (S - 1) * (size_t)b->stream_stride + (size_t)(cc - 1) * (size_t)b->channel_stride + T * (size_t)b->hop;
     wf::Staging io(m, st, !wf::is_device_ptr(b->pcm));
-    const float *d_pcm = io.in_bytes(m->s_pcm, b->pcm, span * sample_bytes);
+    wf::PcmView pcm{io.in_bytes(m->s_pcm, b->pcm, pb.span * pb.sample_bytes), b->stream_stride, b->channel_stride};
     float *d_db = io.out(m->s_db, is_feed ? nullptr : b->out_db, out_n);
     float *d_lin = io.out(m->s_lin, b->out_lin, out_n);
     unsigned char *d_silent = io.out(m->s_silent, is_feed ? nullptr : b->out_silent, S * T);
@@ -844,34 +854,18 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b_in, void *cuda_s
     const size_t slot = (size_t)b->first_stream;
     WF_CHECK(m, wf::time_begin(m, st));
     // with a sync offset the kernels read (line ++ new)[0 .. T*hop) and the line keeps the last D samples (wf_splice.hpp)
-    long long stream_stride = b->stream_stride, channel_stride = b->channel_stride;
     if(m->D > 0)
     {
-        const long long tl = (long long)T * b->hop, wl = std::max<long long>(tl, m->D), cs = wf::splice_stride(wl, s16);
-        if((rc = m->s_window.reserve(m, (S * cc * (size_t)cs * sample_bytes + 3) / 4)))
+        const long long tl = (long long)T * b->hop;
+        if((rc = wf::splice_holdback(m, m->d_line + slot * cc * m->D, m->D, (int)S, cc, tl, std::max<long long>(tl, m->D),
+                                     pb.s16, m->s_window, pcm, st)))
             return rc;
-        wf::Splice sp{};
-        sp.hist = m->d_line + slot * cc * m->D;
-        sp.win = m->s_window.p;
-        sp.pcm = d_pcm;
-        sp.stream_stride = b->stream_stride;
-        sp.channel_stride = b->channel_stride;
-        sp.win_cs = cs;
-        sp.ws = 0;
-        sp.wl = wl;
-        sp.L = tl;
-        sp.R = m->D;
-        WF_CHECK(m, wf::launch_splice(sp, (int)S, cc, s16, st));
-        m->launches += 1;
-        d_pcm = m->s_window;
-        stream_stride = cc * cs;
-        channel_stride = cs;
     }
 
     MParams p{};
-    p.pcm = d_pcm;
-    p.stream_stride = stream_stride;
-    p.channel_stride = channel_stride;
+    p.pcm = pcm.pcm;
+    p.stream_stride = pcm.stream_stride;
+    p.channel_stride = pcm.channel_stride;
     p.ring[0] = m->d_hist[0] + slot * cc * W;
     p.ring[1] = m->d_hist[1] + slot * cc * W;
     p.par = m->d_par + slot;
@@ -915,11 +909,12 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b_in, void *cuda_s
     constexpr int kWarps = 8;
     // 4-sample group loads (128-bit for float, 64-bit for int16) need rows aligned to 4 samples (W is a multiple of 16
     // samples already).  The facts are stated in samples, so an int16 call takes the float call's path and summation order.
-    const int vec4 = (((uintptr_t)d_pcm & (4 * sample_bytes - 1)) == 0) && ((stream_stride & 3) == 0) &&
-                     ((channel_stride & 3) == 0);
+    const int vec4 = (((uintptr_t)pcm.pcm & (4 * pb.sample_bytes - 1)) == 0) && ((pcm.stream_stride & 3) == 0) &&
+                     ((pcm.channel_stride & 3) == 0);
     // one-pass path: the window is a whole number of hops (meter_fused_kernel)
     const size_t fused_smem = ((size_t)pc * ((size_t)(W / b->hop) + T) + T * pc) * sizeof(float);
     const bool fused = m->use_fused && vec4 && (W % b->hop) == 0 && (b->hop % 4) == 0 && fused_smem <= 96 * 1024;
+    const MeterKernels &k = m->kern[pb.s16];
     if(fused)
     {
         p.bl = b->hop;
@@ -936,57 +931,17 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b_in, void *cuda_s
             return rc;
         p.part = m->d_part + slot * p.part_stride;
         p.tag = (m->part_gen << 32) | b->hop;
-        auto launch = [&](auto kernel) -> cudaError_t {
-            if(fused_smem > 48 * 1024)
-            {
-                cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-                if(err != cudaSuccess)
-                    return err;
-            }
-            kernel<<<(int)S, 256, fused_smem, st>>>(p);
-            return cudaGetLastError();
-        };
-        auto launch_mode = [&](auto ts) -> cudaError_t {
-            using TS = decltype(ts);
-            switch(m->cfg.mode)
-            {
-            case WF_METER_PEAK: return launch(meter_fused_kernel<WF_METER_PEAK, TS>);
-            case WF_METER_RMS: return launch(meter_fused_kernel<WF_METER_RMS, TS>);
-            default: return launch(meter_fused_kernel<WF_METER_INPUT_RMS, TS>);
-            }
-        };
-        WF_CHECK(m, s16 ? launch_mode(int16_t{}) : launch_mode(float{}));
+        WF_CHECK(m, wf::launch_kernel(k.fused, m->device, (unsigned)S, 256, fused_smem, st, {}, p));
         m->launches += 1;
     }
     else
     {
-    const int g1 = grid_for((long long)S * pc * nchunk, kWarps, m->sm_count), g2 = grid_for((long long)S * T * pc, kWarps, m->sm_count);
-    auto launch_k12 = [&](auto ts) {
-        using TS = decltype(ts);
-        switch(m->cfg.mode)
-        {
-        case WF_METER_PEAK:
-            meter_block_kernel<WF_METER_PEAK, TS><<<g1, kWarps * 32, 0, st>>>(p, vec4);
-            meter_window_kernel<WF_METER_PEAK, TS><<<g2, kWarps * 32, 0, st>>>(p);
-            break;
-        case WF_METER_RMS:
-            meter_block_kernel<WF_METER_RMS, TS><<<g1, kWarps * 32, 0, st>>>(p, vec4);
-            meter_window_kernel<WF_METER_RMS, TS><<<g2, kWarps * 32, 0, st>>>(p);
-            break;
-        default:
-            meter_block_kernel<WF_METER_INPUT_RMS, TS><<<g1, kWarps * 32, 0, st>>>(p, vec4);
-            meter_window_kernel<WF_METER_INPUT_RMS, TS><<<g2, kWarps * 32, 0, st>>>(p);
-            break;
-        }
-    };
-    if(s16)
-        launch_k12(int16_t{});
-    else
-        launch_k12(float{});
-    WF_CHECK(m, cudaGetLastError());
-    meter_scan_kernel<<<(int)((S + 127) / 128), 128, 0, st>>>(p);
-    WF_CHECK(m, cudaGetLastError());
-    m->launches += 3;
+        const int g1 = grid_for((long long)S * pc * nchunk, kWarps, m->sm_count);
+        const int g2 = grid_for((long long)S * T * pc, kWarps, m->sm_count);
+        WF_CHECK(m, wf::launch_kernel(k.block, m->device, g1, kWarps * 32, 0, st, {}, p, vec4));
+        WF_CHECK(m, wf::launch_kernel(k.window, m->device, g2, kWarps * 32, 0, st, {}, p));
+        WF_CHECK(m, wf::launch_kernel(meter_scan_kernel, m->device, (unsigned)((S + 127) / 128), 128, 0, st, {}, p));
+        m->launches += 3;
     }
     WF_CHECK(m, wf::time_end(m, st));
     return io.finish();
@@ -1010,9 +965,9 @@ int wf_meter_reset(wf_meter *m, int32_t first, int32_t count)
     if(count == 0)
         return WF_OK;
     WF_CHECK(m, cudaSetDevice(m->device));
-    meter_reset_kernel<<<std::min(count, m->sm_count * 4), 256, 0, m->stream>>>(
-        m->d_hist[0], m->d_hist[1], m->d_par, m->d_ptag, m->d_buf, m->d_flags, first, count, m->cfg.capture_channels, m->W);
-    WF_CHECK(m, cudaGetLastError());
+    WF_CHECK(m, wf::launch_kernel(meter_reset_kernel, m->device, std::min(count, m->sm_count * 4), 256, 0, m->stream, {},
+                                  m->d_hist[0].p, m->d_hist[1].p, m->d_par.p, m->d_ptag.p, m->d_buf.p, m->d_flags.p, first,
+                                  count, m->cfg.capture_channels, m->W));
     m->launches++;
     WF_CHECK(m, cudaStreamSynchronize(m->stream));
     return WF_OK;
@@ -1062,11 +1017,8 @@ int meter_state(wf_meter *m, int32_t first, int32_t count, const float *ring, co
     q.D = m->D;
     const int grid = std::min(count, m->sm_count * 4);
     return io.run(m, m->stream, set, [&] {
-        if(set)
-            meter_state_kernel<true><<<grid, 256, 0, m->stream>>>(q);
-        else
-            meter_state_kernel<false><<<grid, 256, 0, m->stream>>>(q);
-        return cudaGetLastError();
+        return wf::launch_kernel(set ? meter_state_kernel<true> : meter_state_kernel<false>, m->device, grid, 256, 0,
+                                 m->stream, {}, q);
     });
 }
 

@@ -1,4 +1,5 @@
-// wf_splice.cu — history ++ new splice of wf_splice.hpp, shared by the spectrum, level-meter and waveform engines.
+// wf_splice.cu — history ++ new splice of wf_splice.hpp, shared by the spectrum, level-meter and waveform engines, and the
+// holdback call the level meter and the waveform make of it.
 #include "wf_splice.hpp"
 
 namespace wf {
@@ -84,6 +85,29 @@ cudaError_t launch_splice(const Splice &s, int streams, int cc, bool s16, cudaSt
     else
         history_splice_kernel<float><<<grid, 256, 0, st>>>(s);
     return cudaGetLastError();
+}
+
+int splice_holdback(HostCore *c, float *hist, int R, int streams, int cc, long long L, long long wl, bool s16,
+                    DevBuf<float> &window, PcmView &view, cudaStream_t st)
+{
+    const long long cs = splice_stride(wl, s16);
+    if(int rc = window.reserve(c, ((size_t)streams * cc * (size_t)cs * (s16 ? 2 : 4) + 3) / 4))
+        return rc;
+    Splice sp{};
+    sp.hist = hist;
+    sp.win = window.p;
+    sp.pcm = view.pcm;
+    sp.stream_stride = view.stream_stride;
+    sp.channel_stride = view.channel_stride;
+    sp.win_cs = cs;
+    sp.ws = 0;
+    sp.wl = wl;
+    sp.L = L;
+    sp.R = R;
+    WF_CHECK(c, launch_splice(sp, streams, cc, s16, st));
+    c->launches++;
+    view = {window.p, cc * cs, cs};
+    return WF_OK;
 }
 
 } // namespace wf

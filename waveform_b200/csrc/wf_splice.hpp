@@ -11,6 +11,7 @@
 
 #include <stdint.h>
 
+#include "wf_host.hpp"
 #include "wfstft.h"
 
 namespace wf {
@@ -45,6 +46,13 @@ inline long long splice_stride(long long len, bool s16)
     const long long q = s16 ? 8 : 4;
     return (len + q - 1) / q * q;
 }
+
+// The sync-offset holdback of the level meter and the waveform: the splice with ws = 0 and no start-up mask, for `streams`
+// x `cc` rows of `view` with L new samples each.  `hist` holds R samples per row from the call's first stream on; `window`
+// grows to the call's window of wl samples per row.  Counts the launch, then points `view` at the window, which the
+// engine's kernels read instead of the call's PCM.
+int splice_holdback(HostCore *c, float *hist, int R, int streams, int cc, long long L, long long wl, bool s16,
+                    DevBuf<float> &window, PcmView &view, cudaStream_t st);
 
 // The samples an audio sync offset of `ms` milliseconds holds back: ns_to_audio_frames(sample_rate, ms * 10^6) for a
 // positive offset (get_audio_sync > 0), else 0.

@@ -1207,14 +1207,18 @@ struct wf_wave : wf::HostCore {
     PlanSlot slots[kSlots];
     int slot_next = 0;
     cudaStream_t last_stream = nullptr;
-    bool chunked = true;  // wave_chunk_kernel (WF_WAVE_CHUNK=0: the per-tick kernel, kept for A/B and bit-identity tests)
-    int chunk_mode = 0, chunk_floats = 0, chunk_per_sm = 8;
+    // The kernel of a call, [display outputs][s16]: wave_chunk_kernel of the engine's channel layout, or with WF_WAVE_CHUNK=0
+    // the per-tick wave_kernel (kept for A/B and bit-identity tests).  The display entries exist with display settings only.
+    struct TickLaunch {
+        const void *kernel = nullptr;
+        size_t smem = 0; // dynamic shared memory before the Gaussian's scratch rows
+        int per_sm = 0;  // resident CTAs per SM: the grid is at most one wave of them
+    } tick[2][2];
     // display stage: only when the config carried display settings (current struct size) and width >= 2
     bool display = false;
     wf::Tables tab;
     wf::DevBuf<float> d_tab;      // interp weights | interp indices | Gaussian
     int disp_scratch = 0;         // floats of Gaussian scratch (dch * width, or 0 without the filter)
-    int disp_per_sm = 4;          // resident CTAs of the DISP chunk kernel
 };
 
 namespace {
@@ -1244,19 +1248,13 @@ bool wave_clock_ok(const wf_wave_config &c)
            ((uint64_t)c.meter_ms * 1000000ull) / (uint64_t)c.width != 0 && wf::sync_offset_ok(c.sync_offset_ms);
 }
 
-template<typename TS>
-const void *chunk_kernel_of(int mode, bool disp)
+// The tick kernel for parameters P and sample type TS: the chunk kernel of channel layout `mode`, or the per-tick kernel
+template<class P, typename TS>
+const void *tick_kernel(bool chunked, int mode)
 {
-    static const void *const k[2][4] = {
-        {(const void *)wave_chunk_kernel<0, WParams, TS>, (const void *)wave_chunk_kernel<1, WParams, TS>,
-         (const void *)wave_chunk_kernel<2, WParams, TS>, (const void *)wave_chunk_kernel<3, WParams, TS>},
-        {(const void *)wave_chunk_kernel<0, WDisp, TS>, (const void *)wave_chunk_kernel<1, WDisp, TS>,
-         (const void *)wave_chunk_kernel<2, WDisp, TS>, (const void *)wave_chunk_kernel<3, WDisp, TS>}};
-    return k[disp ? 1 : 0][mode];
-}
-const void *chunk_kernel(int mode, bool disp, bool s16)
-{
-    return s16 ? chunk_kernel_of<int16_t>(mode, disp) : chunk_kernel_of<float>(mode, disp);
+    static const void *const chunk[4] = {(const void *)wave_chunk_kernel<0, P, TS>, (const void *)wave_chunk_kernel<1, P, TS>,
+                                         (const void *)wave_chunk_kernel<2, P, TS>, (const void *)wave_chunk_kernel<3, P, TS>};
+    return chunked ? chunk[mode] : (const void *)wave_kernel<P, TS>;
 }
 
 // The tick-by-tick timestamp walk of tick_waveform for packets of `hop` samples that end "now" (wave_tick), on the host
@@ -1394,38 +1392,27 @@ int wf_wave_create_with_clock(const wf_wave_config *cfg_in, int32_t device_clock
         // the Gaussian's scratch rows follow the kernel's own shared memory in the DISP kernels
         w->disp_scratch = (display && w->tab.cfg.filter_mode == WF_FILTER_GAUSS) ? w->dch * cfg->width : 0;
         {
-            const int ring_bytes = (int)((2 * (size_t)cfg->width + w->disp_scratch) * sizeof(float));
-            if(ring_bytes > 48 * 1024) // widths above 6144: both scrolling rings exceed the default 48 KB
-            {
-                WF_CHECK(w, cudaFuncSetAttribute(wave_kernel<WParams, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * (size_t)cfg->width * sizeof(float))));
-                WF_CHECK(w, cudaFuncSetAttribute(wave_kernel<WParams, int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * (size_t)cfg->width * sizeof(float))));
-                if(display)
-                {
-                    WF_CHECK(w, cudaFuncSetAttribute(wave_kernel<WDisp, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, ring_bytes));
-                    WF_CHECK(w, cudaFuncSetAttribute(wave_kernel<WDisp, int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, ring_bytes));
-                }
-            }
-        }
-        {
-            w->chunked = wf::env_flag("WF_WAVE_CHUNK", true);
-            const bool two = cfg->capture_channels > 1;
-            w->chunk_mode = cfg->stereo ? (two ? 2 : 3) : (two ? 1 : 0);
-            static const int mult[4] = {2, 4, 4, 3};
-            w->chunk_floats = mult[w->chunk_mode] * cfg->width;
+            const bool chunked = wf::env_flag("WF_WAVE_CHUNK", true), two = cfg->capture_channels > 1;
+            const int mode = cfg->stereo ? (two ? 2 : 3) : (two ? 1 : 0); // the chunk kernel's channel layout
+            static const int mult[4] = {2, 4, 4, 3};                       // its floats per point; the per-tick kernel's: 2
+            const size_t smem = (size_t)(chunked ? mult[mode] : 2) * cfg->width * sizeof(float);
+            const void *const kernels[2][2] = {
+                {tick_kernel<WParams, float>(chunked, mode), tick_kernel<WParams, int16_t>(chunked, mode)},
+                {tick_kernel<WDisp, float>(chunked, mode), tick_kernel<WDisp, int16_t>(chunked, mode)}};
             for(int disp = 0; disp < (display ? 2 : 1); ++disp)
             {
-                const int bytes = (w->chunk_floats + (disp ? w->disp_scratch : 0)) * (int)sizeof(float);
-                int per_sm = 0;
-                for(const bool s16 : {false, true})
+                int per_sm = 8;
+                if(chunked)
                 {
-                    const void *k = chunk_kernel(w->chunk_mode, disp != 0, s16);
-                    if(bytes > 48 * 1024)
-                        WF_CHECK(w, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-                    if(!s16) // the float kernel's occupancy sizes the grid of both (one resident wave: streams are equal
-                             // work, a partial second wave is a tail)
-                        WF_CHECK(w, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, 256, (size_t)bytes));
+                    // the float kernel's occupancy sizes the grid of both (one resident wave: streams are equal work, a
+                    // partial second wave is a tail); the query needs the shared-memory limit raised first
+                    const size_t bytes = smem + (disp ? w->disp_scratch * sizeof(float) : 0);
+                    WF_CHECK(w, wf::opt_in_smem(kernels[disp][0], w->device, bytes));
+                    WF_CHECK(w, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernels[disp][0], 256, bytes));
+                    per_sm = std::max(1, per_sm);
                 }
-                (disp ? w->disp_per_sm : w->chunk_per_sm) = std::max(1, per_sm);
+                for(int s16 = 0; s16 < 2; ++s16)
+                    w->tick[disp][s16] = {kernels[disp][s16], smem, per_sm};
             }
         }
         int rc;
@@ -1505,14 +1492,9 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b_in, void *cuda_stre
         return WF_OK;
     if(!b->pcm || !(b->out || b->out_points || b->out_pixels))
         return wf::fail(w, WF_ERR_INVALID_ARG, "pcm is null, or none of out / out_points / out_pixels is set");
-    if(b->stream_stride < 0 || b->channel_stride < 0)
-        return wf::fail(w, WF_ERR_INVALID_ARG, "negative strides are not supported");
-    size_t sample_bytes = 0;
-    if(int rc = wf::pcm_sample_bytes(w, b->pcm_format, b->pcm, &sample_bytes))
+    wf::PcmBatch pb;
+    if(int rc = wf::check_pcm_batch(w, *b, w->cfg.capture_channels, w->D, &pb))
         return rc;
-    const bool s16 = b->pcm_format == WF_PCM_S16;
-    if((long long)b->n_ticks * b->hop > 0x7fffffffLL - w->D)
-        return wf::fail(w, WF_ERR_INVALID_ARG, "n_ticks * hop too large for one call");
     if(w->dev_clock && (long long)b->n_ticks * w->cfg.width > 0x7fffffffLL)
         return wf::fail(w, WF_ERR_INVALID_ARG, "n_ticks * width too large for one call");
 
@@ -1541,9 +1523,8 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b_in, void *cuda_stre
 
     // a call with host buffers (told by pcm alone) is staged through device memory
     const size_t out_n = S * T * w->dch * (size_t)W;
-    const size_t span = (S - 1) * (size_t)b->stream_stride + (size_t)(cc - 1) * (size_t)b->channel_stride + T * (size_t)b->hop;
     wf::Staging io(w, st, !wf::is_device_ptr(b->pcm));
-    const float *d_pcm = io.in_bytes(w->s_pcm, b->pcm, span * sample_bytes);
+    wf::PcmView pcm{io.in_bytes(w->s_pcm, b->pcm, pb.span * pb.sample_bytes), b->stream_stride, b->channel_stride};
     const float *d_rms = io.in(w->s_rms, b->input_rms, S * T);
     float *d_out = io.out(w->s_out, b->out, out_n);
     float *d_points = io.out(w->s_points, b->out_points, out_n);
@@ -1554,40 +1535,23 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b_in, void *cuda_stre
         return io.rc;
     WF_CHECK(w, wf::time_begin(w, st));
     // with a sync offset the plan indexes into holdback ++ new, and the holdback keeps the last D samples (wf_splice.hpp)
-    long long stream_stride = b->stream_stride, channel_stride = b->channel_stride;
     if(w->D > 0)
     {
-        const long long wl = (long long)w->D + (long long)T * b->hop, cs = wf::splice_stride(wl, s16);
-        if((rc = w->s_window.reserve(w, (S * cc * (size_t)cs * sample_bytes + 3) / 4)))
+        const long long tl = (long long)T * b->hop;
+        if((rc = wf::splice_holdback(w, w->d_hold, w->D, (int)S, cc, tl, w->D + tl, pb.s16, w->s_window, pcm, st)))
             return rc;
-        wf::Splice sp{};
-        sp.hist = w->d_hold;
-        sp.win = w->s_window.p;
-        sp.pcm = d_pcm;
-        sp.stream_stride = b->stream_stride;
-        sp.channel_stride = b->channel_stride;
-        sp.win_cs = cs;
-        sp.ws = 0;
-        sp.wl = wl;
-        sp.L = (long long)T * b->hop;
-        sp.R = w->D;
-        WF_CHECK(w, wf::launch_splice(sp, (int)S, cc, s16, st));
-        w->launches++;
-        d_pcm = w->s_window;
-        stream_stride = cc * cs;
-        channel_stride = cs;
     }
     if(w->dev_clock)
     {
         const WaveWalk k = wave_walk(w->cfg, w->ws, (uint64_t)w->D, b->hop);
-        wave_plan_kernel<<<1, kPlanThreads, 0, st>>>(w->d_clock, k, b->n_ticks, w->d_off, w->d_src, w->d_ticks);
-        WF_CHECK(w, cudaGetLastError());
+        WF_CHECK(w, wf::launch_kernel(wave_plan_kernel, w->device, 1, kPlanThreads, 0, st, {}, w->d_clock.p, k, b->n_ticks,
+                                      w->d_off.p, w->d_src.p, w->d_ticks.p));
         w->launches++;
     }
     WParams p{};
-    p.pcm = d_pcm;
-    p.stream_stride = stream_stride;
-    p.channel_stride = channel_stride;
+    p.pcm = pcm.pcm;
+    p.stream_stride = pcm.stream_stride;
+    p.channel_stride = pcm.channel_stride;
     p.input_rms = d_rms;
     p.src = w->d_src;
     p.off = w->d_off;
@@ -1606,6 +1570,7 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b_in, void *cuda_stre
     p.vol_target = w->cfg.volume_target;
     p.max_gain = w->cfg.max_gain;
     p.db_min = w->db_min;
+    const wf_wave::TickLaunch &l = w->tick[disp][pb.s16];
     WDisp pd{};
     if(disp)
     {
@@ -1625,26 +1590,14 @@ int wf_wave_process_async(wf_wave *w, const wf_wave_batch *b_in, void *cuda_stre
         pd.dbrange_f = (float)(t.cfg.ceiling_db - t.cfg.floor_db);
         pd.px_hi = t.px_hi;
         pd.px_cpos = t.px_cpos;
-        pd.scratch_off = w->chunked ? w->chunk_floats : 2 * W;
+        pd.scratch_off = (int)(l.smem / sizeof(float));
         pd.vec4 = ((W & 3) == 0) && ((reinterpret_cast<uintptr_t>(d_points) & 15) == 0) &&
                   ((reinterpret_cast<uintptr_t>(d_pixels) & 15) == 0);
     }
-    const int per_sm = w->chunked ? (disp ? w->disp_per_sm : w->chunk_per_sm) : 8;
-    const int grid = (int)std::min<size_t>(S, (size_t)w->sm_count * per_sm);
+    const int grid = (int)std::min<size_t>(S, (size_t)w->sm_count * l.per_sm);
     const size_t scratch = disp ? (size_t)w->disp_scratch * sizeof(float) : 0;
     void *args[] = {disp ? (void *)&pd : (void *)&p};
-    if(w->chunked)
-        WF_CHECK(w, cudaLaunchKernel(chunk_kernel(w->chunk_mode, disp, s16), dim3(grid), dim3(256), args,
-                                     (size_t)w->chunk_floats * sizeof(float) + scratch, st));
-    else if(disp && s16)
-        wave_kernel<WDisp, int16_t><<<grid, 256, 2 * (size_t)W * sizeof(float) + scratch, st>>>(pd);
-    else if(disp)
-        wave_kernel<WDisp, float><<<grid, 256, 2 * (size_t)W * sizeof(float) + scratch, st>>>(pd);
-    else if(s16)
-        wave_kernel<WParams, int16_t><<<grid, 256, 2 * (size_t)W * sizeof(float), st>>>(p);
-    else
-        wave_kernel<WParams, float><<<grid, 256, 2 * (size_t)W * sizeof(float), st>>>(p);
-    WF_CHECK(w, cudaGetLastError());
+    WF_CHECK(w, wf::launch_kernel(l.kernel, w->device, grid, 256, l.smem + scratch, st, {}, args));
     w->launches++;
     WF_CHECK(w, wf::time_end(w, st));
     return io.finish();
@@ -1664,10 +1617,9 @@ int wf_wave_reset(wf_wave *w)
     if(!w)
         return WF_ERR_INVALID_ARG;
     WF_CHECK(w, cudaSetDevice(w->device));
-    wave_reset_kernel<<<std::min(w->cfg.max_streams, w->sm_count * 4), 256, 0, w->stream>>>(w->d_state, w->d_flags,
-                                                                                          w->cfg.max_streams, w->dch,
-                                                                                          w->cfg.width, w->db_min);
-    WF_CHECK(w, cudaGetLastError());
+    WF_CHECK(w, wf::launch_kernel(wave_reset_kernel, w->device, std::min(w->cfg.max_streams, w->sm_count * 4), 256, 0,
+                                  w->stream, {}, w->d_state.p, w->d_flags.p, w->cfg.max_streams, w->dch, w->cfg.width,
+                                  w->db_min));
     w->launches++;
     WF_CHECK(w, cudaStreamSynchronize(w->stream));
     return WF_OK;
@@ -1717,11 +1669,8 @@ int wave_state(wf_wave *w, int32_t first, int32_t count, const float *db, const 
     q.D = w->D;
     const int grid = std::min(count, w->sm_count * 4);
     return io.run(w, w->stream, set, [&] {
-        if(set)
-            wave_state_kernel<true><<<grid, 256, 0, w->stream>>>(q);
-        else
-            wave_state_kernel<false><<<grid, 256, 0, w->stream>>>(q);
-        return cudaGetLastError();
+        return wf::launch_kernel(set ? wave_state_kernel<true> : wave_state_kernel<false>, w->device, grid, 256, 0,
+                                 w->stream, {}, q);
     });
 }
 
