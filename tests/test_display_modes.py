@@ -16,8 +16,11 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from gpu_common import clean_knobs, set_knobs  # noqa: F401 (fixture)
 from helpers import synth_pcm
 from refdata import digest
+
+pytestmark = pytest.mark.usefixtures("clean_knobs")
 
 ROOT = Path(__file__).resolve().parents[1]
 STORE = Path(__file__).resolve().parent / "golden" / "reference_display.npz"
@@ -364,7 +367,7 @@ def _wave_runs(settings, ch, hop, S, T, monkeypatch, chunk, want_db=True):
     pcm, rms = _case(settings, ch, hop, T, S)
     pcm[1] = 0.0
     pcm[2, :, : 30 * hop] = 1.0
-    monkeypatch.setenv("WF_WAVE_CHUNK", chunk)
+    set_knobs(monkeypatch, {"WF_WAVE_CHUNK": chunk})
     eng = WaveEngine(settings, channels=ch, max_streams=S)
     parts = [eng.process(pcm[:, :, : 13 * hop], 13, hop, input_rms=None if rms is None else rms[:, :13], want_db=want_db,
                          want_points=True, want_pixels=True),
@@ -401,7 +404,7 @@ def test_gpu_meter_display_vs_restatement(settings, ch, hop, fused, monkeypatch)
     import torch
     from waveform_b200 import MeterEngine
 
-    monkeypatch.setenv("WF_METER_FUSED", fused)
+    set_knobs(monkeypatch, {"WF_METER_FUSED": fused})
     S, T = 6, 30
     pcm = synth_pcm(S, ch, T * hop, seed=5)
     pcm[1] = 0.0

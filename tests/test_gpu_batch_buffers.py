@@ -12,7 +12,9 @@ from __future__ import annotations
 import numpy as np
 import pytest
 
-pytestmark = pytest.mark.gpu
+from gpu_common import clean_knobs  # noqa: F401 (fixture)
+
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 
 N, HOP, T, S = 2048, 1024, 48, 1100
 SETTINGS = {"fft_size": N, "normalize_volume": True, "volume_target": -12.0, "max_gain": 20.0,

@@ -4,16 +4,17 @@ from __future__ import annotations
 
 import pytest
 
+from gpu_common import clean_knobs, set_knobs  # noqa: F401 (fixture)
 from helpers import device_pcm, parity_report
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 
 
 def test_fast2048_unaligned_output_takes_generic_kernel(monkeypatch):
     import torch
     from waveform_b200 import Engine
 
-    monkeypatch.setenv("WF_TEAM_W", "1")  # keep the aligned run on the warp-per-stream kernel at this stream count
+    set_knobs(monkeypatch, {"WF_TEAM_W": "1"})  # keep the aligned run on the warp-per-stream kernel at this stream count
     S, T, N, B = 300, 4, 2048, 1024
     settings = {"fft_size": N, "window": "hann", "gravity": 0.65}
     pcm = device_pcm(S, 1, T * N, seed=2048)

@@ -22,46 +22,22 @@ import numpy as np
 import pytest
 
 from fp64_spectrum import Fp64Spectrum, compare, normwise_vs_truth
+from gpu_common import CATALOGUE, FAMILIES, clean_knobs, route_id, set_knobs  # noqa: F401 (fixture)
 from helpers import synth_pcm
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 
 GOLDEN = Path(__file__).parent / "golden"
 T = 8               # ticks per run, in two calls of 4
 
-FAMILIES = ["stft2048_fast_kernel", "stft2048_team_kernel", "stft_warp2_kernel", "stft_warp2_kernel/display",
-            "stft_v3_kernel", "stft16384_parity_kernel", "stft_wide_kernel", "stft_fused_kernel",
-            "stft_anyn_kernel/smem", "stft_anyn_kernel/L2"]
-
-# (family, N, channels, stereo, environment, display outputs)
-ROUTES = [
-    ("stft2048_fast_kernel", 2048, 1, False, {"WF_TEAM_W": "1"}, False),
-    ("stft2048_team_kernel", 2048, 1, False, {"WF_TEAM_W": "4"}, False),
-    *[("stft_warp2_kernel", n, 1, False, {}, False) for n in (800, 1456, 1664, 1408, 1792)],
-    *[("stft_warp2_kernel/display", n, 1, False, {}, True) for n in (800, 1456, 1024)],
-    ("stft_v3_kernel", 1024, 1, False, {}, False),
-    ("stft_v3_kernel", 2048, 1, False, {"WF_FORCE_GENERIC": "1"}, False),
-    ("stft_v3_kernel", 4096, 2, True, {}, False),
-    ("stft_v3_kernel", 4096, 2, False, {}, False),
-    ("stft_v3_kernel", 8192, 1, False, {}, False),
-    ("stft_v3_kernel", 16384, 1, False, {"WF_PAR16384": "0"}, False),
-    ("stft16384_parity_kernel", 16384, 1, False, {}, False),
-    ("stft_wide_kernel", 4096, 1, False, {"WF_V3": "0", "WF_WIDE_R": "2"}, False),
-    ("stft_wide_kernel", 32768, 1, False, {"WF_WIDE_R": "2"}, False),
-    *[("stft_fused_kernel", n, 1, False, {}, False) for n in (128, 256, 512)],
-    ("stft_fused_kernel", 2048, 1, False, {"WF_FORCE_GENERIC": "1", "WF_V3": "0", "WF_WIDE_R": "1"}, False),
-    ("stft_fused_kernel", 32768, 1, False, {"WF_WIDE_R": "1"}, False),
-    *[("stft_anyn_kernel/smem", n, 1, False, {"WF_WARP2": "0"}, False) for n in (800, 1456, 1664)],
-    ("stft_anyn_kernel/smem", 8128, 1, False, {}, False),
-    *[("stft_anyn_kernel/L2", n, 1, False, {}, False) for n in (40000, 65344, 65488, 65536)],
-]
+ROUTES = [CATALOGUE[k] for k in (
+    "fast-2048", "team-2048", "warp2-800", "warp2-1456", "warp2-1664", "warp2-1408", "warp2-1792",
+    "warp2-800-display", "warp2-1456-display", "warp2-1024-display", "v3-1024", "v3-2048-generic", "v3-4096-stereo",
+    "v3-4096-mix", "v3-8192", "v3-16384", "parity-16384", "wide-4096", "wide-32768", "fused-128", "fused-256",
+    "fused-512", "fused-2048", "fused-32768", "smem-800", "smem-1456", "smem-1664", "smem-8128", "l2-40000",
+    "l2-65344", "l2-65488", "l2-65536")]
 
 SEEN: dict[str, list] = {}      # family -> [(N, max error against float64, error of the reference)]
-
-
-def _route_id(r):
-    fam, N, cc, stereo, env, disp = r
-    return f"{fam.replace('/', '-')}-{N}{'-stereo' if stereo else ('-mix' if cc == 2 else '')}"
 
 
 def _yardstick(N):
@@ -108,16 +84,13 @@ def _options(N, all_options):
             True)
 
 
-@pytest.mark.parametrize("route", ROUTES, ids=[_route_id(r) for r in ROUTES])
+@pytest.mark.parametrize("route", ROUTES, ids=[route_id(r) for r in ROUTES])
 def test_kernel_against_float64(route, monkeypatch):
     import torch
     from waveform_b200 import Engine
 
     fam, N, cc, stereo, env, disp = route
-    for k in ("WF_TEAM_W", "WF_WIDE_R", "WF_V3", "WF_PAR16384", "WF_WARP2", "WF_WARP2_DISPLAY", "WF_FORCE_GENERIC"):
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+    set_knobs(monkeypatch, env)
     yard = _yardstick(N)
     hops = sorted({N, N // 4} | ({800} if N >= 1024 else set()), reverse=True)
     worst = 0.0
@@ -186,10 +159,7 @@ def test_every_kernel_family_ran(monkeypatch):
 
     seen = set()
     for fam, N, cc, stereo, env, disp in ROUTES:
-        for k in ("WF_TEAM_W", "WF_WIDE_R", "WF_V3", "WF_PAR16384", "WF_WARP2", "WF_WARP2_DISPLAY", "WF_FORCE_GENERIC"):
-            monkeypatch.delenv(k, raising=False)
-        for k, v in env.items():
-            monkeypatch.setenv(k, v)
+        set_knobs(monkeypatch, env)
         settings = {"fft_size": N, **({"channel_mode": "stereo"} if stereo else {})}
         eng = Engine(settings, channels=cc, max_streams=2)
         x = torch.from_numpy(synth_pcm(2, cc, 3 * N + N)).cuda()
@@ -217,7 +187,7 @@ def test_meter_rms_against_float64(kind, hop, fused, monkeypatch):
     from waveform_b200 import MeterEngine
     from waveform_b200.engine import METER_INPUT_RMS
 
-    monkeypatch.setenv("WF_METER_FUSED", fused)
+    set_knobs(monkeypatch, {"WF_METER_FUSED": fused})
     S, ch, n_ticks = 3, 2, 2000
     settings = {} if kind == "feed" else {"meter_buf": 1000, "rms_mode": True, "temporal_smoothing": "none"}
     eng = MeterEngine(settings, channels=ch, max_streams=S, mode=METER_INPUT_RMS if kind == "feed" else None)

@@ -9,9 +9,10 @@ import numpy as np
 import pytest
 
 from helpers import parity_report, synth_pcm
+from gpu_common import clean_knobs  # noqa: F401 (fixture)
 from refdata import frame_peak, reference, sample_index
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 ROOT = Path(__file__).resolve().parents[1]
 
 

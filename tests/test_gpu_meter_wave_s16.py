@@ -17,7 +17,9 @@ import ctypes as C
 import numpy as np
 import pytest
 
-pytestmark = pytest.mark.gpu
+from gpu_common import assert_bits_equal, clean_knobs, set_knobs, to_host  # noqa: F401 (fixture)
+
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 
 SCALE = np.float32(2.0 ** -15)
 
@@ -43,18 +45,6 @@ def _signals(S, cc, ns, seed, zero_ticks=None):
 
 def _f32(x):
     return x.astype(np.float32) * SCALE
-
-
-def _np(d):
-    return {k: (v.cpu().numpy() if hasattr(v, "cpu") else v) for k, v in d.items()}
-
-
-def _bits_equal(a, b, ctx):
-    a, b = _np(a), _np(b)
-    assert a.keys() == b.keys(), ctx
-    for k in a:
-        assert a[k].dtype == b[k].dtype and a[k].shape == b[k].shape, (k, ctx)
-        assert np.array_equal(a[k].view(np.uint8), b[k].view(np.uint8)), (k, ctx)
 
 
 def _dev(x, offset=0):
@@ -97,7 +87,7 @@ def _meter_call(eng, x, T, hop, fmt, offset, seconds, want_pixels):
     import torch
 
     torch.cuda.synchronize()
-    return _np(out), eng.launch_count - before
+    return to_host(out), eng.launch_count - before
 
 
 @pytest.mark.parametrize("opts", ["plain", "fastpeaks-tvexp", "reset"])
@@ -106,7 +96,7 @@ def _meter_call(eng, x, T, hop, fmt, offset, seconds, want_pixels):
 @pytest.mark.parametrize("mode", list(METER_MODES))
 def test_meter_s16_matches_f32_bit_for_bit(mode, cc, path, opts, monkeypatch):
     hop, fused, extra, offset, launches = METER_PATHS[path]
-    monkeypatch.setenv("WF_METER_FUSED", fused)
+    set_knobs(monkeypatch, {"WF_METER_FUSED": fused})
     S, T = 5, 12 if mode != "feed" else 16
     settings = {"fast_peaks": True, "temporal_smoothing": "tv_exp_moving_avg"} if opts == "fastpeaks-tvexp" else None
     e16, e32 = _meter_pair(mode, cc, S, settings)
@@ -119,7 +109,7 @@ def test_meter_s16_matches_f32_bit_for_bit(mode, cc, path, opts, monkeypatch):
         g16, n16 = _meter_call(e16, xs, T, hop, "s16", offset, secs[k], want_pixels)
         g32, n32 = _meter_call(e32, _f32(xs), T, hop, "f32", offset, secs[k], want_pixels)
         ctx = (mode, cc, path, opts, k)
-        _bits_equal(g16, g32, ctx)
+        assert_bits_equal(g16, g32, ctx)
         assert n16 == n32 == launches, (n16, n32, ctx)
         if opts == "reset" and k == 0:
             for e in (e16, e32):
@@ -129,7 +119,7 @@ def test_meter_s16_matches_f32_bit_for_bit(mode, cc, path, opts, monkeypatch):
     x3 = _f32(_signals(S, cc, T * hop + extra, seed=7))
     g16, _ = _meter_call(e16, x3, T, hop, "f32", offset, secs[0], want_pixels)
     g32, _ = _meter_call(e32, x3, T, hop, "f32", offset, secs[0], want_pixels)
-    _bits_equal(g16, g32, (mode, cc, path, opts, "state"))
+    assert_bits_equal(g16, g32, (mode, cc, path, opts, "state"))
 
 
 def test_meter_formats_alternated_on_one_engine():
@@ -142,7 +132,7 @@ def test_meter_formats_alternated_on_one_engine():
             xs = np.ascontiguousarray(x[:, :, k * T * hop: (k + 1) * T * hop])
             a, _ = _meter_call(mixed, xs if fmt == "s16" else _f32(xs), T, hop, fmt, 0, 1 / 60, mode != "feed")
             b, _ = _meter_call(ref, _f32(xs), T, hop, "f32", 0, 1 / 60, mode != "feed")
-            _bits_equal(a, b, (mode, k, fmt))
+            assert_bits_equal(a, b, (mode, k, fmt))
 
 
 def test_meter_buffer_kinds():
@@ -159,8 +149,8 @@ def test_meter_buffer_kinds():
             pinned = torch.from_numpy(xs).pin_memory()
             pin = engines[1].process(pinned.numpy(), T, hop, pcm_format="s16", want_pixels=mode != "feed")
             page = engines[2].process(xs, T, hop, pcm_format="s16", want_pixels=mode != "feed")
-            _bits_equal(pin, dev, (mode, "pinned", k))
-            _bits_equal(page, dev, (mode, "pageable", k))
+            assert_bits_equal(pin, dev, (mode, "pinned", k))
+            assert_bits_equal(page, dev, (mode, "pageable", k))
 
 
 # ---- waveform -------------------------------------------------------------------------------------------------------
@@ -195,7 +185,7 @@ def _wave_call(eng, x, T, hop, fmt, rms, display, device=True):
     out = eng.process(pcm, T, hop, input_rms=r, want_points=disp, want_pixels=disp, pcm_format=fmt)
     torch.cuda.synchronize()
     assert eng.launch_count - before == 1
-    return _np(out)
+    return to_host(out)
 
 
 @pytest.mark.parametrize("normalize", [False, True], ids=["plain", "normalized"])
@@ -203,7 +193,7 @@ def _wave_call(eng, x, T, hop, fmt, rms, display, device=True):
 @pytest.mark.parametrize("chunk", ["1", "0"], ids=["chunked", "per-tick"])
 @pytest.mark.parametrize("layout", list(WAVE_LAYOUTS))
 def test_wave_s16_matches_f32_bit_for_bit(layout, chunk, display, normalize, monkeypatch):
-    monkeypatch.setenv("WF_WAVE_CHUNK", chunk)
+    set_knobs(monkeypatch, {"WF_WAVE_CHUNK": chunk})
     S, T, hop = 5, 24, 800
     e16, e32, cc = _wave_pair(layout, display, normalize, S)
     x = _signals(S, cc, 2 * T * hop, seed=cc * 100 + len(display))
@@ -218,14 +208,14 @@ def test_wave_s16_matches_f32_bit_for_bit(layout, chunk, display, normalize, mon
         r = None if rms is None else np.ascontiguousarray(rms[:, k * T: (k + 1) * T])
         g16 = _wave_call(e16, xs, T, hop, "s16", r, display)
         g32 = _wave_call(e32, _f32(xs), T, hop, "f32", r, display)
-        _bits_equal(g16, g32, (layout, chunk, display, normalize, k))
+        assert_bits_equal(g16, g32, (layout, chunk, display, normalize, k))
         if k == 0:
             # (volume normalisation adds its gain to the 0 dB entries, so they are no longer 0.0f)
             assert g16["silent"][1].any() == (layout != "mix" and not normalize) and not g16["silent"][0].any()
     x3 = _f32(_signals(S, cc, T * hop, seed=9))
     r3 = None if rms is None else np.ascontiguousarray(rms[:, :T])
-    _bits_equal(_wave_call(e16, x3, T, hop, "f32", r3, display), _wave_call(e32, x3, T, hop, "f32", r3, display),
-                (layout, chunk, display, normalize, "state"))
+    assert_bits_equal(_wave_call(e16, x3, T, hop, "f32", r3, display), _wave_call(e32, x3, T, hop, "f32", r3, display),
+                      (layout, chunk, display, normalize, "state"))
 
 
 def test_wave_formats_alternated_and_buffer_kinds():
@@ -243,7 +233,7 @@ def test_wave_formats_alternated_and_buffer_kinds():
             xs = np.ascontiguousarray(x[:, :, k * T * hop: (k + 1) * T * hop])
             a = _wave_call(mixed, xs if fmt == "s16" else _f32(xs), T, hop, fmt, None, "catmull-rom-gauss")
             b = _wave_call(ref, _f32(xs), T, hop, "f32", None, "catmull-rom-gauss")
-            _bits_equal(a, b, (layout, k, fmt))
+            assert_bits_equal(a, b, (layout, k, fmt))
             if fmt == "s16":
                 pinned = torch.from_numpy(xs).pin_memory()
                 p = _wave_call(pin_e, pinned.numpy(), T, hop, "s16", None, "catmull-rom-gauss", device=False)
@@ -251,8 +241,8 @@ def test_wave_formats_alternated_and_buffer_kinds():
             else:
                 p = _wave_call(pin_e, _f32(xs), T, hop, "f32", None, "catmull-rom-gauss", device=False)
                 q = _wave_call(page_e, _f32(xs), T, hop, "f32", None, "catmull-rom-gauss", device=False)
-            _bits_equal(p, a, (layout, k, "pinned"))
-            _bits_equal(q, a, (layout, k, "pageable"))
+            assert_bits_equal(p, a, (layout, k, "pinned"))
+            assert_bits_equal(q, a, (layout, k, "pageable"))
 
 
 # ---- the volume-normalisation chain, fully in int16 -------------------------------------------------------------------
@@ -281,8 +271,8 @@ def test_normalization_chain_all_int16():
             outs.append({"rms": rms, **{f"spec_{a}": b for a, b in sp.items()}, **{f"wave_{a}": b for a, b in wv.items()}})
         chains[fmt] = outs
     for k in range(2):
-        _bits_equal(chains["s16"][k], chains["f32"][k], ("chain", k))
-    assert np.isfinite(_np(chains["s16"][1])["spec_db"]).all()
+        assert_bits_equal(chains["s16"][k], chains["f32"][k], ("chain", k))
+    assert np.isfinite(to_host(chains["s16"][1])["spec_db"]).all()
 
 
 # ---- ABI ------------------------------------------------------------------------------------------------------------
@@ -344,4 +334,4 @@ def test_meter_wave_numpy_int16_without_keyword_stays_unscaled():
     for mk in (lambda: _meter_pair("rms", 2, 2)[0], lambda: _wave_pair("mix", "none", False, 2)[0]):
         a = mk().process(x, 8, 800)
         b = mk().process(x.astype(np.float32), 8, 800)
-        _bits_equal(a, b, "int16 numpy without pcm_format")
+        assert_bits_equal(a, b, "int16 numpy without pcm_format")

@@ -12,26 +12,11 @@ from __future__ import annotations
 import numpy as np
 import pytest
 
+from gpu_common import assert_bits_equal, bits, capture, clean_knobs, replay, set_knobs  # noqa: F401 (fixture)
 from helpers import synth_pcm
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 SR = 48000
-
-
-def _bits(a):
-    return np.ascontiguousarray(a).view(np.uint8)
-
-
-def _host(out):
-    return {k: (v.cpu().numpy() if hasattr(v, "cpu") else np.array(v)) for k, v in out.items() if v is not None}
-
-
-def _assert_same(got, want, what):
-    got, want = _host(got), _host(want)
-    assert got.keys() == want.keys(), what
-    for k in want:
-        assert got[k].shape == want[k].shape, (what, k)
-        assert np.array_equal(_bits(got[k]), _bits(want[k])), (what, k)
 
 
 def _slots(out, lo, hi):
@@ -86,15 +71,6 @@ def _meter_call(e, x, T, hop, fmt, first=0):
     return e.process(x, T, hop, first_stream=first, pcm_format=fmt, want_pixels=e.cfg.mode != METER_INPUT_RMS)
 
 
-def _assert_same_state(sa, sb, what):
-    assert sa.keys() == sb.keys(), what
-    for k in sa:
-        if sa[k] is None:
-            assert sb[k] is None, (what, k)
-        else:
-            assert sa[k].shape == sb[k].shape and np.array_equal(_bits(sa[k]), _bits(sb[k])), (what, k)
-
-
 @pytest.mark.parametrize("dest", ["fresh", "used"])
 @pytest.mark.parametrize("fused", [True, False], ids=["fused", "three-kernel"])
 @pytest.mark.parametrize("calls", list(METER_CALLS), ids=list(METER_CALLS))
@@ -104,7 +80,7 @@ def test_meter_split_run(name, settings, mode, cc, fmt, calls, fused, dest, monk
     rings are in the second half and, on the one-pass path, their partials are valid for c3's hop.  The restore must write
     the half the parity selects and drop those partials, or B's c3 reads B's own earlier audio."""
     if not fused:
-        monkeypatch.setenv("WF_METER_FUSED", "0")
+        set_knobs(monkeypatch, {"WF_METER_FUSED": "0"})
     S, first = 3, 2
     a, b = _meter_pair(settings, mode, cc, S, S + 4)
     schedule = METER_CALLS[calls]
@@ -121,8 +97,8 @@ def test_meter_split_run(name, settings, mode, cc, fmt, calls, fused, dest, monk
                 assert state["flags"][1] == 1  # a silent stream crosses the checkpoint
             b.set_state(state, first_stream=first)
         if i >= 2:
-            _assert_same(_meter_call(b, xs[i], T, hop, fmt, first=first), want, (name, calls, dest, i))
-    _assert_same_state(b.get_state(first, S), a.get_state(), (name, calls, dest, "final"))
+            assert_bits_equal(_meter_call(b, xs[i], T, hop, fmt, first=first), want, (name, calls, dest, i))
+    assert_bits_equal(b.get_state(first, S), a.get_state(), (name, calls, dest, "final"))
 
 
 # ---- waveform: split runs ---------------------------------------------------------------------------------------------
@@ -182,8 +158,8 @@ def test_wave_split_run(name, settings, cc, fmt, want, clock_a, clock_b):
         if i >= 2:
             y, r = _embed(x, rms, first, S_b, 300 + i, fmt, settings)
             got = b.process(y, T, hop, input_rms=r, pcm_format=fmt, **want)
-            _assert_same(_slots(got, first, first + S), ref, (name, i))
-    _assert_same_state(b.get_state(first, S), a.get_state(), (name, "final"))
+            assert_bits_equal(_slots(got, first, first + S), ref, (name, i))
+    assert_bits_equal(b.get_state(first, S), a.get_state(), (name, "final"))
     assert b.get_clock() == a.get_clock()
 
 
@@ -201,7 +177,7 @@ def test_wave_migration_into_a_busy_engine():
         src.process(_samples(2, cc, T * hop, 400 + i, fmt), T, hop)
     for i, (T, hop) in enumerate([(2, 97), (5, 800), (1, 3000)]):
         y = _samples(5, cc, T * hop, 450 + i, fmt)
-        _assert_same(dst.process(y, T, hop, **want), twin.process(y, T, hop, **want), ("busy", i))
+        assert_bits_equal(dst.process(y, T, hop, **want), twin.process(y, T, hop, **want), ("busy", i))
     clk = src.get_clock()
     assert clk != dst.get_clock()
     dst.set_state(src.get_state(), first_stream=1)
@@ -212,30 +188,13 @@ def test_wave_migration_into_a_busy_engine():
         y = _samples(5, cc, T * hop, 550 + i, fmt)
         y[1:3] = x
         got = dst.process(y, T, hop, **want)
-        _assert_same(_slots(got, 1, 3), src.process(x, T, hop, **want), ("moved", i))
+        assert_bits_equal(_slots(got, 1, 3), src.process(x, T, hop, **want), ("moved", i))
         other = twin.process(y, T, hop, **want)
         for lo, hi in ((0, 1), (3, 5)):
-            _assert_same(_slots(got, lo, hi), _slots(other, lo, hi), ("others", i, lo))
+            assert_bits_equal(_slots(got, lo, hi), _slots(other, lo, hi), ("others", i, lo))
 
 
 # ---- graphs -----------------------------------------------------------------------------------------------------------
-
-def _capture(fn):
-    import torch
-
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        out = fn()
-    return g, out
-
-
-def _replay(g, xin, x):
-    import torch
-
-    xin.copy_(torch.from_numpy(x).cuda())
-    g.replay()
-    torch.cuda.synchronize()
-
 
 @pytest.mark.parametrize("hop", [800, 700], ids=["one-pass", "general"])
 def test_meter_graph_replays_read_restored_state(hop):
@@ -250,7 +209,7 @@ def test_meter_graph_replays_read_restored_state(hop):
     settings = {"rms_mode": True, "audio_sync_offset": 30}
     a, b, donor = (MeterEngine(settings, channels=cc, max_streams=S) for _ in range(3))
     xin = torch.zeros((S, cc, T * hop), device="cuda")
-    g, out = _capture(lambda: a.process(xin, T, hop, want_pixels=True))
+    g, out = capture(lambda: a.process(xin, T, hop, want_pixels=True))
     for i in range(7):
         restore = i in (1, 4)  # after 1 and after 4 replays
         if restore:
@@ -260,11 +219,11 @@ def test_meter_graph_replays_read_restored_state(hop):
         else:
             donor.process(_samples(S, cc, 5 * hop, 600 + i, "f32"), 5, hop)
         x = _samples(S, cc, T * hop, 650 + i, "f32")
-        _replay(g, xin, x)
-        _assert_same(out, b.process(x, T, hop, want_pixels=True), ("replay", i))
+        replay(g, [xin], [x])
+        assert_bits_equal(out, b.process(x, T, hop, want_pixels=True), ("replay", i))
         if restore:
-            _assert_same(out, donor.process(x, T, hop, want_pixels=True), ("donor", i))
-    _assert_same_state(a.get_state(), b.get_state(), "final")
+            assert_bits_equal(out, donor.process(x, T, hop, want_pixels=True), ("donor", i))
+    assert_bits_equal(a.get_state(), b.get_state(), "final")
 
 
 def test_wave_graph_replays_read_restored_state_and_clock():
@@ -279,7 +238,7 @@ def test_wave_graph_replays_read_restored_state_and_clock():
     a = WaveEngine(settings, channels=cc, max_streams=S, device_clock=True)
     b, donor = (WaveEngine(settings, channels=cc, max_streams=S) for _ in range(2))
     xin = torch.zeros((S, cc, T * hop), device="cuda")
-    g, out = _capture(lambda: a.process(xin, T, hop, want_pixels=True))
+    g, out = capture(lambda: a.process(xin, T, hop, want_pixels=True))
     for i in range(7):
         restore = i in (1, 4)
         if restore:
@@ -290,10 +249,10 @@ def test_wave_graph_replays_read_restored_state_and_clock():
         else:
             donor.process(_samples(S, cc, (1 + i) * 441, 700 + i, "f32"), 1 + i, 441)
         x = _samples(S, cc, T * hop, 750 + i, "f32")
-        _replay(g, xin, x)
-        _assert_same(out, b.process(x, T, hop, want_pixels=True), ("replay", i))
+        replay(g, [xin], [x])
+        assert_bits_equal(out, b.process(x, T, hop, want_pixels=True), ("replay", i))
         if restore:
-            _assert_same(out, donor.process(x, T, hop, want_pixels=True), ("donor", i))
+            assert_bits_equal(out, donor.process(x, T, hop, want_pixels=True), ("donor", i))
         assert a.get_clock() == b.get_clock()
 
 
@@ -307,14 +266,14 @@ def test_round_trips_change_nothing():
                         device_clock=c) for c in (True, False))
     for i, (T, hop) in enumerate([(4, 800), (3, 900), (5, 7)]):
         x = _samples(3, 2, T * hop, 800 + i, "f32")
-        _assert_same(m.process(x, T, hop, want_pixels=True), mt.process(x, T, hop, want_pixels=True), ("meter", i))
-        _assert_same(w.process(x, T, hop), wt.process(x, T, hop), ("wave", i))
+        assert_bits_equal(m.process(x, T, hop, want_pixels=True), mt.process(x, T, hop, want_pixels=True), ("meter", i))
+        assert_bits_equal(w.process(x, T, hop), wt.process(x, T, hop), ("wave", i))
         m.set_state(m.get_state())
         m.set_state(m.get_state(1, 1), first_stream=1)
         w.set_state(w.get_state())
         w.set_clock(w.get_clock())
-    _assert_same_state(m.get_state(), mt.get_state(), "meter")
-    _assert_same_state(w.get_state(), wt.get_state(), "wave")
+    assert_bits_equal(m.get_state(), mt.get_state(), "meter")
+    assert_bits_equal(w.get_state(), wt.get_state(), "wave")
 
 
 def test_fresh_state_and_resets():
@@ -355,7 +314,7 @@ def test_fresh_state_and_resets():
         x = _samples(2, 2, 3 * 800, 910, "f32")
         out = w.process(x, 3, 800)
         st = w.get_state()
-        assert np.array_equal(_bits(st["db"]), _bits(out["out"][:, -1]))  # the last tick's rows
+        assert np.array_equal(bits(st["db"]), bits(out["out"][:, -1]))  # the last tick's rows
         assert np.array_equal(st["hold"], x[:, :, -1920:])
         w.reset()
         st = w.get_state()
@@ -409,11 +368,11 @@ def test_out_of_range_and_refused_clocks_change_nothing():
         e.set_clock(edge)
     for i, (T, hop) in enumerate([(3, 1), (2, 800)]):
         z = _samples(3, 2, T * hop, 970 + i, "f32")
-        _assert_same(w3.process(z, T, hop, want_pixels=True), w2.process(z, T, hop, want_pixels=True), ("edge", i))
+        assert_bits_equal(w3.process(z, T, hop, want_pixels=True), w2.process(z, T, hop, want_pixels=True), ("edge", i))
         assert w3.get_clock() == w2.get_clock()
         if i == 0:
             assert w2.get_clock()["waveform_ts"] == edge["waveform_ts"]  # no points yet: the clock's waveform_ts stayed
-    _assert_same_state(m.get_state(), mt.get_state(), "meter")
+    assert_bits_equal(m.get_state(), mt.get_state(), "meter")
     y = _samples(3, 2, 4 * 800, 960, "f32")
-    _assert_same(w.process(y, 4, 800), wt.process(y, 4, 800), "after refusals")
-    _assert_same(m.process(y, 4, 800), mt.process(y, 4, 800), "meter after refusals")
+    assert_bits_equal(w.process(y, 4, 800), wt.process(y, 4, 800), "after refusals")
+    assert_bits_equal(m.process(y, 4, 800), mt.process(y, 4, 800), "meter after refusals")

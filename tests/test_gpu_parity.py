@@ -7,9 +7,10 @@ from __future__ import annotations
 import numpy as np
 import pytest
 
+from gpu_common import clean_knobs, set_knobs  # noqa: F401 (fixture)
 from helpers import check_points, parity_report, synth_pcm
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 
 
 def _oracle_batch(settings, channels, pcm, T, hop, rms=None, want_points=False):
@@ -115,9 +116,9 @@ def test_fast2048_matches_generic_and_oracle(monkeypatch):
     S, T, N = 37, 9, 2048
     pcm = synth_pcm(S, 1, T * N, zero_frames=[(2, 2, 6), (5, 0, 9)], frame_len=N, hop=N)
     fast = Engine(settings, channels=1, max_streams=S).process(torch.from_numpy(pcm).cuda(), T, N)
-    monkeypatch.setenv("WF_FORCE_GENERIC", "1")
+    set_knobs(monkeypatch, {"WF_FORCE_GENERIC": "1"})
     gen = Engine(settings, channels=1, max_streams=S).process(torch.from_numpy(pcm).cuda(), T, N)
-    monkeypatch.delenv("WF_FORCE_GENERIC")
+    set_knobs(monkeypatch, {})
     torch.cuda.synchronize()
     f, g = fast["db"].cpu().numpy(), gen["db"].cpu().numpy()
     ref_db, _, ref_sil = _oracle_batch(settings, 1, pcm, T, N)
@@ -348,10 +349,9 @@ def test_wide_kernel_is_bit_identical_to_one_group_kernel(settings, channels, ho
     from waveform_b200 import Engine
 
     S = 3
-    monkeypatch.setenv("WF_V3", v3)
-    monkeypatch.setenv("WF_WIDE_R", "1")
+    set_knobs(monkeypatch, {"WF_V3": v3, "WF_WIDE_R": "1"})
     e1 = Engine(settings, channels=channels, max_streams=S)
-    monkeypatch.setenv("WF_WIDE_R", str(R))
+    set_knobs(monkeypatch, {"WF_V3": v3, "WF_WIDE_R": str(R)})
     e2 = Engine(settings, channels=channels, max_streams=S)
     N = e1.fft_size
     hop = N // hop_div
@@ -377,8 +377,7 @@ def test_wide_kernel_is_bit_identical_to_one_group_kernel(settings, channels, ho
 def test_wide_kernel_gate_hold_and_wakeup(R, v3, monkeypatch):
     """Silence inside a round of R ticks: decay, freeze below floor-10 dB, wake-up — the lazily evaluated cluster-wide
     reduction must flip m_last_silent on the same tick as the reference (src/source_generic.cpp:63-95)."""
-    monkeypatch.setenv("WF_V3", v3)
-    monkeypatch.setenv("WF_WIDE_R", str(R))
+    set_knobs(monkeypatch, {"WF_V3": v3, "WF_WIDE_R": str(R)})
     settings = {"fft_size": 4096, "window": "hann", "gravity": 0.3, "floor": -40, "channel_mode": "stereo"}
     S, T, N = 3, 37, 4096
     pcm = synth_pcm(S, 2, T * N)

@@ -15,45 +15,17 @@ import numpy as np
 import pytest
 
 from fp64_spectrum import Fp64Spectrum, compare
+from gpu_common import CATALOGUE, assert_bits_equal, clean_knobs, route_id, set_knobs  # noqa: F401 (fixture)
 from helpers import synth_pcm
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 
 T = 8  # ticks per run, in two calls of 4
-KNOBS = ("WF_TEAM_W", "WF_WIDE_R", "WF_V3", "WF_PAR16384", "WF_WARP2", "WF_WARP2_DISPLAY", "WF_FORCE_GENERIC")
 
-# (family, N, channels, stereo, environment, display outputs): the conditions tests/test_gpu_fp64.py routes with
-ROUTES = [
-    ("stft2048_fast_kernel", 2048, 1, False, {"WF_TEAM_W": "1"}, False),
-    ("stft2048_team_kernel", 2048, 1, False, {"WF_TEAM_W": "4"}, False),
-    ("stft_warp2_kernel", 800, 1, False, {}, False),
-    ("stft_warp2_kernel", 1456, 1, False, {}, False),
-    ("stft_warp2_kernel/display", 800, 1, False, {}, True),
-    ("stft_warp2_kernel/display", 1024, 1, False, {}, True),
-    ("stft_v3_kernel", 1024, 1, False, {}, False),
-    ("stft_v3_kernel", 4096, 2, True, {}, True),
-    ("stft_v3_kernel", 4096, 2, False, {}, False),
-    ("stft_v3_kernel", 16384, 1, False, {"WF_PAR16384": "0"}, False),
-    ("stft16384_parity_kernel", 16384, 1, False, {}, False),
-    ("stft_wide_kernel", 4096, 1, False, {"WF_V3": "0", "WF_WIDE_R": "2"}, True),
-    ("stft_wide_kernel", 32768, 1, False, {"WF_WIDE_R": "2"}, False),
-    ("stft_fused_kernel", 256, 1, False, {}, True),
-    ("stft_fused_kernel", 2048, 2, False, {"WF_FORCE_GENERIC": "1", "WF_V3": "0", "WF_WIDE_R": "1"}, False),
-    ("stft_anyn_kernel/smem", 800, 1, False, {"WF_WARP2": "0"}, True),
-    ("stft_anyn_kernel/L2", 40000, 1, False, {}, False),
-]
-
-
-def _route_id(r):
-    fam, N, cc, stereo, env, disp = r
-    return f"{fam.replace('/', '-')}-{N}{'-stereo' if stereo else ('-mix' if cc == 2 else '')}"
-
-
-def _set_env(monkeypatch, env):
-    for k in KNOBS:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+ROUTES = [CATALOGUE[k] for k in (
+    "fast-2048", "team-2048", "warp2-800", "warp2-1456", "warp2-800-display", "warp2-1024-display", "v3-1024",
+    "v3-4096-stereo-display", "v3-4096-mix", "v3-16384", "parity-16384", "wide-4096-display", "wide-32768",
+    "fused-256-display", "fused-2048-mix", "smem-800-display", "l2-40000")]
 
 
 def _signals(N, cc, hop, pad=16):
@@ -103,13 +75,6 @@ def _run(eng, x, hop, fmt, disp, extras):
     return got, eng.get_state(), eng.last_kernel_name()
 
 
-def _assert_bits_equal(a, b, ctx):
-    assert a.keys() == b.keys(), ctx
-    for k in a:
-        assert a[k].dtype == b[k].dtype and a[k].shape == b[k].shape, (k, ctx)
-        assert np.array_equal(a[k].view(np.uint8), b[k].view(np.uint8)), (k, ctx)
-
-
 def _check_fp64(settings, cc, x, hop, got, eng, extras, ctx):
     db_min = float(eng.db_min)
     xf = x.astype(np.float32) * np.float32(2.0 ** -15)
@@ -141,12 +106,12 @@ def _extras(S, seed):
 
 
 @pytest.mark.parametrize("all_opt", [False, True], ids=["plain", "all-options"])
-@pytest.mark.parametrize("route", ROUTES, ids=[_route_id(r) for r in ROUTES])
+@pytest.mark.parametrize("route", ROUTES, ids=[route_id(r) for r in ROUTES])
 def test_s16_matches_f32_bit_for_bit(route, all_opt, monkeypatch):
     from waveform_b200 import Engine
 
     fam, N, cc, stereo, env, disp = route
-    _set_env(monkeypatch, env)
+    set_knobs(monkeypatch, env)
     for hop in sorted({N, (N // 4) & ~7}, reverse=True):     # multiples of 8 samples: both formats' frames 16-byte aligned
         x = _signals(N, cc, hop)
         S = x.shape[0]
@@ -159,8 +124,8 @@ def test_s16_matches_f32_bit_for_bit(route, all_opt, monkeypatch):
         ctx = (fam, N, hop, all_opt, n16)
         assert n32.startswith(fam.split("/")[0] + "<") and (("display" in n32) == fam.endswith("/display")), (ctx, n32)
         assert n16 == n32 + " s16", (n16, n32)
-        _assert_bits_equal(g16, g32, ctx)
-        _assert_bits_equal(st16, st32, ctx)
+        assert_bits_equal(g16, g32, ctx)
+        assert_bits_equal(st16, st32, ctx)
         _check_fp64(settings, cc, x, hop, g16, e16, extras, ctx)
 
 
@@ -169,7 +134,7 @@ def test_s16_alignment_routes(monkeypatch):
     int16 the CTA-per-tick kernel (the next family in routing order), and is still right against float64."""
     from waveform_b200 import Engine
 
-    _set_env(monkeypatch, {"WF_TEAM_W": "1"})
+    set_knobs(monkeypatch, {"WF_TEAM_W": "1"})
     N, hop = 2048, 2044
     x = _signals(N, 1, hop)
     settings = _options(N, False, False)
@@ -206,11 +171,11 @@ def test_s16_buffer_kinds(N, cc, stereo):
     f32 = Engine(settings, channels=cc, max_streams=1)
     want = [f32.process(f.astype(np.float32) * np.float32(2.0 ** -15), 1, N) for f in frames]
     for r, w in zip(ref, want):
-        _assert_bits_equal(r, w, ("device vs float32", N, cc))
+        assert_bits_equal(r, w, ("device vs float32", N, cc))
 
     host = Engine(settings, channels=cc, max_streams=1)
     for f, r in zip(frames, ref):
-        _assert_bits_equal(host.process(f, 1, N, pcm_format="s16"), r, ("pageable", N, cc))
+        assert_bits_equal(host.process(f, 1, N, pcm_format="s16"), r, ("pageable", N, cc))
 
     mapped = Engine(settings, channels=cc, max_streams=1)
     dch, B = mapped.display_channels, mapped.bins
@@ -222,7 +187,7 @@ def test_s16_buffer_kinds(N, cc, stereo):
             _raw_call(mapped, pin, 1, 1, N, cc * N, N, pout, psil, "s16")
             db = np.frombuffer((C.c_float * (dch * B)).from_address(pout), np.float32).reshape(r["db"].shape).copy()
             sil = np.frombuffer((C.c_uint8 * 1).from_address(psil), np.uint8).reshape(r["silent"].shape).copy()
-            _assert_bits_equal({"db": db, "silent": sil}, r, ("wf_host_alloc", N, cc))
+            assert_bits_equal({"db": db, "silent": sil}, r, ("wf_host_alloc", N, cc))
         assert mapped.last_kernel_name().endswith(" s16")
     finally:
         for q in (pin, pout, psil):
@@ -252,7 +217,7 @@ def test_s16_pinned_host_chunked():
     assert host.last_kernel_name() == dev.last_kernel_name()
     assert torch.equal(out_db.view(torch.int32), want["db"].cpu().view(torch.int32))
     assert torch.equal(out_sil, want["silent"].cpu())
-    _assert_bits_equal(host.get_state(), dev.get_state(), "pinned vs device state")
+    assert_bits_equal(host.get_state(), dev.get_state(), "pinned vs device state")
 
 
 def test_s16_side_stream_after_busy_producer():
@@ -335,7 +300,7 @@ def test_numpy_int16_without_keyword_stays_unscaled():
     x = np.random.default_rng(1).integers(-200, 200, size=(2, 1, 2 * N), dtype=np.int16)
     a = Engine({"fft_size": N}, channels=1, max_streams=2).process(x, 2, N)
     b = Engine({"fft_size": N}, channels=1, max_streams=2).process(x.astype(np.float32), 2, N)
-    _assert_bits_equal(a, b, "int16 numpy without pcm_format")
+    assert_bits_equal(a, b, "int16 numpy without pcm_format")
     s = Engine({"fft_size": N}, channels=1, max_streams=2).process(x, 2, N, pcm_format="s16")
     assert not np.array_equal(a["db"], s["db"])
     with pytest.raises(ValueError):

@@ -17,15 +17,13 @@ import numpy as np
 import pytest
 
 from fp64_spectrum import Fp64Spectrum, compare
+from gpu_common import clean_knobs, set_knobs  # noqa: F401 (fixture)
 from helpers import parity_report, synth_pcm
 from refdata import frame_peak, reference, sample_index
 from test_rates_cpu import FPS, GRID, auto_size, fps_value, frames_to_ns, grid_id, sync_delay, tick_counts
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 ROOT = Path(__file__).resolve().parents[1]
-
-KNOBS = ("WF_TEAM_W", "WF_WIDE_R", "WF_V3", "WF_PAR16384", "WF_WARP2", "WF_WARP2_DISPLAY", "WF_FORCE_GENERIC", "WF_SPLIT",
-         "WF_METER_FUSED", "WF_WAVE_CHUNK")
 
 # ---- routing: the rule of wf_engine.cu choose_route, restated for these sizes -------------------------------------------
 
@@ -54,13 +52,6 @@ def test_routing_rule_facts():
     assert expected_kernel(720, 1, False, 735)[0].startswith("stft_anyn_kernel<1>")
     assert expected_kernel(720, 1, False, 736) == ("stft_warp2_kernel<",)
     assert expected_kernel(720, 2, False, 736)[0].startswith("stft_anyn_kernel<2>")
-
-
-def _set_env(monkeypatch, env=None):
-    for k in KNOBS:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in (env or {}).items():
-        monkeypatch.setenv(k, v)
 
 
 # ---- 1. spectrum at every automatic size ----------------------------------------------------------------------------------
@@ -99,14 +90,13 @@ def _grid_signal(N, cc, n, seed):
 
 @pytest.mark.parametrize("layout", list(LAYOUTS))
 @pytest.mark.parametrize("point", GRID, ids=[grid_id(p) for p in GRID])
-def test_spectrum_at_the_automatic_size(point, layout, monkeypatch):
+def test_spectrum_at_the_automatic_size(point, layout):
     """Plain device calls, host (numpy) calls and capture-ring calls over the same frames, plain and all options, with
     seconds = 1 / fps: each stream within 1e-6 of float64 (fp64_spectrum.compare) with the same silent flags, the ring
     calls bit for bit the plain device calls, and each call on the kernel the routing rule names."""
     import torch
     from waveform_b200 import Engine
 
-    _set_env(monkeypatch)
     sr, fps = point
     cc, stereo = LAYOUTS[layout]
     N = auto_size(sr, fps)
@@ -254,7 +244,7 @@ def test_meter_at_44100_against_the_oracle(case, hop, fused, buf, monkeypatch):
     from waveform_b200 import MeterEngine
     from waveform_b200.engine import METER_INPUT_RMS
 
-    _set_env(monkeypatch, {"WF_METER_FUSED": fused})
+    set_knobs(monkeypatch, {"WF_METER_FUSED": fused})
     settings, cc = METER_CASES[case]
     feed = not settings
     if feed and hop > 1024:
@@ -350,7 +340,7 @@ def test_meter_rms_against_float64_at_44100(kind, hop, fused, monkeypatch):
     from waveform_b200 import MeterEngine
     from waveform_b200.engine import METER_INPUT_RMS
 
-    _set_env(monkeypatch, {"WF_METER_FUSED": fused})
+    set_knobs(monkeypatch, {"WF_METER_FUSED": fused})
     S_, ch, n_ticks = 3, 2, 400 if kind == "rms" else 900
     settings = {} if kind == "feed" else {"meter_buf": 150, "rms_mode": True, "temporal_smoothing": "none"}
     eng = MeterEngine(settings, sample_rate=44100, channels=ch, max_streams=S_,
@@ -436,7 +426,7 @@ def test_wave_at_44100(case, ms, monkeypatch):
     ws = {**settings, **({"audio_sync_offset": ms} if ms else {})}
     runs = {}
     for chunk in ("1", "0"):
-        _set_env(monkeypatch, {"WF_WAVE_CHUNK": chunk})
+        set_knobs(monkeypatch, {"WF_WAVE_CHUNK": chunk})
         for clock in (False, True):
             eng = WaveEngine(ws, sample_rate=sr, channels=cc, max_streams=S_, device_clock=clock)
             outs, pos, t0 = [], 0, 0

@@ -11,62 +11,43 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from gpu_common import CATALOGUE, assert_bits_equal, clean_knobs, set_knobs  # noqa: F401 (fixture)
 from helpers import check_points, synth_pcm
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 
-KNOBS = ("WF_TEAM_W", "WF_WIDE_R", "WF_V3", "WF_PAR16384", "WF_WARP2", "WF_WARP2_DISPLAY", "WF_FORCE_GENERIC")
 
-# (kernel family of the spectrum call, knobs, settings, capture channels)
+def _case(route, **display):
+    """(kernel family of the spectrum call, knobs, settings, capture channels): a route with these display settings."""
+    r = CATALOGUE[route]
+    settings = {"fft_size": r.N, **({"channel_mode": "stereo"} if r.stereo else {}), **display}
+    return r.family.split("/")[0], r.env, settings, r.cc
+
+
 FAMILY_CASES = [
-    ("stft_warp2_kernel", {}, {"fft_size": 1024, "interp_mode": "lanczos", "height": 300}, 1),
-    ("stft_warp2_kernel", {}, {"fft_size": 2048, "display_mode": "bars", "interp_mode": "catmull_rom", "rounded_caps": True,
-                               "min_bar_height": 5, "bar_width": 10, "bar_gap": 2}, 1),
-    ("stft_warp2_kernel", {}, {"fft_size": 800, "interp_mode": "point", "filter_mode": "gauss", "mirror_freq_axis": True}, 1),
-    ("stft_v3_kernel", {}, {"fft_size": 1024, "channel_mode": "stereo", "channel_spacing": 20, "mirror_freq_axis": True,
-                            "filter_mode": "gauss", "height": 400}, 2),
-    ("stft_v3_kernel", {}, {"fft_size": 4096, "display_mode": "bars", "channel_mode": "stereo", "channel_spacing": 10,
-                            "rounded_caps": True, "mirror_freq_axis": True, "interp_mode": "point"}, 2),
-    ("stft_v3_kernel", {}, {"fft_size": 4096, "display_mode": "bars", "interp_mode": "lanczos", "min_bar_height": 4}, 2),
-    ("stft_wide_kernel", {"WF_V3": "0"}, {"fft_size": 8192, "interp_mode": "lanczos", "filter_mode": "gauss"}, 1),
-    ("stft_wide_kernel", {"WF_V3": "0"}, {"fft_size": 4096, "display_mode": "bars", "interp_mode": "catmull_rom",
-                                          "mirror_freq_axis": True, "channel_mode": "stereo"}, 2),
-    ("stft_fused_kernel", {"WF_V3": "0", "WF_WIDE_R": "1"},
-     {"fft_size": 2048, "display_mode": "bars", "interp_mode": "lanczos", "min_bar_height": 3, "channel_mode": "stereo",
-      "channel_spacing": 6}, 2),
-    ("stft_fused_kernel", {"WF_V3": "0", "WF_WIDE_R": "1", "WF_WARP2_DISPLAY": "0"},
-     {"fft_size": 512, "interp_mode": "catmull_rom", "filter_mode": "gauss"}, 1),
-    ("stft_anyn_kernel", {}, {"fft_size": 800, "channel_mode": "stereo", "display_mode": "bars", "interp_mode": "catmull_rom",
-                              "rounded_caps": True, "bar_width": 8, "bar_gap": 3}, 2),
-    ("stft_anyn_kernel", {"WF_WARP2": "0"}, {"fft_size": 1456, "interp_mode": "lanczos", "mirror_freq_axis": True}, 1),
+    _case("warp2-1024-display", interp_mode="lanczos", height=300),
+    _case("warp2-2048-display", display_mode="bars", interp_mode="catmull_rom", rounded_caps=True, min_bar_height=5,
+          bar_width=10, bar_gap=2),
+    _case("warp2-800-display", interp_mode="point", filter_mode="gauss", mirror_freq_axis=True),
+    _case("v3-1024-stereo-display", channel_spacing=20, mirror_freq_axis=True, filter_mode="gauss", height=400),
+    _case("v3-4096-stereo-display", display_mode="bars", channel_spacing=10, rounded_caps=True, mirror_freq_axis=True,
+          interp_mode="point"),
+    _case("v3-4096-mix-display", display_mode="bars", interp_mode="lanczos", min_bar_height=4),
+    _case("wide-8192-display", interp_mode="lanczos", filter_mode="gauss"),
+    _case("wide-4096-stereo-display", display_mode="bars", interp_mode="catmull_rom", mirror_freq_axis=True),
+    _case("fused-2048-stereo-display", display_mode="bars", interp_mode="lanczos", min_bar_height=3, channel_spacing=6),
+    _case("fused-512-display", interp_mode="catmull_rom", filter_mode="gauss"),
+    _case("smem-800-stereo-display", display_mode="bars", interp_mode="catmull_rom", rounded_caps=True, bar_width=8,
+          bar_gap=3),
+    _case("smem-1456-display", interp_mode="lanczos", mirror_freq_axis=True),
     # a stereo row of 65536 floats does not fit in shared memory: the render kernel keeps it in its L2 scratch
-    ("stft_anyn_kernel", {}, {"fft_size": 65536, "channel_mode": "stereo", "interp_mode": "lanczos", "width": 640}, 2),
+    _case("l2-65536-stereo-display", interp_mode="lanczos", width=640),
 ]
 
 
 def _case_id(c):
     fam, env, s, cc = c
     return f"{fam}-{s['fft_size']}-{s.get('display_mode', 'curve')}-{'stereo' if s.get('channel_mode') == 'stereo' else cc}"
-
-
-def _knobs(monkeypatch, env):
-    for k in KNOBS:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
-
-
-def _bits(x):
-    import torch
-    x = x.detach().cpu() if hasattr(x, "detach") else torch.from_numpy(np.ascontiguousarray(x))
-    return x.contiguous().view(torch.int32).numpy()
-
-
-def _assert_same(a, b, what):
-    ba, bb = _bits(a), _bits(b)
-    assert ba.shape == bb.shape, what
-    bad = np.flatnonzero(ba.ravel() != bb.ravel())
-    assert bad.size == 0, (what, bad.size, bad[:8])
 
 
 def _spectrum(eng, settings, T=6, S=4, silent=True, **kw):
@@ -88,7 +69,7 @@ def test_render_of_own_db_is_bit_identical(case, monkeypatch):
     from waveform_b200 import Engine
 
     fam, env, settings, cc = case
-    _knobs(monkeypatch, env)
+    set_knobs(monkeypatch, env)
     S, T = (2, 2) if settings["fft_size"] > 32768 else (4, 6)
     eng = Engine(settings, channels=cc, max_streams=S)
     out = _spectrum(eng, settings, T=T, S=S, want_points=True, want_pixels=True)
@@ -104,15 +85,15 @@ def test_render_of_own_db_is_bit_identical(case, monkeypatch):
     torch.cuda.synchronize()
     assert eng.last_kernel_name().startswith("render_kernel<")
     for key in ("points", "pixels", "min"):
-        _assert_same(r[key], out[key], (key, name))
+        assert_bits_equal(r[key], out[key], (key, name))
     # points only (the display stage stores them without its shared-memory rows), pixels only
     rp = eng.render(db, want_points=True)
     rx = eng.render(db, want_pixels=True)
     torch.cuda.synchronize()
-    _assert_same(rp["points"], out["points"], ("points only", name))
-    _assert_same(rx["pixels"], out["pixels"], ("pixels only", name))
-    _assert_same(rx["min"], out["min"], ("min only", name))
-    _assert_same(db, db0, "db untouched")
+    assert_bits_equal(rp["points"], out["points"], ("points only", name))
+    assert_bits_equal(rx["pixels"], out["pixels"], ("pixels only", name))
+    assert_bits_equal(rx["min"], out["min"], ("min only", name))
+    assert_bits_equal(db, db0, "db untouched")
 
 
 PEAK_CASES = [FAMILY_CASES[1], FAMILY_CASES[3], FAMILY_CASES[4], FAMILY_CASES[6]]
@@ -125,7 +106,7 @@ def test_render_with_peak(case, monkeypatch):
     from waveform_b200 import Engine
 
     fam, env, settings, cc = case
-    _knobs(monkeypatch, env)
+    set_knobs(monkeypatch, env)
     eng = Engine(settings, channels=cc, max_streams=4)
     out = _spectrum(eng, settings, want_peak=True)
     db, peak = out["db"], out["peak"]
@@ -137,11 +118,11 @@ def test_render_with_peak(case, monkeypatch):
     r_keep = eng.render(db, peak, -3.0, 20.0, want_points=True, want_pixels=True)
     r0 = eng.render(ref, want_points=True, want_pixels=True)
     torch.cuda.synchronize()
-    _assert_same(got, ref, "write_db equals peak_normalize")
-    _assert_same(db, db0, "db untouched without write_db")
+    assert_bits_equal(got, ref, "write_db equals peak_normalize")
+    assert_bits_equal(db, db0, "db untouched without write_db")
     for key in ("points", "pixels", "min"):
-        _assert_same(r[key], r0[key], key)
-        _assert_same(r_keep[key], r0[key], key)
+        assert_bits_equal(r[key], r0[key], key)
+        assert_bits_equal(r_keep[key], r0[key], key)
     # against the oracle's render_curve / render_bars of the normalised rows
     nref = ref.cpu().numpy()
     o = OracleSource(settings, channels=cc)
@@ -171,7 +152,7 @@ def test_host_and_device_inputs_agree():
     rh = eng.render(db_h, want_points=True, want_pixels=True)
     torch.cuda.synchronize()
     for key in rd:
-        _assert_same(rd[key], rh[key], key)
+        assert_bits_equal(rd[key], rh[key], key)
     # with a peak and write_db: device rows + device peak, device rows + host peak, host rows + host peak (in place)
     a = db_d.clone()
     ra = eng.render(a, peak_d, -6.0, 12.0, write_db=True, want_points=True, want_pixels=True)
@@ -180,20 +161,20 @@ def test_host_and_device_inputs_agree():
     c = db_h.copy()
     rc = eng.render(c, peak_h, -6.0, 12.0, write_db=True, want_points=True, want_pixels=True)
     torch.cuda.synchronize()
-    _assert_same(a, b, "host peak")
-    _assert_same(a, c, "host rows")
+    assert_bits_equal(a, b, "host peak")
+    assert_bits_equal(a, c, "host rows")
     for key in ra:
-        _assert_same(ra[key], rb[key], key)
-        _assert_same(ra[key], rc[key], key)
+        assert_bits_equal(ra[key], rb[key], key)
+        assert_bits_equal(ra[key], rc[key], key)
     # a row base that is not 16-byte aligned takes the scalar path: same bits
     flat = torch.empty(db_d.numel() + 1, device="cuda")
     flat[1:] = db_d.reshape(-1)
     odd = flat[1:].view(db_d.shape)
     ro = eng.render(odd, peak_d, -6.0, 12.0, write_db=True, want_points=True, want_pixels=True)
     torch.cuda.synchronize()
-    _assert_same(odd, a, "unaligned rows")
+    assert_bits_equal(odd, a, "unaligned rows")
     for key in ra:
-        _assert_same(ro[key], ra[key], key)
+        assert_bits_equal(ro[key], ra[key], key)
 
 
 def test_render_on_a_side_stream_is_ordered_after_its_producer():
@@ -215,11 +196,11 @@ def test_render_on_a_side_stream_is_ordered_after_its_producer():
         after = dst.clone()
     torch.cuda.synchronize()
     for key in expect:
-        _assert_same(r[key], expect[key], key)
+        assert_bits_equal(r[key], expect[key], key)
     ref = out["db"].clone()
     eng.peak_normalize(ref, out["peak"], -3.0, 20.0)
     torch.cuda.synchronize()
-    _assert_same(after, ref, "db written back on the side stream")
+    assert_bits_equal(after, ref, "db written back on the side stream")
 
 
 def test_render_errors():
@@ -317,7 +298,7 @@ def test_process_normalized_display_equals_the_steps_by_hand():
     eng.peak_normalize(out["db"], out["peak"], -3.0, 25.0)
     r = eng.render(out["db"], want_points=True, want_pixels=True)
     torch.cuda.synchronize()
-    _assert_same(a["db"], out["db"], "db")
-    _assert_same(a["peak"], out["peak"], "peak")
+    assert_bits_equal(a["db"], out["db"], "db")
+    assert_bits_equal(a["peak"], out["peak"], "peak")
     for key in ("points", "pixels", "min"):
-        _assert_same(a[key], r[key], key)
+        assert_bits_equal(a[key], r[key], key)

@@ -15,40 +15,27 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from gpu_common import CATALOGUE, assert_bits_equal, clean_knobs, route_id, set_knobs  # noqa: F401 (fixture)
 from helpers import synth_pcm
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 
-KNOBS = ("WF_TEAM_W", "WF_WIDE_R", "WF_V3", "WF_PAR16384", "WF_WARP2", "WF_WARP2_DISPLAY", "WF_FORCE_GENERIC", "WF_SPLIT")
-
-# (family, N, channels, stereo, environment, display outputs, streams, start of the last call's kernel name)
-ROUTES = [
-    ("stft2048_fast_kernel", 2048, 1, False, {"WF_TEAM_W": "1"}, False, 5, "stft2048_fast_kernel<12,1,1,1> grid 5 x 8 warps"),
-    ("stft2048_fast_kernel/split", 2048, 1, False, {"WF_TEAM_W": "1"}, False, 300, "stft2048_fast_kernel<12,1,1,1> grid 132 x 8 warps"),
-    ("stft2048_team_kernel", 2048, 1, False, {"WF_TEAM_W": "4"}, False, 5, "stft2048_team_kernel<4,1> grid 5 x 4 teams"),
-    ("stft_warp2_kernel", 800, 1, False, {}, False, 5, "stft_warp2_kernel<20,20> N=800"),
-    ("stft_warp2_kernel/display", 1024, 1, False, {}, True, 5, "stft_warp2_kernel<16,32,display> N=1024"),
-    ("stft_v3_kernel", 1024, 1, False, {}, False, 5, "stft_v3_kernel<1024,1,"),
-    ("stft_v3_kernel", 4096, 2, False, {}, False, 5, "stft_v3_kernel<4096,2,"),
-    ("stft_v3_kernel", 4096, 2, True, {}, True, 5, "stft_v3_kernel<4096,2,"),
-    ("stft16384_parity_kernel", 16384, 1, False, {}, False, 3, "stft16384_parity_kernel<1> 3 clusters of 2"),
-    ("stft_wide_kernel", 32768, 1, False, {"WF_WIDE_R": "2"}, False, 2, "stft_wide_kernel<32768,1,2>"),
-    ("stft_fused_kernel", 256, 1, False, {}, True, 5, "stft_fused_kernel<256,1>"),
-    ("stft_anyn_kernel/smem", 800, 1, False, {"WF_WARP2": "0"}, True, 5, "stft_anyn_kernel<1> N=800"),
-    ("stft_anyn_kernel/L2", 40000, 1, False, {}, False, 2, "stft_anyn_kernel<1> N=40000"),
-]
-
-
-def _route_id(r):
-    fam, N, cc, stereo = r[:4]
-    return f"{fam.replace('/', '-')}-{N}{'-stereo' if stereo else ('-mix' if cc == 2 else '')}"
-
-
-def _set_env(monkeypatch, env):
-    for k in KNOBS:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+# (route, streams, start of the last call's kernel name)
+ROUTES = [(*CATALOGUE[k], S, name) for k, S, name in [
+    ("fast-2048", 5, "stft2048_fast_kernel<12,1,1,1> grid 5 x 8 warps"),
+    ("fast-2048-split", 300, "stft2048_fast_kernel<12,1,1,1> grid 132 x 8 warps"),
+    ("team-2048", 5, "stft2048_team_kernel<4,1> grid 5 x 4 teams"),
+    ("warp2-800", 5, "stft_warp2_kernel<20,20> N=800"),
+    ("warp2-1024-display", 5, "stft_warp2_kernel<16,32,display> N=1024"),
+    ("v3-1024", 5, "stft_v3_kernel<1024,1,"),
+    ("v3-4096-mix", 5, "stft_v3_kernel<4096,2,"),
+    ("v3-4096-stereo-display", 5, "stft_v3_kernel<4096,2,"),
+    ("parity-16384", 3, "stft16384_parity_kernel<1> 3 clusters of 2"),
+    ("wide-32768", 2, "stft_wide_kernel<32768,1,2>"),
+    ("fused-256-display", 5, "stft_fused_kernel<256,1>"),
+    ("smem-800-display", 5, "stft_anyn_kernel<1> N=800"),
+    ("l2-40000", 2, "stft_anyn_kernel<1> N=40000"),
+]]
 
 
 def _calls(N):
@@ -69,17 +56,6 @@ def _signal(S, cc, n, seed, s16):
     return x.astype(np.float32)
 
 
-def _assert_bits_equal(a, b, ctx):
-    assert a.keys() == b.keys(), ctx
-    for k in a:
-        assert a[k].dtype == b[k].dtype and a[k].shape == b[k].shape, (k, ctx)
-        assert np.array_equal(a[k].view(np.uint8), b[k].view(np.uint8)), (k, ctx)
-
-
-def _state_bits(st):
-    return {k: np.ascontiguousarray(v) for k, v in st.items()}
-
-
 def _run_pair(settings, cc, S, calls, x, fmt, disp, feed):
     """Ring calls on one engine, plain calls over zeros(N) ++ x on another; `feed(eng, pcm, T, hop, ring)` makes one call
     and returns its outputs as numpy.  Asserts per call that outputs, names, state and ring agree."""
@@ -96,9 +72,9 @@ def _run_pair(settings, cc, S, calls, x, fmt, disp, feed):
         got = feed(ring_eng, new, T_, hop, True)
         want = feed(plain_eng, plain, T_, hop, False)
         ctx = (settings, fmt, T_, hop)
-        _assert_bits_equal(got, want, ctx)
+        assert_bits_equal(got, want, ctx)
         assert ring_eng.last_kernel_name() == plain_eng.last_kernel_name() + " ring", ctx
-        _assert_bits_equal(_state_bits(ring_eng.get_state()), _state_bits(plain_eng.get_state()), ctx)
+        assert_bits_equal(ring_eng.get_state(), plain_eng.get_state(), ctx)
         pos += T_ * hop
         want_ring = full[:, :, pos: pos + N].astype(np.float32)
         if x.dtype == np.int16:
@@ -134,10 +110,10 @@ def _host_feed(disp, fmt):
 
 @pytest.mark.parametrize("buf", ["device", "host"])
 @pytest.mark.parametrize("fmt", ["f32", "s16"])
-@pytest.mark.parametrize("route", ROUTES, ids=[_route_id(r) for r in ROUTES])
+@pytest.mark.parametrize("route", ROUTES, ids=[route_id(r) for r in ROUTES])
 def test_ring_matches_plain_bit_for_bit(route, fmt, buf, monkeypatch):
     fam, N, cc, stereo, env, disp, S, name = route
-    _set_env(monkeypatch, env)
+    set_knobs(monkeypatch, env)
     calls = _calls(N)
     x = _signal(S, cc, sum(t * h for t, h in calls), 0x5150 + N, fmt == "s16")
     feed = (_device_feed if buf == "device" else _host_feed)(disp, fmt)

@@ -22,12 +22,12 @@ from pathlib import Path
 import numpy as np
 import pytest
 
-pytestmark = pytest.mark.gpu
+from gpu_common import clean_knobs, set_knobs  # noqa: F401 (fixture)
+
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 
 STORE = Path(__file__).resolve().parent / "golden" / "routes_h100.json"
 RECORDING = os.environ.get("WF_RECORD_ROUTES") == "1"
-KNOBS = ("WF_FORCE_GENERIC", "WF_V3", "WF_WIDE_R", "WF_TEAM_W", "WF_PAR16384", "WF_WARP2", "WF_WARP2_DISPLAY",
-         "WF_SPLIT", "WF_ZERO_COPY")
 
 OPT = {"fast_peaks": True}                      # an option that selects a kernel's EXTRA variant and needs no input
 LANCZOS = {"interp_mode": "lanczos"}
@@ -196,10 +196,7 @@ def test_route(case, monkeypatch):
             pytest.skip(f"routes recorded on a {table['device']} with {table['sm_count']} SMs; this device has {sm}")
         assert case in table["routes"], f"{case}: not in {STORE.name}; record it with WF_RECORD_ROUTES=1"
     N, settings, cc, env, S, T, calls = CASES[case]
-    for k in KNOBS:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+    set_knobs(monkeypatch, env)
     if isinstance(S, tuple):
         S = S[0] * sm + S[1]
     eng = Engine({"fft_size": N, **settings}, channels=cc, max_streams=S)

@@ -17,9 +17,10 @@ import numpy as np
 import pytest
 
 from fp64_spectrum import Fp64Spectrum, compare
+from gpu_common import clean_knobs, set_knobs  # noqa: F401 (fixture)
 from helpers import check_points, device_pcm, parity_report, synth_pcm
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 
 SMS = 132  # H100 SXM: the N=2048 kernel launches one CTA per SM
 
@@ -101,7 +102,7 @@ FAST_SHAPES = [
 @pytest.mark.parametrize("S,T,calls", FAST_SHAPES)
 def test_fast2048_parity_at_measured_geometry(S, T, calls, monkeypatch):
     """The warp-per-stream kernel at its real launch geometries (WF_TEAM_W=1 keeps the small shapes on it too)."""
-    monkeypatch.setenv("WF_TEAM_W", "1")
+    set_knobs(monkeypatch, {"WF_TEAM_W": "1"})
     settings = {"fft_size": 2048, "window": "hann", "gravity": 0.65}
     eng, out, _ = _run_and_check(settings, 1, S, T, calls=calls)
     assert eng.last_kernel_name().startswith("stft2048_fast"), eng.last_kernel_name()
@@ -118,11 +119,10 @@ def test_fast2048_split_runs_are_bit_identical_to_whole_streams(S, T, calls, opt
     import torch
     from waveform_b200 import Engine
 
-    monkeypatch.setenv("WF_TEAM_W", "1")
     settings = {"fft_size": 2048, "window": "hann", "gravity": 0.65, **opts}
     res = {}
     for mode in ("1", "0"):
-        monkeypatch.setenv("WF_SPLIT", mode)
+        set_knobs(monkeypatch, {"WF_TEAM_W": "1", "WF_SPLIT": mode})
         eng = Engine(settings, channels=1, max_streams=S)
         pcm = device_pcm(S, 1, (T - 1) * 2048 + 2048, seed=77 + S, zero_every=3, frame_len=2048 * max(1, T // 3))
         parts, t0 = [], 0
@@ -152,7 +152,7 @@ def test_warp2_split_runs_are_bit_identical_to_whole_streams(N, S, T, points, mo
         settings["interp_mode"] = "catmull_rom"
     res = {}
     for mode in ("1", "0"):
-        monkeypatch.setenv("WF_SPLIT", mode)
+        set_knobs(monkeypatch, {"WF_SPLIT": mode})
         eng = Engine(settings, channels=1, max_streams=S)
         pcm = device_pcm(S, 1, T * N, seed=5 + N, zero_every=3, frame_len=N * max(1, T // 3))
         a = eng.process(pcm[:, :, : 2 * N].contiguous(), 2, N, want_points=points, want_pixels=points)
@@ -183,7 +183,7 @@ def test_team2048_parity_and_bit_identity(S, T, calls, W, monkeypatch):
     settings = {"fft_size": 2048, "window": "hann", "gravity": 0.65}
     eng, out, pcm = _run_and_check(settings, 1, S, T, calls=calls)
     assert eng.last_kernel_name().startswith(f"stft2048_team_kernel<{W},"), eng.last_kernel_name()
-    monkeypatch.setenv("WF_TEAM_W", "1")
+    set_knobs(monkeypatch, {"WF_TEAM_W": "1"})
     ref_eng = Engine(settings, channels=1, max_streams=S)
     ref = ref_eng.process(pcm, T, 2048)
     torch.cuda.synchronize()
@@ -211,7 +211,7 @@ def test_team2048_all_options_match_fast_kernel(W, monkeypatch):
     x, r, k = torch.from_numpy(pcm).cuda(), torch.from_numpy(rms).cuda(), torch.from_numpy(skip).cuda()
     outs = []
     for w in (W, 1):
-        monkeypatch.setenv("WF_TEAM_W", str(w))
+        set_knobs(monkeypatch, {"WF_TEAM_W": str(w)})
         eng = Engine(settings, channels=1, max_streams=S)
         a = eng.process(x[:, :, : 16 * N].contiguous(), 16, N, input_rms=r[:, :16].contiguous(), skip_mask=k[:, :16].contiguous(), want_peak=True)
         b = eng.process(x[:, :, 16 * N:].contiguous(), T - 16, N, input_rms=r[:, 16:].contiguous(), skip_mask=k[:, 16:].contiguous(), want_peak=True)
@@ -277,7 +277,7 @@ def test_warp2_display_variant(settings, S, T, monkeypatch):
     assert "display" in e2.last_kernel_name()
     for key in ("points", "pixels", "min", "silent"):
         assert torch.equal(a[key], b[key]), key
-    monkeypatch.setenv("WF_WARP2_DISPLAY", "0")
+    set_knobs(monkeypatch, {"WF_WARP2_DISPLAY": "0"})
     e3 = Engine(settings, channels=1, max_streams=S)
     c = e3.process(pcm, T, N, want_points=True, want_pixels=True)
     torch.cuda.synchronize()
@@ -303,7 +303,7 @@ def test_golden_vectors_spectrum_only(path, team_w, monkeypatch):
     settings = json.loads(str(z["settings"]))
     from waveform_b200 import Engine
 
-    monkeypatch.setenv("WF_TEAM_W", team_w)   # "1": warp-per-stream kernel; "0": the engine's routing (one stream -> a team)
+    set_knobs(monkeypatch, {"WF_TEAM_W": team_w})   # "1": warp-per-stream kernel; "0": the engine's routing (one stream -> a team)
     eng = Engine(settings, channels=int(z["channels"]), max_streams=1)
     rms = z["rms"][None, :] if z["rms"].size else None
     out = eng.process(z["pcm"][None], int(z["n_frames"]), int(z["hop"]), seconds=float(z["seconds"]), input_rms=rms)
@@ -321,7 +321,7 @@ def test_fast2048_gate_decay_freeze_wake(split, team_w, monkeypatch):
     """Decay -> freeze -> wake-up on the warp-per-stream kernel (team_w = 1) and on the team kernel (lazy team-wide gate
     reduction), with the call boundary inside the decay (7) and inside the frozen stretch (12): the next call must see the
     held dB row and both gate flags."""
-    monkeypatch.setenv("WF_TEAM_W", str(team_w))
+    set_knobs(monkeypatch, {"WF_TEAM_W": str(team_w)})
     settings = {"fft_size": 2048, "window": "hann", "gravity": 0.3, "floor": -40}
     S, T, N = 5, 30, 2048
     pcm = synth_pcm(S, 1, T * N)
@@ -450,11 +450,11 @@ def test_warp2_nonpow2_sizes_parity(N, monkeypatch):
             assert err.max() < 1e-6 and not bad_floor, (settings, s, err.max())
             assert np.array_equal(sil[s].astype(bool), tr["silent"]), (settings, s)
         assert np.array_equal(sil, ref_sil) and ref_sil.sum() > 10
-        monkeypatch.setenv("WF_WARP2", "0")
+        set_knobs(monkeypatch, {"WF_WARP2": "0"})
         old = Engine(settings, channels=1, max_streams=S)
         c = old.process(x, T, N)
         torch.cuda.synchronize()
-        monkeypatch.delenv("WF_WARP2")
+        set_knobs(monkeypatch, {})
         assert old.last_kernel_name().startswith("stft_anyn"), old.last_kernel_name()
         rep2 = parity_report(got, c["db"].cpu().numpy(), db_min=eng.db_min)
         assert rep2["ok"], rep2
@@ -469,7 +469,7 @@ def test_per_tick_seconds_tv_exponential(N, S, team_w, monkeypatch):
     from oracle.oraclebind import OracleSource
     from waveform_b200 import Engine
 
-    monkeypatch.setenv("WF_TEAM_W", team_w)
+    set_knobs(monkeypatch, {"WF_TEAM_W": team_w})
     settings = {"fft_size": N, "window": "hann", "temporal_smoothing": "tv_exp_moving_avg", "gravity": 0.5}
     T = 12
     rng = np.random.default_rng(11)
@@ -516,7 +516,7 @@ def test_par16384_bin_parity_cluster(variant, monkeypatch):
     x = torch.from_numpy(pcm).cuda()
     outs = {}
     for name, flag in (("par", "1"), ("v3", "0")):
-        monkeypatch.setenv("WF_PAR16384", flag)
+        set_knobs(monkeypatch, {"WF_PAR16384": flag})
         eng = Engine(settings, channels=1, max_streams=S)
 
         def kw(a, b):
@@ -556,7 +556,7 @@ def test_zero_copy_live_path_equals_staged_path(monkeypatch):
     pcm = synth_pcm(1, cc, 6 * N, seed=2)[0]
     outs = {}
     for name, zc in (("zero_copy", "1"), ("staged", "0")):
-        monkeypatch.setenv("WF_ZERO_COPY", zc)
+        set_knobs(monkeypatch, {"WF_ZERO_COPY": zc})
         eng = Engine(settings, channels=cc, max_streams=1)
         L, B, dch = eng.L, eng.bins, eng.display_channels
         pin = L.wf_host_alloc(cc * N * 4)

@@ -7,9 +7,10 @@ reference's own code in both runs; only the per-frame pipeline differs (FFTW + s
 import numpy as np
 import pytest
 
+from gpu_common import clean_knobs  # noqa: F401 (fixture)
 from helpers import parity_report, synth_pcm
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 
 
 def _pair(settings, channels):

@@ -16,9 +16,10 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from gpu_common import assert_bits_equal, bits, clean_knobs, set_knobs  # noqa: F401 (fixture)
 from helpers import synth_pcm
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 SR = 48000
 
 
@@ -30,10 +31,6 @@ def _signal(S, cc, n, seed, s16):
     x = synth_pcm(S, cc, n, seed=seed)
     x[:, :, n // 3: n // 3 + n // 5] = 0.0  # digital silence: the gate and m_last_silent
     return np.round(x * 32767.0).astype(np.int16) if s16 else x.astype(np.float32)
-
-
-def _bits(a):
-    return np.ascontiguousarray(a).view(np.uint8)
 
 
 # ---- spectrum ------------------------------------------------------------------------------------------------------
@@ -79,12 +76,9 @@ def _spectrum_pair(settings, cc, S, calls, x, ms, feed, caller_mask=None, first_
         got = feed(ring_eng, new, T_, hop, True, first_stream, ring_mask)
         want = feed(plain_eng, plain, T_, hop, False, first_stream, plain_mask)
         ctx = (settings, ms, T_, hop)
-        assert got.keys() == want.keys()
-        for k in got:
-            assert np.array_equal(_bits(got[k]), _bits(want[k])), (k, ctx)
+        assert_bits_equal(got, want, ctx)
         assert ring_eng.last_kernel_name() == plain_eng.last_kernel_name() + " ring", ctx
-        for k, v in ring_eng.get_state().items():
-            assert np.array_equal(_bits(v), _bits(plain_eng.get_state()[k])), (k, ctx)
+        assert_bits_equal(ring_eng.get_state(), plain_eng.get_state(), ctx)
         pos += T_ * hop
         want_ring = full[:, :, pos: pos + N + D].astype(np.float32)
         if x.dtype == np.int16:
@@ -259,7 +253,7 @@ def test_spectrum_no_offset_is_todays_call(ms):
         names.append(e.last_kernel_name())
         launches.append(e.L.wf_launch_count(e.h) - l0)
         assert e.get_ring().shape == (4, 1, 2048)
-    assert all(np.array_equal(_bits(o), _bits(outs[0])) for o in outs)
+    assert all(np.array_equal(bits(o), bits(outs[0])) for o in outs)
     assert len(set(names)) == 1 and len(set(launches)) == 1
 
 
@@ -298,16 +292,14 @@ def test_meter_offset_is_a_zero_prefixed_stream(name, settings, cc, mode, ms, fm
             gb = {k: v.cpu().numpy() for k, v in b.process(torch.from_numpy(pb).cuda(), T_, hop, first_stream=1,
                                                           pcm_format=fmt).items()}
             torch.cuda.synchronize()
-        for k in ga:
-            assert np.array_equal(_bits(ga[k]), _bits(gb[k])), (name, ms, k, T_, hop)
+        assert_bits_equal(ga, gb, (name, ms, T_, hop))
         pos += T_ * hop
     a.reset(0, 3)  # leaves the delay lines alone: the next call still starts with the held-back samples
     b.reset(0, 3)
     ga = a.process(np.ascontiguousarray(x[:, :, :1600]), 2, 800, first_stream=1, pcm_format=fmt)
     held = np.concatenate([xd[:, :, pos: pos + D], x[:, :, :1600]], axis=2)  # the line: the last D samples so far
     gb = b.process(np.ascontiguousarray(held[:, :, :1600]), 2, 800, first_stream=1, pcm_format=fmt)
-    for k in ga:
-        assert np.array_equal(_bits(ga[k]), _bits(gb[k])), (name, ms, k, "after reset")
+    assert_bits_equal(ga, gb, (name, ms, "after reset"))
 
 
 @pytest.mark.parametrize("ms", [10, 1000])
@@ -348,8 +340,7 @@ def test_meter_no_offset_is_todays_call():
         outs.append(e.process(x, 10, 800))
         launches.append(e.L.wf_meter_launch_count(e.h) - l0)
     for o in outs[1:]:
-        for k in o:
-            assert np.array_equal(_bits(o[k]), _bits(outs[0][k]))
+        assert_bits_equal(o, outs[0], "no offset")
     assert len(set(launches)) == 1
 
 
@@ -404,7 +395,7 @@ def test_wave_offset_chunked_and_per_tick_kernels_agree(settings, cc, s16, monke
     fmt = "s16" if s16 else "f32"
     outs = {}
     for chunk in ("1", "0"):
-        monkeypatch.setenv("WF_WAVE_CHUNK", chunk)
+        set_knobs(monkeypatch, {"WF_WAVE_CHUNK": chunk})
         eng = WaveEngine({**settings, "audio_sync_offset": ms}, channels=cc, max_streams=S)
         pos, got = 0, []
         for T_, hop in calls:
@@ -415,8 +406,7 @@ def test_wave_offset_chunked_and_per_tick_kernels_agree(settings, cc, s16, monke
             pos += T_ * hop
         outs[chunk] = got
     for a, b in zip(outs["1"], outs["0"]):
-        for k in a:
-            assert np.array_equal(_bits(a[k]), _bits(b[k])), k
+        assert_bits_equal(a, b, "chunked vs per-tick")
 
 
 def test_wave_no_offset_is_todays_call():
@@ -430,6 +420,5 @@ def test_wave_no_offset_is_todays_call():
         outs.append(e.process(x, 30, 800, want_points=True))
         launches.append(e.L.wf_wave_launch_count(e.h) - l0)
     for o in outs[1:]:
-        for k in o:
-            assert np.array_equal(_bits(o[k]), _bits(outs[0][k]))
+        assert_bits_equal(o, outs[0], "no offset")
     assert len(set(launches)) == 1

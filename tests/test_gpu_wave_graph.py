@@ -15,25 +15,12 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from gpu_common import assert_bits_equal, capture, clean_knobs, replay, set_knobs, to_host  # noqa: F401 (fixture)
 from helpers import synth_pcm
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("clean_knobs")]
 SR = 48000
 GOLD = sorted((Path(__file__).parent / "golden").glob("wave_*.npz"))
-
-
-def _bits(a):
-    return np.ascontiguousarray(a).view(np.uint8)
-
-
-def _host(out):
-    return {k: (v.cpu().numpy() if hasattr(v, "cpu") else np.array(v)) for k, v in out.items()}
-
-
-def _assert_same(got, want, what):
-    assert got.keys() == want.keys(), what
-    for k in want:
-        assert np.array_equal(_bits(got[k]), _bits(want[k])), (what, k)
 
 
 def _samples(S, cc, n, seed, fmt):
@@ -55,24 +42,6 @@ def _twins(settings, ch, S):
     from waveform_b200 import WaveEngine
 
     return WaveEngine(settings, channels=ch, max_streams=S, device_clock=True), WaveEngine(settings, channels=ch, max_streams=S)
-
-
-def _capture(fn):
-    import torch
-
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        out = fn()
-    return g, out
-
-
-def _replay(g, inputs, values):
-    import torch
-
-    for buf, v in zip(inputs, values):
-        buf.copy_(_dev(v))
-    g.replay()
-    torch.cuda.synchronize()
 
 
 def _walk(settings, hops):
@@ -136,8 +105,8 @@ def test_eager_calls_equal_the_host_clock(name, settings, ch, fmt, want):
         rms = _dev(np.random.default_rng(i).uniform(0.01, 0.3, (S, T)).astype(np.float32)) \
             if settings.get("normalize_volume") else None
         la, lb = a.launch_count, b.launch_count
-        got = _host(a.process(x, T, hop, input_rms=rms, pcm_format=fmt, **want))
-        _assert_same(got, _host(b.process(x, T, hop, input_rms=rms, pcm_format=fmt, **want)), (name, i, hop))
+        got = to_host(a.process(x, T, hop, input_rms=rms, pcm_format=fmt, **want))
+        assert_bits_equal(got, to_host(b.process(x, T, hop, input_rms=rms, pcm_format=fmt, **want)), (name, i, hop))
         assert a.launch_count - la == b.launch_count - lb + 1  # the plan kernel
         assert a.last_kernel_ms() >= 0
 
@@ -149,7 +118,7 @@ def test_eager_extreme_widths(width, want):
     a, b = _twins(settings, 2, S)
     for i, hop in enumerate((800, 3, 9000, 441)):
         x = _dev(_samples(S, 2, T * hop, 40 + i, "f32"))
-        _assert_same(_host(a.process(x, T, hop, **want)), _host(b.process(x, T, hop, **want)), (width, i))
+        assert_bits_equal(to_host(a.process(x, T, hop, **want)), to_host(b.process(x, T, hop, **want)), (width, i))
 
 
 @pytest.mark.parametrize("seed", range(8))
@@ -166,7 +135,7 @@ def test_long_calls_through_runs_and_breaks(seed):
         T = max(1, min(int(rng.integers(1, 3000)), 3_000_000 // hop))
         x = _dev(_samples(1, ch, T * hop, 950 + 10 * seed + i, "f32"))
         la, lb = a.launch_count, b.launch_count
-        _assert_same(_host(a.process(x, T, hop)), _host(b.process(x, T, hop)), (settings, ch, i, hop, T))
+        assert_bits_equal(to_host(a.process(x, T, hop)), to_host(b.process(x, T, hop)), (settings, ch, i, hop, T))
         assert a.launch_count - la == b.launch_count - lb + 1
 
 
@@ -183,12 +152,12 @@ def test_replays_from_a_fresh_engine_cross_the_startup():
     assert counts[0] == 0 and counts[-1] > 0
     a, b = _twins(settings, 2, S)
     xin = torch.zeros((S, 2, T * hop), device="cuda")
-    g, out = _capture(lambda: a.process(xin, T, hop, want_pixels=True))
+    g, out = capture(lambda: a.process(xin, T, hop, want_pixels=True))
     assert a.last_kernel_ms() < 0
     for i in range(8):
         x = _samples(S, 2, T * hop, 100 + i, "f32")
-        _replay(g, [xin], [x])
-        _assert_same(_host(out), _host(b.process(_dev(x), T, hop, want_pixels=True)), ("replay", i))
+        replay(g, [xin], [x])
+        assert_bits_equal(to_host(out), to_host(b.process(_dev(x), T, hop, want_pixels=True)), ("replay", i))
 
 
 def test_replays_interleaved_with_eager_calls_and_two_graphs():
@@ -199,18 +168,18 @@ def test_replays_interleaved_with_eager_calls_and_two_graphs():
     a, b = _twins(settings, 2, S)
     shapes = [(1, 800), (4, 97)]
     xins = [torch.zeros((S, 2, T * hop), device="cuda") for T, hop in shapes]
-    graphs = [_capture(lambda T=T, hop=hop, xin=xin: a.process(xin, T, hop)) for (T, hop), xin in zip(shapes, xins)]
+    graphs = [capture(lambda T=T, hop=hop, xin=xin: a.process(xin, T, hop)) for (T, hop), xin in zip(shapes, xins)]
     for i in range(9):
         T, hop = shapes[i % 2] if i % 3 else (2, 2000)
         x = _samples(S, 2, T * hop, 200 + i, "f32")
-        want = _host(b.process(_dev(x), T, hop))
+        want = to_host(b.process(_dev(x), T, hop))
         if i % 3:
             g, out = graphs[i % 2]
-            _replay(g, [xins[i % 2]], [x])
-            got = _host(out)
+            replay(g, [xins[i % 2]], [x])
+            got = to_host(out)
         else:
-            got = _host(a.process(_dev(x), T, hop))
-        _assert_same(got, want, ("interleaved", i))
+            got = to_host(a.process(_dev(x), T, hop))
+        assert_bits_equal(got, want, ("interleaved", i))
 
 
 # ---- 4. live ticks ---------------------------------------------------------------------------------------------------
@@ -236,14 +205,14 @@ def test_live_tick_in_mapped_host_memory():
         def tick():
             assert L.wf_wave_process_async(a.h, C.byref(wb), torch.cuda.current_stream().cuda_stream) == 0
 
-        g, _ = _capture(tick)
+        g, _ = capture(tick)
         for i in range(6):
             x = _samples(1, 2, hop, 300 + i, "f32")
             x_h[...] = x
             g.replay()
             torch.cuda.synchronize()
-            want = _host(b.process(_dev(x), 1, hop, want_db=False, want_pixels=True))
-            _assert_same({"silent": sil_h.copy(), "pixels": px_h.copy(), "min": min_h.copy()}, want, ("mapped", i))
+            want = to_host(b.process(_dev(x), 1, hop, want_db=False, want_pixels=True))
+            assert_bits_equal({"silent": sil_h.copy(), "pixels": px_h.copy(), "min": min_h.copy()}, want, ("mapped", i))
     finally:
         for p in (pin, ppx, pmin, psil):
             L.wf_host_free(p)
@@ -265,11 +234,11 @@ def test_rms_feed_and_waveform_chain_as_one_graph():
         return {"rms": rms, **w.process(x, T, hop, input_rms=rms, want_db=False, want_pixels=True)}
 
     xin = torch.zeros((S, cc, T * hop), device="cuda")
-    g, out = _capture(lambda: tick(*chains[0], xin))
+    g, out = capture(lambda: tick(*chains[0], xin))
     for i in range(6):
         x = _samples(S, cc, T * hop, 400 + i, "f32")
-        _replay(g, [xin], [x])
-        _assert_same(_host(out), _host(tick(*chains[1], _dev(x))), ("chain", i))
+        replay(g, [xin], [x])
+        assert_bits_equal(to_host(out), to_host(tick(*chains[1], _dev(x))), ("chain", i))
 
 
 # ---- 5. the per-tick kernel ------------------------------------------------------------------------------------------
@@ -277,16 +246,16 @@ def test_rms_feed_and_waveform_chain_as_one_graph():
 def test_per_tick_kernel_replays(monkeypatch):
     import torch
 
-    monkeypatch.setenv("WF_WAVE_CHUNK", "0")
+    set_knobs(monkeypatch, {"WF_WAVE_CHUNK": "0"})
     S, T, hop = 2, 3, 441
     settings = {"width": 301, "meter_buf": 40, "channel_mode": "stereo", "audio_sync_offset": 15}
     a, b = _twins(settings, 1, S)
     xin = torch.zeros((S, 1, T * hop), device="cuda")
-    g, out = _capture(lambda: a.process(xin, T, hop, want_points=True))
+    g, out = capture(lambda: a.process(xin, T, hop, want_points=True))
     for i in range(6):
         x = _samples(S, 1, T * hop, 500 + i, "f32")
-        _replay(g, [xin], [x])
-        _assert_same(_host(out), _host(b.process(_dev(x), T, hop, want_points=True)), ("per-tick", i))
+        replay(g, [xin], [x])
+        assert_bits_equal(to_host(out), to_host(b.process(_dev(x), T, hop, want_points=True)), ("per-tick", i))
 
 
 # ---- 6. buffer growth ------------------------------------------------------------------------------------------------
@@ -298,13 +267,13 @@ def test_larger_eager_call_after_a_capture_keeps_the_graph_working():
     settings = {"width": 800, "meter_buf": 150, "audio_sync_offset": 30}
     a, b = _twins(settings, 2, S)
     xin = torch.zeros((S, 2, T * hop), device="cuda")
-    g, out = _capture(lambda: a.process(xin, T, hop))
+    g, out = capture(lambda: a.process(xin, T, hop))
     for i in range(4):
         x = _samples(S, 2, T * hop, 600 + i, "f32")
-        _replay(g, [xin], [x])
-        _assert_same(_host(out), _host(b.process(_dev(x), T, hop)), ("replay", i))
+        replay(g, [xin], [x])
+        assert_bits_equal(to_host(out), to_host(b.process(_dev(x), T, hop)), ("replay", i))
         big = _dev(_samples(S, 2, (40 + 8 * i) * hop, 650 + i, "f32"))  # more plan space and a larger window each time
-        _assert_same(_host(a.process(big, 40 + 8 * i, hop)), _host(b.process(big, 40 + 8 * i, hop)), ("growth", i))
+        assert_bits_equal(to_host(a.process(big, 40 + 8 * i, hop)), to_host(b.process(big, 40 + 8 * i, hop)), ("growth", i))
 
 
 # ---- 7. refusals -----------------------------------------------------------------------------------------------------
@@ -327,13 +296,13 @@ def test_pageable_pcm_is_refused_under_capture_and_the_clock_stays():
         errors.append(ei.value)
         return c.process(xin, T, hop)
 
-    g, out = _capture(body)
+    g, out = capture(body)
     assert len(errors) == 1 and errors[0].status == WF_ERR_INVALID_ARG and "graph" in str(errors[0])
     x = _samples(S, 2, T * hop, 701, "f32")
-    _replay(g, [xin], [x])
-    _assert_same(_host(out), _host(d.process(_dev(x), T, hop)), "capture after the refusal")
+    replay(g, [xin], [x])
+    assert_bits_equal(to_host(out), to_host(d.process(_dev(x), T, hop)), "capture after the refusal")
     y = _dev(_samples(S, 2, T * hop, 702, "f32"))
-    _assert_same(_host(a.process(y, T, hop)), _host(b.process(y, T, hop)), "first eager call after the refusal")
+    assert_bits_equal(to_host(a.process(y, T, hop)), to_host(b.process(y, T, hop)), "first eager call after the refusal")
 
 
 # ---- 8. the reference's rows through replays -------------------------------------------------------------------------
@@ -352,11 +321,11 @@ def test_one_tick_graph_replays_reproduce_the_golden_rows(path):
     eng = WaveEngine(settings, channels=ch, max_streams=1, device_clock=True)
     xin = torch.zeros((1, ch, hop), device="cuda")
     rin = torch.zeros((1, 1), device="cuda")
-    g, o = _capture(lambda: eng.process(xin, 1, hop, input_rms=rin if rms is not None else None))
+    g, o = capture(lambda: eng.process(xin, 1, hop, input_rms=rin if rms is not None else None))
     rows, sil = [], []
     for t in range(T):
-        _replay(g, [xin, rin], [np.ascontiguousarray(z["pcm"][None, :, t * hop:(t + 1) * hop]),
-                                np.full((1, 1), 0.0 if rms is None else rms[t], np.float32)])
+        replay(g, [xin, rin], [np.ascontiguousarray(z["pcm"][None, :, t * hop:(t + 1) * hop]),
+                               np.full((1, 1), 0.0 if rms is None else rms[t], np.float32)])
         rows.append(o["out"].cpu().numpy()[0, 0])
         sil.append(int(o["silent"].cpu().numpy()[0, 0]))
     out, ref = np.stack(rows), z["out"]

@@ -14,8 +14,11 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from gpu_common import clean_knobs, set_knobs  # noqa: F401 (fixture)
 from helpers import synth_pcm
 from refdata import digest, reference
+
+pytestmark = pytest.mark.usefixtures("clean_knobs")
 
 GOLD = sorted((Path(__file__).parent / "golden").glob("meter_*.npz"))
 
@@ -242,7 +245,7 @@ def test_gpu_meter_one_pass_path_carries_block_partials(mode, monkeypatch):
     pcm[:, :, total // 3: total // 2] = 0.0
     outs = {}
     for name, env in (("fused", "1"), ("general", "0")):
-        monkeypatch.setenv("WF_METER_FUSED", env)
+        set_knobs(monkeypatch, {"WF_METER_FUSED": env})
         eng = MeterEngine(settings, channels=ch, max_streams=S, mode=eng_mode)
         pos, res = 0, []
         for i, (hop, T, sl) in enumerate(plan):

@@ -13,8 +13,11 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from gpu_common import clean_knobs, set_knobs  # noqa: F401 (fixture)
 from helpers import synth_pcm
 from refdata import digest, reference
+
+pytestmark = pytest.mark.usefixtures("clean_knobs")
 
 GOLD = sorted((Path(__file__).parent / "golden").glob("wave_*.npz"))
 
@@ -256,7 +259,7 @@ def _chunk_vs_per_tick(settings, ch, hop, S, T, monkeypatch):
         rms[2] = 10.0 ** (settings.get("volume_target", -8.0) / 20.0)  # compensation of exactly... whatever log10f gives
     outs = {}
     for chunk in ("1", "0"):
-        monkeypatch.setenv("WF_WAVE_CHUNK", chunk)
+        set_knobs(monkeypatch, {"WF_WAVE_CHUNK": chunk})
         eng = WaveEngine(settings, channels=ch, max_streams=S)
         a = eng.process(pcm[:, :, : 13 * hop], 13, hop, input_rms=None if rms is None else rms[:, :13])
         b = eng.process(pcm[:, :, 13 * hop:], T - 13, hop, input_rms=None if rms is None else rms[:, 13:])
