@@ -9,19 +9,10 @@
 // speed (the power-of-two kernels are the fast ones).  Everything after the FFT (split pass, magnitude, slope, EMA,
 // gate, dBFS, volume, roll-off, interpolation, Gaussian) restates the same reference lines as wf_kernels.cuh.
 #pragma once
+#include "wf_anyn.hpp"
 #include "wf_kernels.cuh"
 
 namespace wf {
-
-struct AnyPlan {
-    int M;          // N/2
-    int n_pass;
-    int radix[20];
-    float2 *scratch; // per-CTA [2][M] complex work buffers in global memory (L2) when they do not fit in shared
-                     // memory (N > ~27000, e.g. the plugin's "large FFT" sizes up to 65536); null = shared memory
-};
-
-constexpr int kAnyThreads = 256;
 
 template<int CC, typename TS>
 __global__ void __launch_bounds__(kAnyThreads) stft_anyn_kernel(const __grid_constant__ KParams p,

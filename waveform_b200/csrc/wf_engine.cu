@@ -17,10 +17,10 @@
 #include <vector>
 
 #include "wf_host.hpp"
-#include "wf_kernels.cuh"
-#include "wf_fast2048.cuh"
-#include "wf_anyn.cuh"
-#include "wf_v3.cuh"
+#include "wf_kparams.hpp"
+#include "wf_anyn.hpp"
+#include "wf_fast2048.hpp"
+#include "wf_fused.hpp"
 #include "wf_wide.hpp"
 #include "wf_v3.hpp"
 #include "wf_team2048.hpp"
@@ -414,40 +414,6 @@ Route choose_route(const wf_engine *e, const KParams &kp, const CallFacts &f)
             .smem = in_smem ? work + extra : extra, .scratch = !in_smem};
 }
 
-// stft_fused_kernel<N, CC, TS> with its CTA size and exchange buffers; *groups := streams per CTA
-template<int N, int CC, typename TS>
-KernelRef fused_kernel(int *groups)
-{
-    using G = Geo<N>;
-    *groups = G::GROUPS;
-    return {(const void *)stft_fused_kernel<N, CC, TS>, G::CTA, (size_t)G::GROUPS * G::BUF * sizeof(float2)};
-}
-
-template<int CC, typename TS>
-KernelRef fused_kernel(int N, int *groups)
-{
-    switch(N)
-    {
-    case 128: return fused_kernel<128, CC, TS>(groups);
-    case 256: return fused_kernel<256, CC, TS>(groups);
-    case 512: return fused_kernel<512, CC, TS>(groups);
-    case 1024: return fused_kernel<1024, CC, TS>(groups);
-    case 2048: return fused_kernel<2048, CC, TS>(groups);
-    case 4096: return fused_kernel<4096, CC, TS>(groups);
-    case 8192: return fused_kernel<8192, CC, TS>(groups);
-    case 16384: return fused_kernel<16384, CC, TS>(groups);
-    case 32768: return fused_kernel<32768, CC, TS>(groups);
-    default: return {};
-    }
-}
-
-// stft2048_fast_kernel<kMaxWarpsPerCta, TSM, GATE, EXTRA, TS>, indexed by TSM * 4 + GATE * 2 + EXTRA
-template<typename TS, int... I>
-std::array<const void *, sizeof...(I)> fast_kernels(std::integer_sequence<int, I...>)
-{
-    return {(const void *)stft2048_fast_kernel<fast::kMaxWarpsPerCta, (I & 4) != 0, (I & 2) != 0, (I & 1) != 0, TS>...};
-}
-
 // How a route launches: the kernel instantiation, its shape and launch mode, the argument it takes after KParams, and its
 // name (wf_last_kernel_name).
 struct Launch {
@@ -473,15 +439,11 @@ Launch plan_launch(const wf_engine *e, const Route &r, const KParams &kp, const 
     switch(r.family)
     {
     case Family::fast:
-    {
-        static const std::array kernels = {fast_kernels<float>(std::make_integer_sequence<int, 8>{}),
-                                           fast_kernels<int16_t>(std::make_integer_sequence<int, 8>{})};
-        l = {kernels[r.s16][r.tsm * 4 + r.gate * 2 + r.x], (unsigned)r.grid, r.w * 32u, (size_t)fast::smem_bytes(r.w),
-             {.pdl = true}};
+        k = fast2048_kernel(r.tsm, r.gate, r.x, r.s16);
+        l = {k.kernel, (unsigned)r.grid, r.w * 32u, (size_t)fast::smem_bytes(r.w), {.pdl = true}};
         snprintf(buf, sizeof buf, "stft2048_fast_kernel<%d,%d,%d,%d> grid %d x %d warps", fast::kMaxWarpsPerCta, (int)r.tsm,
                  (int)r.gate, r.x, r.grid, r.w);
         break;
-    }
     case Family::team:
         k = team2048_kernel(r.w, r.x, r.s16);
         l = {k.kernel, (unsigned)r.grid, k.block, k.smem, {.pdl = true}};
@@ -509,23 +471,17 @@ Launch plan_launch(const wf_engine *e, const Route &r, const KParams &kp, const 
         break;
     case Family::fused:
     {
-        static constexpr KernelRef (*kernels[2][2])(int, int *) = {{fused_kernel<1, float>, fused_kernel<2, float>},
-                                                                   {fused_kernel<1, int16_t>, fused_kernel<2, int16_t>}};
         int groups = 1;
-        k = kernels[r.s16][cc - 1](N, &groups);
+        k = fused_kernel(N, cc, r.s16, &groups);
         l = {k.kernel, (S + groups - 1) / groups, k.block, k.smem + display_smem(kp, f, groups)};
         snprintf(buf, sizeof buf, "stft_fused_kernel<%d,%d>", N, cc);
         break;
     }
     case Family::anyn:
-    {
-        static const void *const kernels[2][2] = {
-            {(const void *)stft_anyn_kernel<1, float>, (const void *)stft_anyn_kernel<2, float>},
-            {(const void *)stft_anyn_kernel<1, int16_t>, (const void *)stft_anyn_kernel<2, int16_t>}};
-        l = {kernels[r.s16][cc - 1], (unsigned)r.grid, kAnyThreads, r.smem, {}, Arg::any};
+        k = anyn_kernel(cc, r.s16);
+        l = {k.kernel, (unsigned)r.grid, k.block, r.smem, {}, Arg::any};
         snprintf(buf, sizeof buf, "stft_anyn_kernel<%d> N=%d", cc, N);
         break;
-    }
     }
     l.name = r.s16 ? std::string(buf) + " s16" : std::string(buf);
     return l;
@@ -539,9 +495,8 @@ int materialize_hold(wf_engine *e, cudaStream_t st)
         return WF_OK;
     const Tables &t = e->tab;
     const int S = t.cfg.max_streams;
-    materialize_hold_kernel<<<std::min(S, e->sm_count * 8), 256, 0, st>>>(e->d_state, e->d_hold, e->d_flags, S, t.B,
-                                                                          t.output_channels, t.db_min);
-    WF_CHECK(e, cudaGetLastError());
+    WF_CHECK(e, launch_kernel(materialize_hold_kernel, e->device, std::min(S, e->sm_count * 8), 256, 0, st, {}, e->d_state,
+                              e->d_hold, e->d_flags, S, t.B, t.output_channels, t.db_min));
     e->launches++;
     e->hold_implicit = e->hold_replayed;
     return WF_OK;
@@ -1050,7 +1005,7 @@ static int launch_range(wf_engine *e, const wf_batch *b, const BatchBufs &bufs, 
             sp.T = b->n_frames;
             sp.hop = b->hop;
         }
-        WF_CHECK(e, launch_splice(sp, count, cc, s16, st));
+        WF_CHECK(e, launch_splice(sp, e->device, count, cc, s16, st));
         e->launches++;
     }
     if(int rc = launch_route(e, r, l, kp, st))
@@ -1307,10 +1262,11 @@ int wf_reset_state(wf_engine *e, int32_t first, int32_t count)
     const bool below = !(t.db_min > (float)(t.cfg.floor_db - 10));
     const unsigned char fl = (unsigned char)(1u | (below ? 6u : 0u));
     const size_t B = (size_t)t.B;
-    spectrum_reset_kernel<<<std::min(count, e->sm_count * 8), 256, 0, e->stream>>>(
-        e->d_state + (size_t)first * t.cfg.capture_channels * B, e->d_hold + (size_t)first * t.output_channels * B, e->d_flags + first,
-        count, (int)(t.cfg.capture_channels * B), (int)(t.output_channels * B), (int)(t.display_channels * B), t.db_min, fl);
-    WF_CHECK(e, cudaGetLastError());
+    WF_CHECK(e, launch_kernel(spectrum_reset_kernel, e->device, std::min(count, e->sm_count * 8), 256, 0, e->stream, {},
+                              e->d_state + (size_t)first * t.cfg.capture_channels * B,
+                              e->d_hold + (size_t)first * t.output_channels * B, e->d_flags + first, count,
+                              (int)(t.cfg.capture_channels * B), (int)(t.output_channels * B), (int)(t.display_channels * B),
+                              t.db_min, fl));
     e->launches++;
     WF_CHECK(e, cudaStreamSynchronize(e->stream));
     return WF_OK;
@@ -1449,9 +1405,8 @@ int wf_peak_normalize(wf_engine *e, float *data, int32_t n_streams, int32_t n_fr
     WF_CHECK(e, time_begin(e, st));
     const long long rows = (long long)n_streams * n_frames * rows_per_frame;
     const int grid = (int)std::min<long long>(rows, (long long)e->sm_count * 16);
-    peak_normalize_kernel<<<grid, 256, 0, st>>>(d_data, n_streams, n_frames, rows_per_frame, row_len, d_peak, target_db,
-                                                max_gain);
-    WF_CHECK(e, cudaGetLastError());
+    WF_CHECK(e, launch_kernel(peak_normalize_kernel, e->device, grid, 256, 0, st, {}, d_data, n_streams, n_frames,
+                              rows_per_frame, row_len, d_peak, target_db, max_gain));
     e->launches++;
     WF_CHECK(e, time_end(e, st));
     if(dev)

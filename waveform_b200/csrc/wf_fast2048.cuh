@@ -16,24 +16,14 @@
 // Semantics are those of wf_kernels.cuh / src/source_generic.cpp:26-180; differences are confined to the
 // last-ulp behaviour of sqrt/log (well inside the 1e-5 parity bar, see DESIGN.md §Parity).
 #pragma once
+#include "wf_fast2048.hpp"
 #include "wf_kernels.cuh"
 
 namespace wf {
 
 namespace fast {
 
-constexpr int kN = 2048;
-constexpr int kM = 1024;
-// Per warp, in this order: the TMA landing buffer of the next frame (8 KiB); the padded transpose buffer, which after
-// pass B stages the frame's dB row for its bulk store (8448 B); the mbarrier and the split-mode hand-over flag (16 B).
-// Every part is 16-byte aligned.  The EMA state of the stream lives in registers.
-constexpr int kLandBytes = kN * 4;
-constexpr int kXposeBytes = 32 * 33 * 8;
-constexpr int kWarpBytes = kLandBytes + kXposeBytes + 16;
-constexpr int kTableBytes = (1024 + 1024 + 512) * 8;
-constexpr int kMaxWarpsPerCta = 12; // 1 CTA/SM: 12 warps x 16.3 KB + 20 KB tables = 215 KB of shared memory, 168 registers/thread
-constexpr int smem_bytes(int warps_per_cta) { return kTableBytes + warps_per_cta * kWarpBytes; }
-static_assert(smem_bytes(kMaxWarpsPerCta) <= 227 * 1024, "one CTA per SM must fit");
+// the kernel's shared-memory layout (kWarpBytes, kTableBytes, smem_bytes) is in wf_fast2048.hpp
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 

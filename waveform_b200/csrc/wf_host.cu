@@ -90,8 +90,7 @@ int fill_device(HostCore *c, float *p, long long n, float v, cudaStream_t st)
     if(n <= 0)
         return WF_OK;
     const int blocks = (int)std::min<long long>((n + 255) / 256, 1184);
-    fill_kernel<<<blocks, 256, 0, st>>>(p, n, v);
-    WF_CHECK(c, cudaGetLastError());
+    WF_CHECK(c, launch_kernel(fill_kernel, c->device, blocks, 256, 0, st, {}, p, n, v));
     c->launches++;
     return WF_OK;
 }
@@ -110,7 +109,7 @@ cudaError_t opt_in_smem(const void *kernel, int device, size_t bytes)
     return err;
 }
 
-cudaError_t launch_kernel(const void *kernel, int device, unsigned grid, unsigned block, size_t smem, cudaStream_t st,
+cudaError_t launch_kernel(const void *kernel, int device, dim3 grid, unsigned block, size_t smem, cudaStream_t st,
                           LaunchMode mode, void **args)
 {
     if(!kernel)
@@ -130,7 +129,7 @@ cudaError_t launch_kernel(const void *kernel, int device, unsigned grid, unsigne
         attr[n++].val.clusterDim = {mode.cluster, 1, 1};
     }
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
+    cfg.gridDim = grid;
     cfg.blockDim = dim3(block);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;

@@ -244,14 +244,15 @@ struct LaunchMode {
     unsigned cluster = 1;
 };
 
-// kernel<<<grid, block, smem, st>>>(*args[0], *args[1], ...) on `device` (the current one), opted in to `smem` first.  A
-// null kernel (no instantiation for the asked template arguments) is cudaErrorInvalidDeviceFunction.
-cudaError_t launch_kernel(const void *kernel, int device, unsigned grid, unsigned block, size_t smem, cudaStream_t st,
+// Launches kernel(*args[0], *args[1], ...) as `grid` CTAs of `block` threads with `smem` bytes of dynamic shared memory on
+// stream `st` of `device` (the current one), opted in to `smem` first.  A null kernel (no instantiation for the asked
+// template arguments) is cudaErrorInvalidDeviceFunction.
+cudaError_t launch_kernel(const void *kernel, int device, dim3 grid, unsigned block, size_t smem, cudaStream_t st,
                           LaunchMode mode, void **args);
 
 // The same for a typed kernel and its arguments.
 template<class... P, class... A>
-cudaError_t launch_kernel(void (*kernel)(P...), int device, unsigned grid, unsigned block, size_t smem, cudaStream_t st,
+cudaError_t launch_kernel(void (*kernel)(P...), int device, dim3 grid, unsigned block, size_t smem, cudaStream_t st,
                           LaunchMode mode, A &&...args)
 {
     return [&](P... a) {

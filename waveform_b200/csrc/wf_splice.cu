@@ -77,14 +77,10 @@ __global__ void __launch_bounds__(256) history_splice_kernel(const Splice p)
 
 } // namespace
 
-cudaError_t launch_splice(const Splice &s, int streams, int cc, bool s16, cudaStream_t st)
+cudaError_t launch_splice(const Splice &s, int device, int streams, int cc, bool s16, cudaStream_t st)
 {
-    const dim3 grid((unsigned)streams, (unsigned)cc);
-    if(s16)
-        history_splice_kernel<int16_t><<<grid, 256, 0, st>>>(s);
-    else
-        history_splice_kernel<float><<<grid, 256, 0, st>>>(s);
-    return cudaGetLastError();
+    return launch_kernel(s16 ? history_splice_kernel<int16_t> : history_splice_kernel<float>, device,
+                         dim3((unsigned)streams, (unsigned)cc), 256, 0, st, {}, s);
 }
 
 int splice_holdback(HostCore *c, float *hist, int R, int streams, int cc, long long L, long long wl, bool s16,
@@ -104,7 +100,7 @@ int splice_holdback(HostCore *c, float *hist, int R, int streams, int cc, long l
     sp.wl = wl;
     sp.L = L;
     sp.R = R;
-    WF_CHECK(c, launch_splice(sp, streams, cc, s16, st));
+    WF_CHECK(c, launch_splice(sp, c->device, streams, cc, s16, st));
     c->launches++;
     view = {window.p, cc * cs, cs};
     return WF_OK;

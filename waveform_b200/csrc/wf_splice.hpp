@@ -36,8 +36,8 @@ struct Splice {
     int T, hop;                              // ticks of the call, samples between ticks
 };
 
-// One CTA per (stream, channel) of `streams` x `cc`.  Returns the launch's error.
-cudaError_t launch_splice(const Splice &s, int streams, int cc, bool s16, cudaStream_t st);
+// One CTA per (stream, channel) of `streams` x `cc`, on stream `st` of `device`.  Returns the launch's error.
+cudaError_t launch_splice(const Splice &s, int device, int streams, int cc, bool s16, cudaStream_t st);
 
 // The window stride of `len` samples: rounded up to 16 bytes, so that a window keeps 16-byte alignment wherever the
 // kernels' own facts (hop, strides) allow it.

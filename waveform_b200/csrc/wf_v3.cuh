@@ -22,6 +22,7 @@
 // Reference semantics: src/source_generic.cpp:26-180 (see wf_kernels.cuh for the line-by-line citations).
 #pragma once
 #include "wf_kernels.cuh"
+#include "wf_v3.hpp"
 #include "wf_wide.cuh"
 #include "wf_fast2048.cuh"
 
@@ -62,12 +63,6 @@ struct Geo3 {
 #endif
     static constexpr int TPSM = (P <= 8) ? 1024 : WF_V3_TPSM; // resident threads per SM the register cap allows (64 / 128 registers)
     static constexpr int MINB = (TPSM / TN) > 0 ? (TPSM / TN) : 1;
-};
-
-struct Tw3 {
-    const float2 *tw1; // [A][TN]  W_M^(t*ka)
-    const float2 *tw2; // [B][C]   W_(B*C)^(c*kb)
-    const float2 *tw0; // split plan only: [16][TN] W_M^(a*TN + t) of the radix-2 first stage (tw1/tw2 are the half size's)
 };
 
 // Cluster sizes > 1 with N <= 8192 keep the magnitude inbox in its own double-buffered array: one cluster barrier per round

@@ -9,6 +9,14 @@
 
 namespace wf {
 struct KParams;
+namespace v3 {
+// the inter-pass twiddle tables (v3_build_twiddles) as the CTA-per-tick and N=16384 parity kernels take them after KParams
+struct Tw3 {
+    const float2 *tw1; // [A][TN]  W_M^(t*ka)
+    const float2 *tw2; // [B][C]   W_(B*C)^(c*kb)
+    const float2 *tw0; // split plan only: [16][TN] W_M^(a*TN + t) of the radix-2 first stage (tw1/tw2 are the half size's)
+};
+} // namespace v3
 int v3_min_cluster(int N); // smallest supported cluster size (1, or 2 where the per-thread state would not fit registers)
 // Inter-pass twiddle tables (interleaved re,im), evaluated in double: tw1[ka][t] = W_M^(t*ka), tw2[kb][c] = W_(BC)^(c*kb);
 // tw0 (16384 only) = W_M^(a*TN + t) of the radix-2 first stage, tw1/tw2 then belong to the 4096-point sub-FFTs.  All three
