@@ -82,6 +82,8 @@ struct wf_engine : HostCore {
     DevBuf<float> s_scratch; // any-N kernel work buffers when N/2 complex points x 2 exceed shared memory
     DevBuf<float> s_render;  // wf_render: one dB row per group when a row does not fit in shared memory
     DevBuf<float> s_window;  // frames of a ring call in the plain layout, in the call's sample type (counts floats, as s_pcm)
+    DevBuf<unsigned char> s_state; // staging of wf_get_state / wf_set_state (StateSections)
+    std::vector<unsigned char> h_state;
     // zero-copy verdict of the last host-pointer batch (live ticks reuse the same buffers every call): pcm, then the
     // buffers of batch_bufs
     static constexpr int kBatchBufs = 8;
@@ -136,6 +138,40 @@ static __global__ void spectrum_reset_kernel(float *state, float *hold_db, unsig
         __syncthreads();
         if(threadIdx.x == 0)
             flags[s] = new_flags;
+    }
+}
+
+// wf_get_state / wf_set_state, one CTA per stream of [0, count) (the device arrays start at the first): the state to or from
+// the staging sections x_* (null = skipped).  Restored hold rows set the display bits the kernels keep, and flags bit 0.
+template<bool SET>
+static __device__ void copy_section(float *dev, float *x, long long off, long long n)
+{
+    for(long long k = off + threadIdx.x; x && k < off + n; k += blockDim.x)
+        (SET ? dev[k] : x[k]) = (SET ? x[k] : dev[k]);
+}
+template<bool SET>
+static __global__ void spectrum_state_kernel(float *state, float *hold, unsigned char *flags, float *x_tsmooth, float *x_hold,
+                                             unsigned char *x_flags, int count, int cc, int och, int dch, int B, float thr)
+{
+    const long long ts = (long long)cc * B, hs = (long long)och * B;
+    for(int i = blockIdx.x; i < count; i += gridDim.x)
+    {
+        copy_section<SET>(state, x_tsmooth, i * ts, ts);
+        copy_section<SET>(hold, x_hold, i * hs, hs);
+        unsigned bits = (dch == 1) ? 4u : 0u;
+        for(int d = 0; SET && x_hold && d < dch; ++d)
+        {
+            bool above = false;
+            for(int k = threadIdx.x; k < B; k += blockDim.x)
+                above |= x_hold[i * hs + (long long)d * B + k] > thr;
+            bits |= __syncthreads_or(above) ? 0u : 2u << d; // every bin of row d <= floor_db - 10
+        }
+        if(threadIdx.x == 0 && !SET && x_flags)
+            x_flags[i] = flags[i] & 1u;
+        if(threadIdx.x == 0 && SET && x_hold)
+            flags[i] = (unsigned char)((flags[i] & 1u) | bits);
+        if(threadIdx.x == 0 && SET && x_flags)
+            flags[i] = (unsigned char)((flags[i] & ~1u) | (x_flags[i] & 1u));
     }
 }
 
@@ -556,8 +592,8 @@ int ring_access(wf_engine *e, int32_t first, int32_t count, const void *samples)
 {
     if(!e)
         return WF_ERR_INVALID_ARG;
-    if(first < 0 || count < 0 || (int64_t)first + count > e->tab.cfg.max_streams)
-        return fail(e, WF_ERR_CAPACITY, "ring range out of bounds");
+    if(int rc = check_slot_range(e, first, count, e->tab.cfg.max_streams, "ring"))
+        return rc;
     if(count > 0 && !samples)
         return fail(e, WF_ERR_INVALID_ARG, "samples is null");
     WF_CHECK(e, cudaSetDevice(e->device));
@@ -565,6 +601,38 @@ int ring_access(wf_engine *e, int32_t first, int32_t count, const void *samples)
         return rc;
     WF_CHECK(e, cudaStreamSynchronize(e->stream));
     return WF_OK;
+}
+
+// wf_get_state (set = false) / wf_set_state (set = true): one copy and one launch, not counted as one of the engine's
+int spectrum_state(wf_engine *e, int32_t first, int32_t count, const float *tsmooth, const float *hold_db,
+                   const uint8_t *flags, bool set)
+{
+    if(!e)
+        return WF_ERR_INVALID_ARG;
+    const Tables &t = e->tab;
+    if(int rc = check_slot_range(e, first, count, t.cfg.max_streams, "state"))
+        return rc;
+    WF_CHECK(e, cudaSetDevice(e->device));
+    if(int rc = materialize_hold(e, e->stream))
+        return rc;
+    WF_CHECK(e, cudaStreamSynchronize(e->stream));
+    const size_t n = (size_t)count, cc = (size_t)t.cfg.capture_channels, och = (size_t)t.output_channels, B = (size_t)t.B;
+    StateSections io;
+    const int i_tsmooth = io.add(tsmooth, n * cc * B * sizeof(float));
+    const int i_hold = io.add(hold_db, n * och * B * sizeof(float));
+    const int i_flags = io.add(flags, n);
+    if(io.empty())
+        return WF_OK;
+    if(int rc = io.reserve(e, e->s_state, e->h_state))
+        return rc;
+    // the legacy default stream orders the state call after the work callers enqueued on blocking streams (torch's default)
+    return io.run(e, cudaStreamLegacy, set, [&] {
+        return launch_kernel(set ? spectrum_state_kernel<true> : spectrum_state_kernel<false>, e->device,
+                             std::min(count, e->sm_count * 8), 256, 0, cudaStreamLegacy, {}, e->d_state + first * cc * B,
+                             e->d_hold + first * och * B, e->d_flags + first, io.dev<float>(i_tsmooth),
+                             io.dev<float>(i_hold), io.dev<unsigned char>(i_flags), count, (int)cc, (int)och,
+                             t.display_channels, (int)B, (float)(t.cfg.floor_db - 10));
+    });
 }
 
 } // namespace
@@ -1032,9 +1100,8 @@ int wf_process_async(wf_engine *e, const wf_batch *b_in, void *cuda_stream)
     const int cc = t.cfg.capture_channels, N = t.N;
     if(b->n_streams < 0 || b->n_frames < 0 || b->hop < 1)
         return fail(e, WF_ERR_INVALID_ARG, "n_streams/n_frames must be >= 0 and hop >= 1");
-    if(b->first_stream < 0 || (int64_t)b->first_stream + b->n_streams > t.cfg.max_streams)
-        return fail(e, WF_ERR_CAPACITY, "streams [%d, %d) exceed max_streams %d", b->first_stream,
-                       b->first_stream + b->n_streams, t.cfg.max_streams);
+    if(int rc = check_slot_range(e, b->first_stream, b->n_streams, t.cfg.max_streams, "stream"))
+        return rc;
     if(b->n_streams == 0 || b->n_frames == 0)
         return WF_OK;
     if(!b->pcm)
@@ -1251,8 +1318,8 @@ int wf_reset_state(wf_engine *e, int32_t first, int32_t count)
 {
     if(!e)
         return WF_ERR_INVALID_ARG;
-    if(first < 0 || count < 0 || (int64_t)first + count > e->tab.cfg.max_streams)
-        return fail(e, WF_ERR_CAPACITY, "reset range out of bounds");
+    if(int rc = check_slot_range(e, first, count, e->tab.cfg.max_streams, "reset"))
+        return rc;
     if(count == 0)
         return WF_OK;
     WF_CHECK(e, cudaSetDevice(e->device));
@@ -1274,30 +1341,7 @@ int wf_reset_state(wf_engine *e, int32_t first, int32_t count)
 
 int wf_get_state(wf_engine *e, int32_t first, int32_t count, float *tsmooth, float *hold_db, uint8_t *flags)
 {
-    if(!e)
-        return WF_ERR_INVALID_ARG;
-    const Tables &t = e->tab;
-    if(first < 0 || count < 0 || (int64_t)first + count > t.cfg.max_streams)
-        return fail(e, WF_ERR_CAPACITY, "state range out of bounds");
-    WF_CHECK(e, cudaSetDevice(e->device));
-    {
-        const int rc = materialize_hold(e, e->stream);
-        if(rc)
-            return rc;
-    }
-    WF_CHECK(e, cudaStreamSynchronize(e->stream));
-    const size_t cc = (size_t)t.cfg.capture_channels, och = (size_t)t.output_channels, B = (size_t)t.B;
-    if(tsmooth)
-        WF_CHECK(e, cudaMemcpy(tsmooth, e->d_state + first * cc * B, count * cc * B * sizeof(float), cudaMemcpyDeviceToHost));
-    if(hold_db)
-        WF_CHECK(e, cudaMemcpy(hold_db, e->d_hold + first * och * B, count * och * B * sizeof(float), cudaMemcpyDeviceToHost));
-    if(flags)
-    {
-        WF_CHECK(e, cudaMemcpy(flags, e->d_flags + first, (size_t)count, cudaMemcpyDeviceToHost));
-        for(int i = 0; i < count; ++i)
-            flags[i] &= 1u;
-    }
-    return WF_OK;
+    return spectrum_state(e, first, count, tsmooth, hold_db, flags, false);
 }
 
 int wf_get_ring(wf_engine *e, int32_t first, int32_t count, float *samples)
@@ -1327,53 +1371,7 @@ int wf_set_ring(wf_engine *e, int32_t first, int32_t count, const float *samples
 int wf_set_state(wf_engine *e, int32_t first, int32_t count, const float *tsmooth, const float *hold_db,
                  const uint8_t *flags)
 {
-    if(!e)
-        return WF_ERR_INVALID_ARG;
-    const Tables &t = e->tab;
-    if(first < 0 || count < 0 || (int64_t)first + count > t.cfg.max_streams)
-        return fail(e, WF_ERR_CAPACITY, "state range out of bounds");
-    WF_CHECK(e, cudaSetDevice(e->device));
-    {
-        const int rc = materialize_hold(e, e->stream);
-        if(rc)
-            return rc;
-    }
-    WF_CHECK(e, cudaStreamSynchronize(e->stream));
-    const size_t cc = (size_t)t.cfg.capture_channels, och = (size_t)t.output_channels, B = (size_t)t.B;
-    if(tsmooth)
-        WF_CHECK(e, cudaMemcpy(e->d_state + first * cc * B, tsmooth, count * cc * B * sizeof(float), cudaMemcpyHostToDevice));
-    std::vector<unsigned char> fl((size_t)count);
-    WF_CHECK(e, cudaMemcpy(fl.data(), e->d_flags + first, (size_t)count, cudaMemcpyDeviceToHost));
-    if(hold_db)
-    {
-        WF_CHECK(e, cudaMemcpy(e->d_hold + first * och * B, hold_db, count * och * B * sizeof(float), cudaMemcpyHostToDevice));
-        const float thr = (float)(t.cfg.floor_db - 10);
-        for(int s = 0; s < count; ++s)
-        {
-            unsigned char bits = 0;
-            for(int d = 0; d < t.display_channels; ++d)
-            {
-                bool all_below = true;
-                const float *row = hold_db + ((size_t)s * och + d) * B;
-                for(size_t k = 0; k < B; ++k)
-                    if(row[k] > thr)
-                    {
-                        all_below = false;
-                        break;
-                    }
-                if(all_below)
-                    bits |= (unsigned char)(2u << d);
-            }
-            if(t.display_channels == 1)
-                bits |= 4u;
-            fl[s] = (unsigned char)((fl[s] & 1u) | bits);
-        }
-    }
-    if(flags)
-        for(int s = 0; s < count; ++s)
-            fl[s] = (unsigned char)((fl[s] & ~1u) | (flags[s] & 1u));
-    WF_CHECK(e, cudaMemcpy(e->d_flags + first, fl.data(), (size_t)count, cudaMemcpyHostToDevice));
-    return WF_OK;
+    return spectrum_state(e, first, count, tsmooth, hold_db, flags, true);
 }
 
 int wf_peak_normalize(wf_engine *e, float *data, int32_t n_streams, int32_t n_frames, int32_t row_len,

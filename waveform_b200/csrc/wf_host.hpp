@@ -45,6 +45,16 @@ struct HostCore {
 // Keeps the message for wf_*last_error (when there is an engine) and returns `code`.
 int fail(HostCore *c, int code, const char *fmt, ...) __attribute__((format(printf, 3, 4)));
 
+// WF_ERR_CAPACITY, with a message naming the range, unless slots [first, first + count) of `max_streams` exist (count >= 0).
+// `what` names the call's kind of range ("stream", "state", "reset", "ring").
+inline int check_slot_range(HostCore *c, int32_t first, int32_t count, int max_streams, const char *what)
+{
+    if(first < 0 || count < 0 || (int64_t)first + count > max_streams)
+        return fail(c, WF_ERR_CAPACITY, "%s range [%d, %lld) exceeds max_streams %d", what, first, (long long)first + count,
+                    max_streams);
+    return WF_OK;
+}
+
 // Returns WF_ERR_OOM / WF_ERR_CUDA from the calling function, with the failing call and CUDA's reason as the message,
 // unless `call` succeeds.
 #define WF_CHECK(core, call)                                                                                       \
@@ -353,7 +363,7 @@ class Staging {
 // that the call makes one copy and one launch.  add() places a section 16-byte aligned (null or empty: skipped); after
 // reserve(), dev() gives a section's device pointer (null when skipped).  run() does the call on `st`: a set call packs
 // the sections, copies them to the device and launches; a get call launches, copies them back and unpacks them.  The
-// stream is synchronised before it returns, and the launch counts as one of the engine's.
+// stream is synchronised before it returns.  Whether the launch counts as one of the engine's is the caller's choice.
 class StateSections {
   public:
     int add(const void *host, size_t bytes)
@@ -391,7 +401,6 @@ class StateSections {
             WF_CHECK(c, cudaMemcpyAsync(dbase, hbase, total, cudaMemcpyHostToDevice, st));
         }
         WF_CHECK(c, launch());
-        c->launches++;
         if(!set)
             WF_CHECK(c, cudaMemcpyAsync(hbase, dbase, total, cudaMemcpyDeviceToHost, st));
         WF_CHECK(c, cudaStreamSynchronize(st));

@@ -803,9 +803,8 @@ int wf_meter_process_async(wf_meter *m, const wf_meter_batch *b_in, void *cuda_s
                                                : "display outputs need an engine created with display settings");
     if(b->n_streams < 0 || b->n_ticks < 0 || b->hop < 1)
         return wf::fail(m, WF_ERR_INVALID_ARG, "n_streams/n_ticks must be >= 0 and hop >= 1");
-    if(b->first_stream < 0 || (int64_t)b->first_stream + b->n_streams > m->cfg.max_streams)
-        return wf::fail(m, WF_ERR_CAPACITY, "streams [%d, %d) exceed max_streams %d", b->first_stream,
-                    b->first_stream + b->n_streams, m->cfg.max_streams);
+    if(int rc = wf::check_slot_range(m, b->first_stream, b->n_streams, m->cfg.max_streams, "stream"))
+        return rc;
     if(b->n_streams == 0 || b->n_ticks == 0)
         return WF_OK;
     if(!b->pcm)
@@ -960,8 +959,8 @@ int wf_meter_reset(wf_meter *m, int32_t first, int32_t count)
 {
     if(!m)
         return WF_ERR_INVALID_ARG;
-    if(first < 0 || count < 0 || (int64_t)first + count > m->cfg.max_streams)
-        return wf::fail(m, WF_ERR_CAPACITY, "reset range out of bounds");
+    if(int rc = wf::check_slot_range(m, first, count, m->cfg.max_streams, "reset"))
+        return rc;
     if(count == 0)
         return WF_OK;
     WF_CHECK(m, cudaSetDevice(m->device));
@@ -984,9 +983,8 @@ int meter_state(wf_meter *m, int32_t first, int32_t count, const float *ring, co
 {
     if(!m)
         return WF_ERR_INVALID_ARG;
-    if(first < 0 || count < 0 || (int64_t)first + count > m->cfg.max_streams)
-        return wf::fail(m, WF_ERR_CAPACITY, "state range [%d, %lld) exceeds max_streams %d", first, (long long)first + count,
-                        m->cfg.max_streams);
+    if(int rc = wf::check_slot_range(m, first, count, m->cfg.max_streams, "state"))
+        return rc;
     const size_t n = (size_t)count, cc = (size_t)m->cfg.capture_channels;
     wf::StateSections io;
     const int i_ring = io.add(ring, n * cc * m->W * sizeof(float));
@@ -1017,8 +1015,10 @@ int meter_state(wf_meter *m, int32_t first, int32_t count, const float *ring, co
     q.D = m->D;
     const int grid = std::min(count, m->sm_count * 4);
     return io.run(m, m->stream, set, [&] {
-        return wf::launch_kernel(set ? meter_state_kernel<true> : meter_state_kernel<false>, m->device, grid, 256, 0,
-                                 m->stream, {}, q);
+        const cudaError_t err = wf::launch_kernel(set ? meter_state_kernel<true> : meter_state_kernel<false>, m->device,
+                                                  grid, 256, 0, m->stream, {}, q);
+        m->launches += (err == cudaSuccess);
+        return err;
     });
 }
 

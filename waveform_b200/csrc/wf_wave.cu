@@ -1641,9 +1641,8 @@ int wave_state(wf_wave *w, int32_t first, int32_t count, const float *db, const 
 {
     if(!w)
         return WF_ERR_INVALID_ARG;
-    if(first < 0 || count < 0 || (int64_t)first + count > w->cfg.max_streams)
-        return wf::fail(w, WF_ERR_CAPACITY, "state range [%d, %lld) exceeds max_streams %d", first, (long long)first + count,
-                        w->cfg.max_streams);
+    if(int rc = wf::check_slot_range(w, first, count, w->cfg.max_streams, "state"))
+        return rc;
     const size_t n = (size_t)count, cc = (size_t)w->cfg.capture_channels;
     wf::StateSections io;
     const int i_db = io.add(db, n * w->och * w->cfg.width * sizeof(float));
@@ -1669,8 +1668,10 @@ int wave_state(wf_wave *w, int32_t first, int32_t count, const float *db, const 
     q.D = w->D;
     const int grid = std::min(count, w->sm_count * 4);
     return io.run(w, w->stream, set, [&] {
-        return wf::launch_kernel(set ? wave_state_kernel<true> : wave_state_kernel<false>, w->device, grid, 256, 0,
-                                 w->stream, {}, q);
+        const cudaError_t err = wf::launch_kernel(set ? wave_state_kernel<true> : wave_state_kernel<false>, w->device,
+                                                  grid, 256, 0, w->stream, {}, q);
+        w->launches += (err == cudaSuccess);
+        return err;
     });
 }
 
