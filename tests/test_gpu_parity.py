@@ -344,7 +344,7 @@ def test_wide_kernel_is_bit_identical_to_one_group_kernel(settings, channels, ho
     """Distributing a stream's bins over a cluster must not change a single bit: the recurrences are only
     distributed, never reassociated.  Also checks both against the oracle.  v3 = "1": the CTA-per-tick kernel
     (csrc/wf_v3.cuh, cluster size 1 vs R; 16384 has no size-1 variant, so 2 vs R); "0": the first-generation pair
-    (wf_kernels.cuh vs wf_wide.cuh)."""
+    (wf_fused.cuh vs wf_wide.cuh)."""
     import torch
     from waveform_b200 import Engine
 

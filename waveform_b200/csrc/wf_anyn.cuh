@@ -7,7 +7,7 @@
 //     out[o] = sum_u in[j + u*M/r] * W_M^(u*step),   step = low*M/(Ns*r) + t*M/r   (pass twiddle x radix-r DFT matrix)
 // — O(M * sum(r)) multiply-adds per frame instead of hand-unrolled butterflies: this path favours generality over
 // speed (the power-of-two kernels are the fast ones).  Everything after the FFT (split pass, magnitude, slope, EMA,
-// gate, dBFS, volume, roll-off, interpolation, Gaussian) restates the same reference lines as wf_kernels.cuh.
+// gate, dBFS, volume, roll-off, interpolation, Gaussian) restates the same reference lines as wf_fused.cuh.
 #pragma once
 #include "wf_anyn.hpp"
 #include "wf_kernels.cuh"
@@ -158,7 +158,7 @@ __global__ void __launch_bounds__(kAnyThreads) stft_anyn_kernel(const __grid_con
                     const float2 dif = csub(a, b);
                     const float2 o = make_float2(dif.y, -dif.x);
                     const float2 y = cadd(sum, cmul(o, __ldg(p.tw_post + k)));
-                    float mag = sqrt_mufu(fmaf(y.x, y.x, y.y * y.y)) * p.coef_half;
+                    float mag = sqrt_approx(fmaf(y.x, y.x, y.y * y.y)) * p.coef_half;
                     if(p.slope != nullptr)
                         mag *= __ldg(p.slope + k);
                     if(p.tsmooth)

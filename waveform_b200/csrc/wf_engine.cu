@@ -27,6 +27,7 @@
 #include "wf_warp2.hpp"
 #include "wf_par16384.hpp"
 #include "wf_render.hpp"
+#include "wf_sm90.cuh"
 #include "wf_splice.hpp"
 #include "wf_nvtx.hpp"
 #include "wf_tables.hpp"
@@ -111,8 +112,7 @@ static __global__ void materialize_hold_kernel(const float *state, float *hold_d
             continue;
         for(int k = threadIdx.x; k < B; k += blockDim.x)
         {
-            float l;
-            asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(l) : "f"(state[(size_t)s * B + k]));
+            const float l = lg2_approx_ftz(state[(size_t)s * B + k]);
             hold_db[(size_t)s * och * B + k] = fmaxf(l * 6.02059991327962390f, db_min);
         }
         __syncthreads();

@@ -1,7 +1,7 @@
 // wf_fused.cu — instantiations of stft_fused_kernel (its own translation unit)
 #include "wf_host.hpp"
 #include "wf_fused.hpp"
-#include "wf_kernels.cuh"
+#include "wf_fused.cuh"
 
 namespace wf {
 

@@ -1,4 +1,4 @@
-// wf_fused.hpp — host interface of the fused kernel of the power-of-two sizes (stft_fused_kernel, wf_kernels.cuh)
+// wf_fused.hpp — host interface of the fused kernel of the power-of-two sizes (stft_fused_kernel, wf_fused.cuh)
 #pragma once
 #include "wf_host.hpp"
 

@@ -38,7 +38,6 @@ constexpr size_t smem_bytes() { return kBufBytes + kStageBytes + 16; }
 template<bool EXTRA, int r, typename TS>
 __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &tw, unsigned char *smem_raw, unsigned (*redf)[2])
 {
-    using namespace wide;
     using namespace par16384;
     constexpr int B = kBins, TN = kTN, P = kP, HP = kHP, MS = kSub;
     float2 *buf = reinterpret_cast<float2 *>(smem_raw);
@@ -96,8 +95,8 @@ __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &t
     uint32_t phase = 0;
     if(tid == 0)
     {
-        fast::mbar_init(mbar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_init(mbar, 1);
+        fence_mbarrier_init();
     }
     __syncthreads();
     // distributed shared memory (the lazy gate reduction) may only be addressed once both CTAs of the cluster are running
@@ -105,8 +104,8 @@ __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &t
     cluster_wait();
     if(use_tma && T > 0 && tid == 0)
     {
-        fast::mbar_expect_tx(mbar, kFrameBytes);
-        fast::tma_load_1d(const_cast<unsigned char *>(stage), pcm_s, kFrameBytes, mbar);
+        mbar_expect_tx(mbar, kFrameBytes);
+        tma_load_1d(const_cast<unsigned char *>(stage), pcm_s, kFrameBytes, mbar);
     }
     const pk::c64 *win = reinterpret_cast<const pk::c64 *>(p.window2) + tid; // pairs (w[2n], w[2n+1]), n = a*TN + tid
     const pk::c64 *tw0 = reinterpret_cast<const pk::c64 *>(tw.tw0) + tid;    // W_8192^(a*TN + tid)
@@ -123,7 +122,7 @@ __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &t
         unsigned long long nzbits = 0;
         if(use_tma)
         {
-            fast::mbar_wait(mbar, phase);
+            mbar_wait(mbar, phase);
             phase ^= 1u;
             // (the rank test sits outside the unrolled loops: inside, ptxas if-converts both variants into predicated code)
             if(r == 0)
@@ -159,9 +158,9 @@ __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &t
             __syncthreads(); // every thread has taken its samples: the staging area can receive the next frame
             if(tid == 0 && t + 1 < T)
             {
-                fast::fence_proxy_async();
-                fast::mbar_expect_tx(mbar, kFrameBytes);
-                fast::tma_load_1d(const_cast<unsigned char *>(stage), frame + p.hop, kFrameBytes, mbar);
+                fence_proxy_async();
+                mbar_expect_tx(mbar, kFrameBytes);
+                tma_load_1d(const_cast<unsigned char *>(stage), frame + p.hop, kFrameBytes, mbar);
             }
         }
         else
@@ -255,7 +254,7 @@ __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &t
                     const float pm = 4.0f * (pk::re(sq) + pk::im(sq));
                     p2 = (r == 0 && tid == 0) ? pm : p2;
                 }
-                pk::c64 m = pk::mul(pk::make(fast::sqrt_approx(p1), fast::sqrt_approx(p2)), pk::make(p.coef_half, p.coef_half));
+                pk::c64 m = pk::mul(pk::make(sqrt_approx_ftz(p1), sqrt_approx_ftz(p2)), pk::make(p.coef_half, p.coef_half));
                 if(EXTRA && p.slope != nullptr)
                     m = pk::mul(m, pk::make(__ldg(p.slope + 2 * k1 + r), __ldg(p.slope + 2 * k2 + r)));
                 if(tsm)
@@ -267,7 +266,7 @@ __device__ __forceinline__ void par16384_body(const KParams &p, const v3::Tw3 &t
                 }
                 pk::split(m, st[2 * j], st[2 * j + 1]);
                 float d1, d2;
-                pk::split(fast::dbfs2(st[2 * j], st[2 * j + 1], p.db_min), d1, d2);
+                pk::split(dbfs2(st[2 * j], st[2 * j + 1], p.db_min), d1, d2);
                 if(EXTRA)
                 {
                     if(p.normalize)
@@ -372,7 +371,7 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(par16384::kTN, 2)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ unsigned redf[2][2]; // [parity of the exchange][rank]: this rank's "all my outputs <= floor-10 dB"
-    if(wide::cluster_ctarank() == 0)
+    if(cluster_ctarank() == 0)
         par16384_body<EXTRA, 0, TS>(p, tw, smem_raw, redf);
     else
         par16384_body<EXTRA, 1, TS>(p, tw, smem_raw, redf);

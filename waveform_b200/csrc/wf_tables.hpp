@@ -2,7 +2,7 @@
 //
 // This is the engine's equivalent of what WAVSource::update() computes once per settings change
 // (reference: src/source.cpp:1077-1322).  Setup is host work in the reference and stays host work here;
-// the per-frame hot path (wf_kernels.cuh) only reads these tables from device memory.
+// the per-frame hot path (the spectrum kernels) only reads these tables from device memory.
 //
 // All float expressions follow the reference's operation order so that tables are bit-identical on
 // glibc (tests/test_tables.py checks that against the compiled reference).  Compiled with

@@ -18,7 +18,8 @@
 // Recurrences are distributed over bins, never reassociated: results are bit-identical to wf_fast2048.cuh.
 // Semantics: src/source_generic.cpp:26-180 as restated there.
 #pragma once
-#include "wf_fast2048.cuh"
+#include "wf_fast2048.hpp"
+#include "wf_kernels.cuh"
 
 namespace wf {
 
@@ -29,24 +30,18 @@ constexpr int kWarpBufBytes = 32 * 33 * 8;                  // padded transpose 
 constexpr int kMagBytes = 1024 * 4;                         // the warp's tick: linear magnitudes
 constexpr int kWarpBytes = kWarpBufBytes + kMagBytes + 16;  // + mbarrier
 constexpr int smem_bytes() { return fast::kTableBytes + kWarps * kWarpBytes + kWarps * kCtlBytes; }
-
-__device__ __forceinline__ void bar_sync(int id, int nthreads)
-{
-    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
 } // namespace team
 
 template<int W, bool EXTRA, typename TS>
 __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(const __grid_constant__ KParams p)
 {
-    using namespace fast;
     using PS = Pcm<TS>;
-    constexpr uint32_t kFrameBytes = PS::frame_bytes(kN); // TMA transfer of one frame
+    constexpr uint32_t kFrameBytes = PS::frame_bytes(fast::kN); // TMA transfer of one frame
     constexpr int TPC = team::kWarps / W; // teams per CTA
-    constexpr int BW = kM / W;            // bins per warp in phase 2
+    constexpr int BW = fast::kM / W;      // bins per warp in phase 2
     constexpr int BPL = BW / 32;          // bins per lane: 2, 4, 8, 16
     constexpr int VEC = (BPL >= 4) ? 4 : 2;
-    constexpr int B = kM;
+    constexpr int B = fast::kM;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float2 *s_win = reinterpret_cast<float2 *>(smem_raw);
     float2 *s_twA = s_win + 1024; // [k2][n1] = W_1024^(k2*n1)
@@ -76,11 +71,11 @@ __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(con
     if(lane == 0)
     {
         mbar_init(mbar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        fence_mbarrier_init();
     }
     __syncthreads();
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    asm volatile("griddepcontrol.wait;" ::: "memory");
+    pdl_launch_dependents();
+    pdl_wait();
 
     // streams are dealt round-robin to CTAs first, then to the CTA's teams: stream of (cta c, team tm, i) = c + G*(tm + TPC*i)
     const int S = p.n_streams, T = p.n_frames;
@@ -141,12 +136,12 @@ __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(con
             const bool wv = __all_sync(0xffffffffu, v);
             if(lane == 0)
                 ctl_outs[wi] = wv ? 1 : 0;
-            team::bar_sync(bar_id, W * 32);
+            bar_sync(bar_id, W * 32);
             bool r = true;
 #pragma unroll
             for(int i = 0; i < W; ++i)
                 r &= ctl_outs[i] != 0;
-            team::bar_sync(bar_id, W * 32);
+            bar_sync(bar_id, W * 32);
             return r;
         };
 
@@ -232,7 +227,7 @@ __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(con
                         const float p512 = 4.0f * (pk::re(sq) + pk::im(sq));
                         p2 = (lane == 0) ? p512 : p2;
                     }
-                    float m1 = sqrt_approx(p1), m2 = sqrt_approx(p2);
+                    float m1 = sqrt_approx_ftz(p1), m2 = sqrt_approx_ftz(p2);
                     if(EXTRA && p.slope != nullptr)
                     {
                         m1 *= __ldg(p.slope + k1);
@@ -244,7 +239,7 @@ __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(con
                 if(lane == 0)
                     ctl_nz[wi] = nz ? 1 : 0;
             }
-            team::bar_sync(bar_id, W * 32);
+            bar_sync(bar_id, W * 32);
 
             // =================== phase 2: this warp's bin slice through the round's ticks, in order ===================
             // Common case — a full round, every frame has signal, no skip mask: straight-line code for the W ticks (the
@@ -333,11 +328,9 @@ __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(con
                         for(int j = 0; j < BPL; j += VEC)
                         {
                             if constexpr(VEC == 4)
-                                asm volatile("st.global.cs.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(odb + j), "f"(d[j]), "f"(d[j + 1]),
-                                             "f"(d[j + 2]), "f"(d[j + 3])
-                                             : "memory");
+                                stg_stream_v4(odb + j, d[j], d[j + 1], d[j + 2], d[j + 3]);
                             else
-                                asm volatile("st.global.cs.v2.f32 [%0], {%1, %2};" ::"l"(odb + j), "f"(d[j]), "f"(d[j + 1]) : "memory");
+                                stg_stream_v2(odb + j, d[j], d[j + 1]);
                         }
                         if(i == W - 1)
                         {
@@ -506,11 +499,9 @@ __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(con
                 for(int j = 0; j < BPL; j += VEC)
                 {
                     if constexpr(VEC == 4)
-                        asm volatile("st.global.cs.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(odb + j), "f"(d[j]), "f"(d[j + 1]), "f"(d[j + 2]),
-                                     "f"(d[j + 3])
-                                     : "memory");
+                        stg_stream_v4(odb + j, d[j], d[j + 1], d[j + 2], d[j + 3]);
                     else
-                        asm volatile("st.global.cs.v2.f32 [%0], {%1, %2};" ::"l"(odb + j), "f"(d[j]), "f"(d[j + 1]) : "memory");
+                        stg_stream_v2(odb + j, d[j], d[j + 1]);
                 }
                 if(gate && !last_silent)
                 {
@@ -531,7 +522,7 @@ __global__ void __launch_bounds__(team::kWarps * 32, 1) stft2048_team_kernel(con
                         atomic_max_float(p.out_peak + tt, gm);
                 }
             }
-            team::bar_sync(bar_id, W * 32); // every slice has consumed the round's magnitudes
+            bar_sync(bar_id, W * 32); // every slice has consumed the round's magnitudes
         }
 
         // ---- state back to the engine; m_decibels mirror (left implicit when it equals dbfs(state)); flags ----

@@ -16,7 +16,7 @@
 #pragma once
 #include <type_traits>
 
-#include "wf_fast2048.cuh"
+#include "wf_kernels.cuh"
 
 namespace wf {
 
@@ -61,7 +61,6 @@ struct Geo {
 template<int L, int P, bool EXTRA, bool DISP, typename TS>
 __global__ void __launch_bounds__(warp2::Geo<L, P>::kWarps * 32, 1) stft_warp2_kernel(const __grid_constant__ KParams p)
 {
-    using namespace fast;
     using G = warp2::Geo<L, P>;
     using PS = Pcm<TS>;
     constexpr int M = G::M, N = G::N, R = G::R, PP = G::PP, Q = G::Q, B = M;
@@ -108,11 +107,11 @@ __global__ void __launch_bounds__(warp2::Geo<L, P>::kWarps * 32, 1) stft_warp2_k
     {
         mbar_init(mbar, 1);
         *seg_done = 0;
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        fence_mbarrier_init();
     }
     __syncthreads();
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    asm volatile("griddepcontrol.wait;" ::: "memory");
+    pdl_launch_dependents();
+    pdl_wait();
 
     const int S = p.n_streams, T = p.n_frames;
     const int GR = gridDim.x;
@@ -269,7 +268,7 @@ __global__ void __launch_bounds__(warp2::Geo<L, P>::kWarps * 32, 1) stft_warp2_k
                 v[n1] = buf64[n1 * PP + lb];
             __syncwarp(); // all generic-proxy accesses to buf are done: it can take the next frame
             if(t + 1 == t1 && s_next >= 0 && t0_next == 0)
-                asm volatile("prefetch.global.L2 [%0];" ::"l"(p.state + (size_t)s_next * B + (lane * 32) % B));
+                prefetch_l2_line(p.state + (size_t)s_next * B + (lane * 32) % B);
             if(lane == 0)
             {
                 const TS *next = nullptr;
@@ -344,7 +343,7 @@ __global__ void __launch_bounds__(warp2::Geo<L, P>::kWarps * 32, 1) stft_warp2_k
                         const float ph = 4.0f * (pk::re(sq) + pk::im(sq));
                         p2 = (lb == 0) ? ph : p2;
                     }
-                    pk::c64 m = pk::make(sqrt_approx(p1), sqrt_approx(p2));
+                    pk::c64 m = pk::make(sqrt_approx_ftz(p1), sqrt_approx_ftz(p2));
                     const int k2c = (k2 >= 0) ? k2 : 0;
                     if(EXTRA && p.slope != nullptr)
                         m = pk::mul(m, pk::make(__ldg(p.slope + k1), __ldg(p.slope + k2c)));
